@@ -2,7 +2,7 @@
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload lres|sres] [--impl ours|reference]
 
-A "step" replays, through this repository's public ops (torch_utils.ops.* -> C ABI -> sm_100a
+A "step" replays, through this repository's public ops (torch_utils.ops.* -> C ABI -> sm_90a
 kernels), every hot-path operator call that one LongVideoGAN training step issues, at the real
 shapes: the call trace was recorded from the unmodified reference networks
 (tools/trace_reference_workload.py -> workloads/*.json) and is replayed as
@@ -22,6 +22,15 @@ in HBM; `e2e` = the same with the step's real-video batch copied from pinned hos
 the result read back inside the timed region; `roofline` = achieved algorithmic HBM GB/s of the
 dominant kernel (bias_act), timed with CUDA events inside the timed steps; `cpu_baseline` = the
 CPU oracle (oracle/, a port of the reference's _ref path) on a bounded sample, reported only.
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step computed, flattened, as DIR/<name>.npy in
+float32: for every replayed call of the generator (G) and discriminator (D) a fixed sample of 8192 elements of its
+output and of the input / bias / weight gradients its backward pass produced (`G012_conv3d_y`, `..._dx`, `..._db`,
+`..._dw`; the last pass of the step that ran the call), and the updated flat parameters of both networks (`g_params`,
+`g_ema`, `d_params`; 2^20-element samples). Sample indices are drawn from fixed seeds (np.unique over
+np.random.default_rng(seed).integers), and so are all inputs, so two builds run with the same arguments can be compared
+output for output. With the option, every call also copies its samples into persistent buffers (small gather kernels
+inside the captured step).
 """
 import argparse
 import json
@@ -40,7 +49,9 @@ import torch  # noqa: E402
 WORKLOADS = {
     # name: (trace file, G pass, D pass, per-GPU batch, frames per sample)
     'lres': ('lres_step.json', 'lres_G', 'lres_D', 8, 128),
-    'sres': ('sres_step.json', 'sres_G', 'sres_D', 16, 8),
+    # super-res per-GPU batch 8: at 16 (the reference's training batch) the step alone runs out of an 80 GB H100; at 8 it
+    # peaks at 38.3 GiB allocated (H100 80GB HBM3, torch.cuda.max_memory_allocated)
+    'sres': ('sres_step.json', 'sres_G', 'sres_D', 8, 8),
 }
 GRAD_ELEMS = {'lres': (83_200_000, 46_400_000), 'sres': (27_200_000, 24_000_000)}   # G, D parameter counts (SURVEY.md 2b)
 HOT_OPS = ('bias_act', 'upfirdn2d', 'filtered_lrelu', 'conv2d_resample', 'conv2d')
@@ -79,23 +90,28 @@ def scaled(shape, batch):
 # our arm: replay through torch_utils.ops on the GPU
 
 def run_backward(y, leaves, dy):
-    """Backward of ONE replayed call. A training step calls loss.backward() once; replaying the calls one by one
-    would pay torch.autograd.grad's Python-side argument validation (~50 us) per call, which is harness overhead,
-    not operator cost -- so the autograd engine is entered directly (what torch.autograd.grad does after validating)."""
+    """Backward of ONE replayed call -> the gradients of `leaves`. A training step calls loss.backward() once; replaying
+    the calls one by one would pay torch.autograd.grad's Python-side argument validation (~50 us) per call, which is
+    harness overhead, not operator cost -- so the autograd engine is entered directly (what torch.autograd.grad does
+    after validating)."""
     try:
-        torch.autograd.variable.Variable._execution_engine.run_backward(
+        return torch.autograd.variable.Variable._execution_engine.run_backward(
             (y,), (dy,), False, False, tuple(leaves), allow_unreachable=True, accumulate_grad=False)
     except (AttributeError, TypeError):
-        torch.autograd.grad(y, leaves, dy, allow_unused=True)
+        return torch.autograd.grad(y, leaves, dy, allow_unused=True)
+
+
+DUMP_SAMPLE = 8192      # elements kept per output / gradient of a replayed call with --dump-outputs
 
 
 class Replay:
-    def __init__(self, calls, batch, device, dtype_policy, ops=None):
+    def __init__(self, calls, batch, device, dtype_policy, ops=None, keep=False):
         if ops is None:
             from torch_utils.ops import bias_act, upfirdn2d, filtered_lrelu, conv2d_resample, conv2d_gradfix, conv_nd
             ops = dict(bias_act=bias_act, upfirdn2d=upfirdn2d, filtered_lrelu=filtered_lrelu, conv2d_resample=conv2d_resample,
                        conv2d=conv2d_gradfix, conv3d=conv_nd.conv3d, conv1d=conv_nd.conv1d)
         self.ops = ops
+        self.keep = keep        # --dump-outputs: every call copies a fixed sample of its output and gradients into it['kept']
         self.last_y = None
         self.device = device
         self.pool = {}
@@ -144,6 +160,19 @@ class Replay:
                 it['bytes_bwd'] = it['bytes_fwd'] + (y.numel() // 4 if coded else (y.numel() * y.element_size() if it['c']['op'] == 'bias_act' else 0))
                 del y
 
+    def _keep(self, it, key, t):
+        """Copies the fixed sample (DUMP_SAMPLE flat indices drawn from a seed per call and key) of `t` into it['kept'][key]."""
+        if not self.keep or t is None:
+            return
+        flat = t.detach().reshape(-1)
+        kept = it.setdefault('kept', {})
+        if key not in kept:
+            seed = next(i for i, o in enumerate(self.items) if o is it) * 4 + ('y', 'dx', 'db', 'dw').index(key)
+            idx = np.unique(np.random.default_rng(seed).integers(0, flat.numel(), size=min(flat.numel(), DUMP_SAMPLE)))
+            kept[key] = (torch.from_numpy(idx).to(flat.device), torch.empty(len(idx), dtype=torch.float32, device=flat.device))
+        idx, buf = kept[key]
+        buf.copy_(flat[idx])
+
     def _buf(self, kind, shape, dt):
         key = (kind, tuple(shape), dt)
         if key not in self.pool:
@@ -172,39 +201,46 @@ class Replay:
         with torch.no_grad():
             for it in self.items:
                 self.last_y = self._fwd(it, it['x'])
+                self._keep(it, 'y', self.last_y)
 
     def forward_backward(self, timer=None, lo=0, hi=None):
         for it in self.items[lo:hi]:
             if it.get('nograd'):
                 with torch.no_grad():
                     self.last_y = self._fwd(it, it['x'])
+                self._keep(it, 'y', self.last_y)
                 continue
             x = it['x'].detach().requires_grad_(True)
-            leaves = [x]
+            leaves, names = [x], ['dx']
             b = it.get('b')
             if b is not None:
                 b = b.detach().requires_grad_(True)
                 leaves.append(b)
+                names.append('db')
             saved_b = it.get('b')
             it['b'] = b
             saved_w = it.get('w')
             if saved_w is not None:
                 it['w'] = saved_w.detach().requires_grad_(True)
                 leaves.append(it['w'])
+                names.append('dw')
             if timer is not None and it['c']['op'] in timer.ops:
                 flops = it.get('flops_fwd')
                 timer.start()
                 y = self._fwd(it, x)
                 timer.stop(it['bytes_fwd_grad'] if flops is None else flops)
+                grads = ()
                 if y.requires_grad:
                     timer.start()
-                    run_backward(y, leaves, it['dy'])
+                    grads = run_backward(y, leaves, it['dy'])
                     timer.stop(it['bytes_bwd'] if flops is None else 2.0 * flops)
             else:
                 y = self._fwd(it, x)
-                if y.requires_grad:
-                    run_backward(y, leaves, it['dy'])
+                grads = run_backward(y, leaves, it['dy']) if y.requires_grad else ()
             self.last_y = y.detach()
+            self._keep(it, 'y', self.last_y)
+            for key, gr in zip(names, grads):
+                self._keep(it, key, gr)
             it['b'] = saved_b
             if saved_w is not None:
                 it['w'] = saved_w
@@ -287,7 +323,20 @@ def measured_peak(kind='hbm'):
             return mp['hbm_gbs'], 'measured (MEASURED_PEAKS.json hbm_gbs)'
         return mp['bf16_tflops_sustained'], 'measured (MEASURED_PEAKS.json bf16_tflops_sustained: the kernel is timed inside a long step)'
     except Exception:
-        return (6650.0, 'fallback (B200_PROFILING.md 6.65 TB/s)') if kind == 'hbm' else (1400.0, 'fallback (B200_PROFILING.md ~1.4 PFLOP/s sustained)')
+        return (3350.0, 'H100 SXM data sheet (3.35 TB/s HBM3; not a measured figure)') if kind == 'hbm' else \
+            (989.0, 'H100 SXM data sheet (989 TFLOP/s dense BF16; not a measured figure)')
+
+
+def dump_outputs(out_dir, arrays, limit=1 << 20):
+    """`arrays` (name -> tensor) -> out_dir/<name>.npy as float32, flattened; more than `limit` elements: a fixed,
+    seeded sample of them (at most 4 MB per array)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        flat = t.detach().reshape(-1)
+        if flat.numel() > limit:
+            idx = np.unique(np.random.default_rng(0).integers(0, flat.numel(), size=limit))
+            flat = flat[torch.from_numpy(idx).to(flat.device)]
+        np.save(os.path.join(out_dir, name + '.npy'), flat.float().cpu().numpy())
 
 
 def metric_name(scope):
@@ -584,16 +633,17 @@ class GradExchange:
 
 # ---------------------------------------------------------------------------------------------
 
-def run_ours(args, workload, scope, steps, rank, world, local_rank, device, with_cpu, with_refcuda):
-    """One workload through this repository's ops on the GPU -> the JSON fields of its line."""
+def run_ours(args, workload, scope, steps, rank, world, local_rank, device, with_cpu, with_refcuda, dump_dir=None):
+    """One workload through this repository's ops on the GPU -> the JSON fields of its line. `dump_dir`: see --dump-outputs."""
     global _scope
     import torch.distributed as dist
     from torch_utils import custom_ops
     _scope = scope
+    torch.manual_seed(1234 + rank)          # every input and weight of the replay: the same from run to run
     g_calls, d_calls, batch, frames = load_trace(workload)
     policy = 'mixed' if workload == 'sres' else 'fp32'
-    G = Replay(g_calls, batch, device, policy)
-    D = Replay(d_calls, batch, device, policy)
+    G = Replay(g_calls, batch, device, policy, keep=bool(dump_dir))
+    D = Replay(d_calls, batch, device, policy, keep=bool(dump_dir))
     kBuckets = 4
     ex_g = ex_d = None
     if world > 1:
@@ -727,6 +777,14 @@ def run_ours(args, workload, scope, steps, rank, world, local_rank, device, with
     timer = KernelTimer(dominant_op)
     ms_total = timed(steps, e2e=False, timer=None if graphs else timer)
     launches = launches_per_step * steps if graphs else custom_ops.launch_count() - launches0
+    if dump_dir and rank == 0:
+        tg, td = (tail_g, tail_d) if world == 1 else (ex_g.tail, ex_d.tail)
+        arrays = {'g_params': tg.opt.flat_params, 'g_ema': tg.ema_flat, 'd_params': td.opt.flat_params}
+        for net, R in (('G', G), ('D', D)):
+            for i, it in enumerate(R.items):
+                for key, (_, buf) in it.get('kept', {}).items():
+                    arrays[f'{net}{i:03d}_{it["c"]["op"]}_{key}'] = buf
+        dump_outputs(dump_dir, arrays)
     step(e2e=True)                           # untimed warm-up of the host-copy flavour
     ms_e2e = timed(steps, e2e=True)
     ms_e2e_eager = timed(steps, e2e=True, eager=True) if graphs else ms_e2e
@@ -785,13 +843,13 @@ def run_ours(args, workload, scope, steps, rank, world, local_rank, device, with
                'roofline': {'bound': 'tensor' if tensor_bound else 'hbm',
                             'kernel': {'bias_act': 'bias_act (vector kernel: forward writing 2-bit sign/clamp codes + backward from the codes with fused dx/db)',
                                        'filtered_lrelu': 'filtered_lrelu (fused up-FIR / lrelu / down-FIR; FP32-issue-bound, its HBM figure is shown for reference)',
-                                       'conv3d': 'conv_igemm_kernel / conv_wgrad_v2_kernel (TMA-fed tcgen05 implicit GEMM; fp32 layers as bf16 hi/lo split: 3 tensor-core '
+                                       'conv3d': 'conv_igemm_kernel / conv_wgrad_v2_kernel (TMA-fed wgmma implicit GEMM; fp32 layers as bf16 hi/lo split: 3 tensor-core '
                                                  'products per algorithmic product, so the tensor pipe executes 3x the achieved figure) incl. its operand re-tiling passes'}[dominant_op],
                             'achieved': achieved,
                             'peak': peak, 'peak_source': peak_src, 'unit': 'TFLOP/s' if tensor_bound else 'GB/s', 'frac': achieved / peak if peak else None,
                             'launches_timed': k_n, 'share_of_step': k_share, 'traffic': traffic, 'traffic_note': traffic_note, 'timing': k_how},
                'clocks': clocks}
-    # the same trace through the REFERENCE'S OWN CUDA ops on this GPU (oracle/_ref: its plugins built unmodified for sm_100a,
+    # the same trace through the REFERENCE'S OWN CUDA ops on this GPU (oracle/_ref: its plugins built unmodified for sm_90a,
     # its Python wrappers, cuDNN for its convolutions) -- eager on both sides, N = 1 only: the "beat-this" baseline
     if rank == 0 and world == 1 and with_refcuda:
         try:
@@ -807,7 +865,7 @@ def run_ours(args, workload, scope, steps, rank, world, local_rank, device, with
                 def rstep():
                     RG.forward_backward(); RD.forward_backward()
                     RG.forward_only(); RD.forward_backward(); RD.forward_backward()
-                # one warm-up step, timed: a slow reference step (the super-res trace takes ~11 s on B200) gets 2 timed steps
+                # one warm-up step, timed: a slow reference step (seconds for the super-res trace) gets 2 timed steps
                 # without a second warm-up, a fast one a second warm-up and up to 5 -- the default run must end within minutes
                 w0, w1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 w0.record()
@@ -829,7 +887,7 @@ def run_ours(args, workload, scope, steps, rank, world, local_rank, device, with
                 rms = t0.elapsed_time(t1) / nref
                 res['ref_cuda'] = {'value': batch * frames / (rms / 1000.0), 'unit': 'frames/s', 'ms_per_step': rms, 'steps': nref,
                                    'launch': 'eager', 'ours_eager_ms_per_step': ms_e2e_eager / steps,
-                                   'what': "the same op trace through the reference's own CUDA plugins (built unmodified for sm_100a, "
+                                   'what': "the same op trace through the reference's own CUDA plugins (built unmodified for sm_90a, "
                                            "oracle/_ref) and Python wrappers on this GPU; compare with ours_eager_ms_per_step (eager, incl. the e2e copies)"}
                 del RG, RD
                 torch.cuda.empty_cache()
@@ -854,9 +912,11 @@ def main():
     ap.add_argument('--impl', default='ours', choices=['ours', 'reference'])
     ap.add_argument('--cpu-budget', type=float, default=4.0,
                     help='seconds of CPU sampling before every (network, op) group has been visited once (the whole sample takes ~30 s at 4: '
-                         'every group is measured at least once; 12 gave 125 s on the 128-thread host of the B200 box)')
+                         'every group is measured at least once; 12 took about two minutes on a 128-thread host)')
     ap.add_argument('--no-cpu', action='store_true')
     ap.add_argument('--no-ref-cuda', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what the last timed step computed to DIR/<name>.npy (see the module docstring)')
     ap.add_argument('--launch', default='graph', choices=['graph', 'eager'],
                     help='graph: the step is captured once into CUDA graphs and replayed (default); eager: every call launched from Python')
     args = ap.parse_args()
@@ -909,7 +969,8 @@ def main():
     from torch_utils import custom_ops
     custom_ops.load_library()
 
-    res = run_ours(args, primary, args.scope, args.steps, rank, world, local_rank, device, with_cpu=not args.no_cpu, with_refcuda=not args.no_ref_cuda)
+    res = run_ours(args, primary, args.scope, args.steps, rank, world, local_rank, device, with_cpu=not args.no_cpu, with_refcuda=not args.no_ref_cuda,
+                   dump_dir=args.dump_outputs)
     sres = ops_only = None
     if args.workload == 'both':
         torch.cuda.empty_cache()

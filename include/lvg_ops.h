@@ -1,5 +1,5 @@
 /*
- * lvg_ops.h -- C ABI of liblvg_ops.so, the sm_100a operator library behind the
+ * lvg_ops.h -- C ABI of liblvg_ops.so, the sm_90a operator library behind the
  * torch_utils.ops drop-in (bias_act, upfirdn2d, filtered_lrelu, conv2d, fma).
  *
  * Conventions
@@ -53,7 +53,7 @@ extern "C" {
 
 int         lvg_abi_version(void);
 const char* lvg_last_error(void);
-/* compile-time facts about the build: "sm_100a;..." */
+/* compile-time facts about the build: "sm_90a;..." */
 const char* lvg_build_info(void);
 /* number of kernels this library has launched in the calling process so far */
 int64_t     lvg_launch_count(void);
@@ -180,14 +180,14 @@ int lvg_fma(const void* a, const void* b, const void* c, void* out, int dtype,
 
 /*
  * Grouped 2-D convolution (cross-correlation, like torch.nn.functional.conv2d)
- * on tcgen05 tensor cores -- the kernel behind conv2d_gradfix.conv2d
+ * on the implicit-GEMM engine below (its T = kt = 1 case) -- the entry behind conv2d_gradfix.conv2d
  * (torch_utils/ops/conv2d_gradfix.py:37-40) for the per-sample-weight
  * "modulated" convolutions (model/generator_sres.py:63-65) and the
  * discriminator convolutions (conv2d_resample.py:29-41).
  *   x [N][G*Cin][H][W]  w [G*Cout][Cin][kh][kw]  y [N][G*Cout][Ho][Wo]
- * NCHW-contiguous fp16 operands, fp32 accumulation in tensor memory, stride 1, 3x3 or 1x1,
+ * NCHW-contiguous fp16 operands, fp32 accumulation, stride 1, 3x3 or 1x1,
  * any batch n (samples share the weights of their group). `workspace` holds the
- * re-tiled weights (lvg_conv2d_fprop_workspace bytes, 16-byte aligned).
+ * re-tiled operands (lvg_conv2d_fprop_workspace bytes, 16-byte aligned).
  * Returns LVG_UNSUPPORTED outside the covered envelope.
  */
 int lvg_conv2d_fprop(const void* x, const void* w, void* y, int dtype,
@@ -198,8 +198,7 @@ int64_t lvg_conv2d_fprop_workspace(int dtype, int n, int groups, int cin, int co
                                    int h, int wd, int kh, int kw, int stride,
                                    int pad_h, int pad_w);
 /*
- * Gradient of the convolution above with respect to its input (same kernel, the weights
- * repacked channel-transposed and spatially mirrored, padding k-1-pad): dx [N][G*Cin][H][W] from
+ * Gradient of the convolution above with respect to its input (lvg_convnd_dgrad): dx [N][G*Cin][H][W] from
  * dy [N][G*Cout][Ho][Wo]. The argument list describes the FORWARD convolution. Same workspace.
  */
 int lvg_conv2d_dgrad(const void* dy, const void* w, void* dx, int dtype,
@@ -210,14 +209,15 @@ int lvg_conv2d_dgrad(const void* dy, const void* w, void* dx, int dtype,
  * Gradient of the same convolution with respect to its weights: dw [G*Cout][Cin][kh][kw] (fp16, summed
  * over the N samples) from x [N][G*Cin][H][W] and dy [N][G*Cout][Ho][Wo]. Replaces the weight-gradient
  * leg of conv2d_gradfix (conv2d_gradfix.py:119-141 -> aten::convolution_backward / cuDNN). The argument
- * list describes the FORWARD convolution. No workspace. Returns -1 outside fp16 / stride 1 / 3x3, 1x1.
+ * list describes the FORWARD convolution. No workspace argument: lvg_convnd_wgrad runs on a stream-ordered
+ * allocation (cudaMallocAsync). Returns -1 outside fp16 / stride 1 / 3x3, 1x1.
  */
 int lvg_conv2d_wgrad(const void* x, const void* dy, void* dw, int dtype,
                      int n, int groups, int cin, int cout, int h, int wd,
                      int kh, int kw, int stride, int pad_h, int pad_w, void* stream);
 
 /*
- * Grouped 1-D / 2-D / 3-D convolution (cross-correlation) on tcgen05 tensor cores, TMA-fed (csrc/conv_igemm.cu): one
+ * Grouped 1-D / 2-D / 3-D convolution (cross-correlation) on Hopper tensor cores (wgmma), TMA-fed (csrc/conv_igemm.cu): one
  * engine for conv2d_gradfix.conv2d / conv_transpose2d (conv2d_gradfix.py:37-45), the F.conv3d calls of the low-res
  * networks (generator_lres.py:119,578; discriminator_lres.py:172) and the F.conv1d calls of the low-res discriminator
  * (discriminator_lres.py:108-127).
@@ -250,7 +250,7 @@ int lvg_convnd_wgrad(const void* x, const void* dy, void* dw, int dtype, int n, 
 /*
  * Introspection: the tiling lvg_convnd_fprop (mode 0) / lvg_convnd_dgrad (mode 1) launches with, as 48 ints -- wgroups, cout
  * (rows of the GEMM), mt, kc, nblk, nimg, lo_blk, to, ho, wo, kt, kh, kw, pad_t, pad_h, pad_w, tt, th, wt, wtb, thb, frame_px,
- * ncols, n0, epi_warps, nbuf, tiles_x, tiles_y, tiles_t, total_tiles, ks, stages, a_resident, a_stage, b_step, b_bytes, b_box,
+ * ncols, tiles_x, tiles_y, tiles_t, total_tiles, ks, stages, a_resident, a_stage, b_step, b_bytes, b_box,
  * stage_bytes, ostride, hos, wos, 0..., [47] = 1 when the call takes the streaming 1x1x1 kernels instead -- host arithmetic only
  * (no device needed): tests/test_igemm_emul.py replays the kernel's addressing with it on the CPU. The argument list describes
  * the FORWARD convolution in both modes.

@@ -6,7 +6,7 @@
 // swish), grad=2 is the second derivative; clamping saturates in the forward
 // and zeroes gradients where the forward output was saturated.
 //
-// B200 design: a pure streaming op (1 read + 1 write forward, 2 reads + 1 write
+// Design: a pure streaming op (1 read + 1 write forward, 2 reads + 1 write
 // backward), so the kernel is organised around bytes in flight: 128-bit
 // loads/stores, four independent packs per thread issued before any use
 // (64 KB in flight per SM at 4 CTAs/SM), grid sized in whole waves of the SM
@@ -188,11 +188,9 @@ __global__ void __launch_bounds__(kThreads, (G == 2 ? 2 : 4)) bias_act_vec_kerne
     T* __restrict__ py = (T*)p.y;
 
     // Fused bias gradient (FUSE_DB): the tiles are walked in RUNS of p.run_tiles (8) consecutive tiles (128 KB of each operand; two
-    // resident waves of CTAs measured best: 0.93 of the copy rate, one wave 0.81-0.89, runs of 4 tiles 0.7-0.8),
-    // runs interleaved over the CTAs like single tiles are in the forward pass -- concurrently resident CTAs stream
-    // one contiguous window of memory, which HBM rewards (a fully contiguous per-CTA range measured 0.75 of the copy
-    // rate, single interleaved tiles with one atomic per warp and tile 0.5: ~100 consecutive tiles share a bias row
-    // and their atomics serialise on one address). Inside a run a warp stays inside one channel ("row" = run of
+    // resident waves of CTAs), runs interleaved over the CTAs like single tiles are in the forward pass -- concurrently resident CTAs stream
+    // one contiguous window of memory, which HBM rewards (single interleaved tiles with one atomic per warp and tile
+    // serialise: ~100 consecutive tiles share a bias row and their atomics hit one address). Inside a run a warp stays inside one channel ("row" = run of
     // step_b elements sharing a bias index) for many packs: each lane keeps a running sum for the warp's current
     // row; only when the row changes or the run ends the warp reduces by shuffle and issues ONE global atomic.
     // No shared memory, no block barriers in the streaming loop.

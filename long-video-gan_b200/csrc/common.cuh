@@ -1,4 +1,4 @@
-// Shared helpers for the liblvg_ops kernels (sm_100a only).
+// Shared helpers for the liblvg_ops kernels (sm_90a only).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -53,7 +53,7 @@ inline int num_sms() {
     if (cached[dev] == 0) {
         int v = 0;
         cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-        cached[dev] = v > 0 ? v : 148;
+        cached[dev] = v > 0 ? v : 132;
     }
     return cached[dev];
 }

@@ -1,359 +1,14 @@
-// Grouped 2-D convolution (cross-correlation) as an implicit GEMM on the 5th-generation tensor
-// cores: tcgen05.mma with fp16 operands from shared memory and fp32 accumulators in tensor memory.
-//
-// This is the kernel behind conv2d_gradfix.conv2d (torch_utils/ops/conv2d_gradfix.py:37-40) for the
-// per-sample-weight "modulated" convolutions of the super-res generator
-// (model/generator_sres.py:63-65: x [1, G*Cin, H, W], w [G*Cout, Cin, 3, 3], padding 2, groups G = N*T)
-// and for the stride-1 discriminator convolutions. The reference hands these to cuDNN.
-//
-// GEMM view, per group g:   D[co][pix] = sum_tap sum_ci  W_tap[co][ci] * X[ci][pix + tap]
-//   M = Cout (tiles of 128 = one UMMA M), N = a TH x WT patch of output pixels (<= 256 columns of
-//   TMEM), K = Cin in chunks of 16 (one UMMA K step) times the kh*kw taps, all accumulated into the
-//   same TMEM tile.
-//
-// Operand staging (no swizzle, "interleaved" canonical layouts of the UMMA shared-memory descriptor):
-//   A  weights, K-major.  A pre-pass (conv_pack_weights_kernel) rewrites the [Cout][Cin][kh*kw]
-//      weights once per call into ready-made 128 x 16 tile images, one per (m-tile, k-chunk, tap),
-//      so the main kernel stages A with plain 16-byte copies. The fp16 NCHW activations cannot be
-//      addressed by tiled TMA (row pitches of the sres layers are 4 mod 8 elements, not multiples of
-//      16 bytes), hence software staging for both operands.
-//   B  activations, MN-major (pixels contiguous, exactly as they sit in NCHW memory). The tile is
-//      staged as [kw x-shifted copies][16 channels][(TH + kh - 1) rows x WT pixels]; a tap (ky, kx)
-//      is then just a different descriptor start address: copy kx, advanced by ky rows. A shift by
-//      one pixel cannot be expressed in a descriptor (16-byte granularity), a shift by one row can.
-//
-// One CTA = one (pixel tile, 128-channel m-tile, group). Per k-chunk: all threads stage A and B,
-// fence to the async proxy, one thread issues kh*kw MMAs and commits them to an mbarrier that gates
-// the next staging round. Two CTAs are resident per SM (<= 72 KB shared memory, 256 TMEM columns
-// each), so one CTA's staging overlaps the other's MMAs. Epilogue: tcgen05.ld -> fp16 -> global.
+// Grouped 2-D convolution entry points (fp16, stride 1, 3x3 or 1x1) of the conv2d plugin, run on the implicit-GEMM engine
+// of conv_igemm.cu: a 2-D convolution is its T = kt = 1 case, with the same NCHW / [G*Cout][Cin][kh][kw] memory layout.
 
 #include "common.cuh"
-#include "tcgen05.cuh"
 
 namespace lvg {
 namespace {
 
-constexpr int kThreads = 256;
-constexpr int kBM = 128;          // UMMA M
-constexpr int kBK = 16;           // channels per k-chunk (= UMMA K for fp16)
-constexpr int kATileBytes = kBM * kBK * 2;   // 4096
-
-struct ConvParams {
-    const __half* x;
-    const __half* wp;        // packed weights
-    __half* y;
-    int groups;              // instances = N * G (grid.z)
-    int wgroups;             // weight groups G: instance i uses the weights of group i % G
-    int cin, cout;           // per group
-    int h, w, ho, wo;
-    int kh, kw, pad_h, pad_w;
-    int th, wt;              // output tile: th rows x wt pixels (wt % 8 == 0, th * wt % 16 == 0, <= 256)
-    int tiles_x, tiles_y;
-    int kc, mt;              // k-chunks, m-tiles
-    int pair_ok;             // x is 4-byte aligned and rows have even length: pixel pairs can be loaded as one word
-};
-
-using namespace tc;
-
-// ------------------------------------------------------------------------------------------------
-// weights -> tile images.  Element (m, k, tap) of the logical A matrix of group g sits at
-//   w[g * gstride + m * sm + k * sk + (flip ? taps-1-tap : tap)]
-// fprop: m = co, k = ci (sm = cin*taps, sk = taps); dgrad: m = ci, k = co (sm = taps, sk = cin*taps), flipped taps.
-// Image of one 128 x 16 tile (K-major, no swizzle): byte offset(m, k) = (k/8)*2048 + (m/8)*128 + (m%8)*16 + (k%8)*2.
-__global__ void __launch_bounds__(256) conv_pack_weights_kernel(const __half* __restrict__ w, __half* __restrict__ wp, int groups,
-                                                                 int m_total, int k_total, int taps, int64_t gstride,
-                                                                 int64_t sm, int64_t sk, int flip, int mt, int kc)
-{
-    // one thread = one 16-byte row of a core matrix (8 consecutive k of one m, one tap)
-    const int64_t total = (int64_t)groups * mt * kc * taps * (kATileBytes / 16);
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-        // decode with tap fastest so that neighbouring threads read neighbouring weights
-        int64_t r = i;
-        const int tap = (int)(r % taps); r /= taps;
-        const int k8 = (int)(r % 2); r /= 2;
-        const int mrow = (int)(r % kBM); r /= kBM;
-        const int kci = (int)(r % kc); r /= kc;
-        const int mti = (int)(r % mt);
-        const int g = (int)(r / mt);
-        const int m = mti * kBM + mrow;
-        const int k0 = kci * kBK + k8 * 8;
-        const int wtap = flip ? taps - 1 - tap : tap;
-        alignas(16) __half v[8];
-#pragma unroll
-        for (int j = 0; j < 8; j++) {
-            const int k = k0 + j;
-            v[j] = (m < m_total && k < k_total) ? w[(int64_t)g * gstride + (int64_t)m * sm + (int64_t)k * sk + wtap] : __float2half(0.f);
-        }
-        const int64_t tile = (((int64_t)g * mt + mti) * kc + kci) * taps + tap;
-        char* dst = reinterpret_cast<char*>(wp) + tile * kATileBytes + k8 * 2048 + (mrow / 8) * 128 + (mrow % 8) * 16;
-        *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(v);
-    }
-}
-
-// ------------------------------------------------------------------------------------------------
-
-template <int KH, int KW>
-__global__ void __launch_bounds__(kThreads, 2) conv_fprop_tc_kernel(ConvParams p)
-{
-    constexpr int TAPS = KH * KW;
-    extern __shared__ __align__(128) unsigned char smem[];
-    __shared__ uint64_t mma_bar;      // the MMAs of a k-chunk have finished reading shared memory
-    __shared__ uint64_t a_bar[2];     // the bulk copy of a chunk's weight tiles has landed (one per A buffer)
-    __shared__ uint32_t tmem_base_slot;
-
-    const int nch_row = p.wt / 8;                          // 16-byte chunks per tile row
-    const int nch = (p.th + KH - 1) * nch_row;             // chunks per (copy, k-group)
-    unsigned char* sA = smem;                              // [2 buffers][TAPS][4096]
-    unsigned char* sB = smem + 2 * TAPS * kATileBytes;     // [KW copies][2 k-groups][nch][128]
-    const uint32_t lbo_b = (uint32_t)nch * 128;            // between the two 8-channel groups
-    const int N = p.th * p.wt;
-
-    const int tile = blockIdx.x;
-    const int ty = tile / p.tiles_x, tx = tile - ty * p.tiles_x;
-    const int mti = blockIdx.y;
-    const int g = blockIdx.z;
-    const int oy0 = ty * p.th, ox0 = tx * p.wt;
-    const int iy0 = oy0 - p.pad_h, ix0 = ox0 - p.pad_w;
-    const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
-
-    if (threadIdx.x == 0) {
-        mbar_init(&mma_bar, 1);
-        mbar_init(&a_bar[0], 1);
-        mbar_init(&a_bar[1], 1);
-        fence_barrier_init();
-    }
-    if (warp == 0) tmem_alloc(&tmem_base_slot, 256);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_d = tmem_base_slot;
-
-    // instruction descriptor: D = f32, A = B = f16, A K-major, B MN-major, N >> 3, M >> 4
-    const uint32_t idesc = (1u << 4) | (1u << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(kBM >> 4) << 24);
-
-    const __half* xg = p.x + (int64_t)g * p.cin * p.h * p.w;
-    const unsigned char* wpg = reinterpret_cast<const unsigned char*>(p.wp) + (((int64_t)(g % p.wgroups) * p.mt + mti) * p.kc) * TAPS * kATileBytes;
-
-    // B staging item = (channel, tile row, 8-pixel chunk): 8 + KW - 1 pixels are fetched as pixel pairs into
-    // registers (prefetch), later written to shared memory as KW shifted 16-byte chunks (commit).
-    // Item order: channel-within-8 fastest, then chunk, so 8 consecutive lanes fill one 128-byte core matrix and
-    // a warp's 16-byte stores cover 512 contiguous bytes. The decomposition of an item does not depend on the
-    // k-chunk, so it is done ONCE here (global offset, shared-memory offset, validity mask of the pixel pairs).
-    constexpr int NPAIR = (8 + KW - 1 + 1) / 2;
-    constexpr int kMaxItems = 4;                           // per thread; host guarantees items <= 4 * kThreads
-    const int rows = p.th + KH - 1;
-    const int items = kBK * rows * nch_row;
-    const bool paired = p.pair_ok && (ix0 & 1) == 0;       // rows and tile start are 4-byte aligned: one load per pair
-    int it_goff[kMaxItems];      // element offset of the item's first pixel inside one k-chunk of x (may point before the row)
-    int it_soff[kMaxItems];      // byte offset of the item's 16-byte slot inside copy 0 of the B buffer
-    int it_ch[kMaxItems];        // channel within the chunk (for the cin bound)
-    unsigned it_mask[kMaxItems]; // bit 2q / 2q+1: pixel 2q / 2q+1 of the item is inside the image
-#pragma unroll
-    for (int s = 0; s < kMaxItems; s++) {
-        const int it = threadIdx.x + s * kThreads;
-        const int clo = it % 8;
-        const int c = (it / 8) % nch_row;
-        const int rr = (it / (8 * nch_row)) % rows;
-        const int ch = (it / (8 * nch_row * rows)) * 8 + clo;
-        const int gy = iy0 + rr;
-        const int gx0 = ix0 + c * 8;
-        unsigned mask = 0;
-        if (it < items && gy >= 0 && gy < p.h) {
-#pragma unroll
-            for (int i = 0; i < 2 * NPAIR; i++)
-                if (gx0 + i >= 0 && gx0 + i < p.w) mask |= 1u << i;
-        }
-        it_mask[s] = mask;
-        it_ch[s] = ch;
-        it_goff[s] = (ch * p.h + gy) * p.w + gx0;
-        it_soff[s] = ((ch / 8) * nch + rr * nch_row + c) * 128 + (ch % 8) * 16;
-    }
-    uint32_t pre[kMaxItems][NPAIR];
-
-    auto prefetch = [&](int kci) {
-        const __half* xc = xg + (int64_t)kci * kBK * p.h * p.w;
-        const int ch_left = p.cin - kci * kBK;             // channels of this chunk that exist
-#pragma unroll
-        for (int s = 0; s < kMaxItems; s++) {
-            const unsigned mask = it_ch[s] < ch_left ? it_mask[s] : 0u;
-            const __half* src = xc + it_goff[s];
-#pragma unroll
-            for (int q = 0; q < NPAIR; q++) {
-                const unsigned m2 = (mask >> (2 * q)) & 3u;
-                uint32_t v = 0;
-                if (paired) {
-                    if (m2 == 3u) v = __ldg(reinterpret_cast<const unsigned int*>(src + 2 * q));
-                } else {
-                    if (m2 & 1u) v = __ldg(reinterpret_cast<const unsigned short*>(src + 2 * q));
-                    if (m2 & 2u) v |= (uint32_t)__ldg(reinterpret_cast<const unsigned short*>(src + 2 * q + 1)) << 16;
-                }
-                pre[s][q] = v;
-            }
-        }
-    };
-    auto commit = [&]() {
-#pragma unroll
-        for (int s = 0; s < kMaxItems; s++) {
-            if (threadIdx.x + s * kThreads < items) {
-                unsigned char* dst0 = sB + it_soff[s];
-#pragma unroll
-                for (int v = 0; v < KW; v++) {
-                    uint4 o;
-                    if (v % 2 == 0) {
-                        o = make_uint4(pre[s][v / 2], pre[s][v / 2 + 1], pre[s][v / 2 + 2], pre[s][v / 2 + 3]);
-                    } else {        // odd shift: high half of pair j with low half of pair j + 1
-                        o = make_uint4(__byte_perm(pre[s][v / 2], pre[s][v / 2 + 1], 0x5432), __byte_perm(pre[s][v / 2 + 1], pre[s][v / 2 + 2], 0x5432),
-                                       __byte_perm(pre[s][v / 2 + 2], pre[s][v / 2 + 3], 0x5432), __byte_perm(pre[s][v / 2 + 3], pre[s][v / 2 + 4 < NPAIR ? v / 2 + 4 : NPAIR - 1], 0x5432));
-                    }
-                    *reinterpret_cast<uint4*>(dst0 + (size_t)(v * 2) * nch * 128) = o;
-                }
-            }
-        }
-    };
-
-    // Software pipeline over the k-chunks (A double-buffered through TMA, B through registers):
-    //   top of iteration k : MMAs of chunk k-1 are done -> B buffer free; write the prefetched chunk k to shared memory
-    //   one thread         : wait for A[k % 2], issue the TAPS MMAs of chunk k, commit, start the bulk copy of A[(k+1) % 2]
-    //   everyone           : prefetch chunk k+1 from global memory into registers while the tensor core works on chunk k
-    if (threadIdx.x == 0) {
-        mbar_expect_tx(&a_bar[0], TAPS * kATileBytes);
-        bulk_copy_g2s(sA, wpg, TAPS * kATileBytes, &a_bar[0]);
-    }
-    prefetch(0);
-    for (int kci = 0; kci < p.kc; kci++) {
-        if (kci > 0) mbar_wait(&mma_bar, (uint32_t)((kci - 1) & 1));
-        commit();
-        fence_proxy_async();
-        tc_fence_before();
-        __syncthreads();
-
-        if (threadIdx.x == 0) {
-            const int buf = kci & 1;
-            mbar_wait(&a_bar[buf], (uint32_t)((kci >> 1) & 1));
-            tc_fence_after();
-#pragma unroll
-            for (int tap = 0; tap < TAPS; tap++) {
-                const int ky = tap / KW, kx = tap % KW;
-                const uint64_t adesc = make_desc(smem_u32(sA + (size_t)buf * TAPS * kATileBytes + tap * kATileBytes), 2048, 128);
-                const uint64_t bdesc = make_desc(smem_u32(sB + ((size_t)(kx * 2) * nch + ky * nch_row) * 128), lbo_b, 128);
-                umma_f16(tmem_d, adesc, bdesc, idesc, (kci > 0 || tap > 0) ? 1u : 0u);
-            }
-            umma_commit(&mma_bar);
-            if (kci + 1 < p.kc) {      // A[(k+1) % 2] was last read by the MMAs of chunk k-1, which have completed
-                mbar_expect_tx(&a_bar[buf ^ 1], TAPS * kATileBytes);
-                bulk_copy_g2s(sA + (size_t)(buf ^ 1) * TAPS * kATileBytes, wpg + (int64_t)(kci + 1) * TAPS * kATileBytes, TAPS * kATileBytes, &a_bar[buf ^ 1]);
-            }
-        }
-        if (kci + 1 < p.kc) prefetch(kci + 1);
-    }
-
-    // ---- epilogue: TMEM -> registers -> fp16 -> global (half2 stores along the pixel axis)
-    mbar_wait(&mma_bar, (uint32_t)((p.kc - 1) & 1));
-    tc_fence_after();
-    {
-        const int q = warp % 4;                 // TMEM lane quadrant this warp may read
-        const int m = mti * kBM + q * 32 + lane;
-        __half* yrow = p.y + ((int64_t)g * p.cout + m) * p.ho * p.wo;
-        for (int n0 = (warp / 4) * 32; n0 < N; n0 += 64) {
-            uint32_t acc[32];
-            tmem_ld32(tmem_d + ((uint32_t)(q * 32) << 16) + (uint32_t)n0, acc);
-            if (m < p.cout) {
-#pragma unroll
-                for (int j = 0; j < 32; j += 2) {
-                    const int n = n0 + j;
-                    const int r = n / p.wt, c = n - r * p.wt;       // wt is even: the pair stays in one row
-                    const int oy = oy0 + r, ox = ox0 + c;
-                    if (n < N && oy < p.ho && ox < p.wo) {
-                        __half* dst = yrow + (int64_t)oy * p.wo + ox;
-                        const __half2 v = __floats2half2_rn(__uint_as_float(acc[j]), __uint_as_float(acc[j + 1]));
-                        if (ox + 1 < p.wo && ((reinterpret_cast<uintptr_t>(dst) & 3) == 0)) {
-                            *reinterpret_cast<__half2*>(dst) = v;
-                        } else {
-                            dst[0] = __low2half(v);
-                            if (ox + 1 < p.wo) dst[1] = __high2half(v);
-                        }
-                    }
-                }
-            }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem_d, 256);
-}
-
-// tile geometry for an output of ho x wo pixels
-void pick_tile(int ho, int wo, int& th, int& wt, int& tiles_x, int& tiles_y)
-{
-    tiles_x = (wo + 63) / 64;
-    wt = ((wo + tiles_x - 1) / tiles_x + 7) / 8 * 8;
-    th = (256 / wt) & ~1;
-    if (th < 2) th = 2;
-    if (th > ho + (ho & 1)) th = ho + (ho & 1);       // no taller than the (even-rounded) image
-    tiles_y = (ho + th - 1) / th;
-}
-
-size_t smem_bytes(int taps, int kh, int kw, int th, int wt)
-{
-    return (size_t)2 * taps * kATileBytes + (size_t)kw * 2 * (th + kh - 1) * (wt / 8) * 128;
-}
-
 bool supported(int dtype, int kh, int kw, int stride)
 {
     return dtype == LVG_F16 && stride == 1 && ((kh == 3 && kw == 3) || (kh == 1 && kw == 1));
-}
-
-int64_t packed_bytes(int groups, int m_total, int k_total, int taps)
-{
-    const int mt = (m_total + kBM - 1) / kBM, kc = (k_total + kBK - 1) / kBK;
-    return (int64_t)groups * mt * kc * taps * kATileBytes;
-}
-
-// shared driver: packs `w` (viewed as A[m][k][tap]) and runs the GEMM-conv of x into y
-int run_conv(const __half* x, const __half* w, __half* y, int n, int groups, int cin_x, int cout_y, int h, int wd, int kh, int kw,
-             int pad_h, int pad_w, int64_t w_gstride, int64_t w_sm, int64_t w_sk, int flip, void* workspace,
-             int64_t workspace_bytes, cudaStream_t s)
-{
-    const int taps = kh * kw;
-    ConvParams p;
-    p.x = x; p.y = y;
-    p.groups = n * groups; p.wgroups = groups; p.cin = cin_x; p.cout = cout_y;
-    p.h = h; p.w = wd; p.kh = kh; p.kw = kw; p.pad_h = pad_h; p.pad_w = pad_w;
-    p.ho = h + 2 * pad_h - kh + 1;
-    p.wo = wd + 2 * pad_w - kw + 1;
-    LVG_REQUIRE(p.ho >= 1 && p.wo >= 1, "conv2d: empty output");
-    p.mt = (cout_y + kBM - 1) / kBM;
-    p.kc = (cin_x + kBK - 1) / kBK;
-    const int64_t need = packed_bytes(groups, cout_y, cin_x, taps);
-    LVG_REQUIRE(workspace && workspace_bytes >= need, "conv2d: workspace too small (%lld < %lld bytes)", (long long)workspace_bytes, (long long)need);
-    LVG_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 15) == 0, "conv2d: workspace must be 16-byte aligned");
-    p.wp = reinterpret_cast<const __half*>(workspace);
-    pick_tile(p.ho, p.wo, p.th, p.wt, p.tiles_x, p.tiles_y);
-    p.pair_ok = ((reinterpret_cast<uintptr_t>(x) & 3) == 0 && (wd & 1) == 0) ? 1 : 0;
-    LVG_REQUIRE((int64_t)n * groups <= 65535 && p.mt <= 65535, "conv2d: too many groups / channel tiles for one launch");
-
-    {
-        const int64_t total = need / 16;
-        int64_t blocks = (total + 255) / 256;
-        const int64_t cap = (int64_t)num_sms() * 32;
-        if (blocks > cap) blocks = cap;
-        conv_pack_weights_kernel<<<(unsigned)blocks, 256, 0, s>>>(w, reinterpret_cast<__half*>(workspace), groups, cout_y, cin_x, taps,
-                                                                  w_gstride, w_sm, w_sk, flip, p.mt, p.kc);
-        LVG_LAUNCH_CHECK();
-    }
-    const size_t smem = smem_bytes(taps, kh, kw, p.th, p.wt);
-    LVG_REQUIRE(smem <= 110 * 1024, "conv2d: tile does not fit shared memory");
-    LVG_REQUIRE(kBK * (p.th + kh - 1) * (p.wt / 8) <= 4 * kThreads, "conv2d: tile has too many staging items");
-    dim3 grid((unsigned)(p.tiles_x * p.tiles_y), (unsigned)p.mt, (unsigned)p.groups);
-    if (kh == 3) {
-        LVG_CUDA(cudaFuncSetAttribute(conv_fprop_tc_kernel<3, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        conv_fprop_tc_kernel<3, 3><<<grid, kThreads, smem, s>>>(p);
-    } else {
-        LVG_CUDA(cudaFuncSetAttribute(conv_fprop_tc_kernel<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        conv_fprop_tc_kernel<1, 1><<<grid, kThreads, smem, s>>>(p);
-    }
-    LVG_LAUNCH_CHECK();
-    return LVG_OK;
 }
 
 }  // namespace
@@ -364,11 +19,9 @@ using namespace lvg;
 extern "C" int64_t lvg_conv2d_fprop_workspace(int dtype, int n, int groups, int cin, int cout, int h, int wd, int kh, int kw,
                                               int stride, int pad_h, int pad_w)
 {
-    (void)h; (void)wd; (void)pad_h; (void)pad_w;
     if (!supported(dtype, kh, kw, stride) || n < 1) return -1;
-    // enough for either direction (fprop packs [cout][cin], dgrad packs [cin][cout])
-    const int64_t a = packed_bytes(groups, cout, cin, kh * kw), b = packed_bytes(groups, cin, cout, kh * kw);
-    return a > b ? a : b;
+    // enough for either direction
+    return lvg_convnd_workspace(dtype, n, groups, cin, cout, 1, h, wd, 1, kh, kw, 0, pad_h, pad_w);
 }
 
 extern "C" int lvg_conv2d_fprop(const void* x, const void* w, void* y, int dtype, int n, int groups, int cin, int cout,
@@ -380,9 +33,8 @@ extern "C" int lvg_conv2d_fprop(const void* x, const void* w, void* y, int dtype
         set_error("conv2d_fprop: outside the tensor-core kernel's envelope (fp16, stride 1, 3x3 or 1x1)");
         return LVG_UNSUPPORTED;
     }
-    const int taps = kh * kw;
-    return run_conv((const __half*)x, (const __half*)w, (__half*)y, n, groups, cin, cout, h, wd, kh, kw, pad_h, pad_w,
-                    (int64_t)cout * cin * taps, (int64_t)cin * taps, taps, 0, workspace, workspace_bytes, (cudaStream_t)stream);
+    return lvg_convnd_fprop(x, w, y, dtype, n, groups, cin, cout, 1, h, wd, 1, kh, kw, 0, pad_h, pad_w, 1, nullptr, 0, 0.f, 1.f, -1.f,
+                            workspace, workspace_bytes, stream);
 }
 
 extern "C" int lvg_conv2d_dgrad(const void* dy, const void* w, void* dx, int dtype, int n, int groups, int cin, int cout,
@@ -394,9 +46,29 @@ extern "C" int lvg_conv2d_dgrad(const void* dy, const void* w, void* dx, int dty
         set_error("conv2d_dgrad: outside the tensor-core kernel's envelope");
         return LVG_UNSUPPORTED;
     }
-    // dx = correlation of dy (ho x wo, cout channels) with the channel-transposed, spatially mirrored weights, padding k-1-pad
-    const int taps = kh * kw;
-    const int ho = h + 2 * pad_h - kh + 1, wo = wd + 2 * pad_w - kw + 1;
-    return run_conv((const __half*)dy, (const __half*)w, (__half*)dx, n, groups, cout, cin, ho, wo, kh, kw, kh - 1 - pad_h, kw - 1 - pad_w,
-                    (int64_t)cout * cin * taps, taps, (int64_t)cin * taps, 1, workspace, workspace_bytes, (cudaStream_t)stream);
+    return lvg_convnd_dgrad(dy, w, dx, dtype, n, groups, cin, cout, 1, h, wd, 1, kh, kw, 0, pad_h, pad_w, 1, workspace, workspace_bytes,
+                            stream);
+}
+
+// The weight gradient takes no workspace argument: the engine's re-tiled operands and partial sums live in a
+// stream-ordered allocation for the duration of the call.
+extern "C" int lvg_conv2d_wgrad(const void* x, const void* dy, void* dw, int dtype, int n, int groups, int cin, int cout,
+                                int h, int wd, int kh, int kw, int stride, int pad_h, int pad_w, void* stream)
+{
+    LVG_REQUIRE(x && dy && dw, "conv2d_wgrad: x, dy, dw must not be NULL");
+    if (!supported(dtype, kh, kw, stride) || n < 1 || pad_h < 0 || pad_w < 0) {
+        set_error("conv2d_wgrad: outside the tensor-core kernel's envelope (fp16, stride 1, 3x3 or 1x1)");
+        return LVG_UNSUPPORTED;
+    }
+    const int64_t need = lvg_convnd_wgrad_workspace(dtype, n, groups, cin, cout, 1, h, wd, 1, kh, kw, 0, pad_h, pad_w);
+    if (need < 0) {
+        set_error("conv2d_wgrad: outside the tensor-core kernel's envelope");
+        return LVG_UNSUPPORTED;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    void* ws = nullptr;
+    LVG_CUDA(cudaMallocAsync(&ws, (size_t)need, s));
+    const int rc = lvg_convnd_wgrad(x, dy, dw, dtype, n, groups, cin, cout, 1, h, wd, 1, kh, kw, 0, pad_h, pad_w, 1, ws, need, stream);
+    LVG_CUDA(cudaFreeAsync(ws, s));
+    return rc;
 }

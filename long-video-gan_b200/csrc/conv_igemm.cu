@@ -1,4 +1,4 @@
-// Grouped 1-D / 2-D / 3-D convolution (cross-correlation) as a TMA-fed implicit GEMM on tcgen05 tensor cores.
+// Grouped 1-D / 2-D / 3-D convolution (cross-correlation) as a TMA-fed implicit GEMM on Hopper tensor cores (wgmma).
 //
 // One engine for every dense contraction on the path:
 //   conv2d_gradfix.conv2d / conv_transpose2d          (torch_utils/ops/conv2d_gradfix.py:37-45; modulated convolutions of
@@ -20,20 +20,20 @@
 //   * N of one MMA runs linearly over the tile INCLUDING its halo columns; the accumulator columns that straddle two rows
 //     are computed and dropped in the epilogue (kw - 1 of every tile_width columns).
 // GEMM view per instance:  D[co][pix] = sum_{kt} sum_{ci} sum_{ky,kx} W[co][ci][kt][ky][kx] * X[ci][t + kt][y + ky][x + kx]
-//   M = 128 output channels, N = TH x (WT + kw - 1) pixels (<= 256 TMEM columns, 2 CTAs per SM),
+//   M = 128 output channels (two warpgroups of 64), N = TH x (WT + kw - 1) pixels (<= 256 register columns),
 //   K = 16 channels per MMA; the K loop runs over (kt, 16-channel step), every stage issues kh*kw MMAs (one per tap).
 // Weights are re-tiled per call into 128 x 16 K-major images per (m-tile, k-step, tap) (conv_pack_w_kernel) and arrive
 // with one cp.async.bulk per stage.
 //
-// Roles (192 threads): warp 0 = TMA producer (one lane), warp 1 = MMA issuer (one lane, owns TMEM), warps 2-5 = epilogue
-// (TMEM -> registers -> [bias, lrelu, gain, clamp] -> NC(T)HW global). Stages hand over through full/empty mbarriers.
+// Roles (384 threads): warp 0 = TMA producer (one lane), warpgroups 1-2 = wgmma consumers, each with its 64 accumulator rows
+// in registers and its own epilogue ([bias, lrelu, gain, clamp] -> NC(T)HW global). Stages hand over through full/empty mbarriers.
 
 #include <cuda.h>
 #include <stdlib.h>
 #include <cuda_bf16.h>
 
 #include "common.cuh"
-#include "tcgen05.cuh"
+#include "wgmma.cuh"
 
 namespace lvg {
 // conv_pointwise.cu: streaming fp32 kernels for 1x1x1 convolutions with few channels (HBM-bound; the engine would re-tile and pad)
@@ -50,10 +50,11 @@ using namespace tc;
 
 constexpr int kBM = 128;
 constexpr int kATile = kBM * 16 * 2;          // one 128 x 16 weight image: 4096 bytes
-constexpr int kThreads = 192;
-constexpr int kEpiWarps = 8;                          // conv_igemm_kernel: two epilogue warps per TMEM lane quadrant (they alternate 32-column blocks)
-constexpr int kIgemmThreads = 64 + 32 * kEpiWarps;
+constexpr int kIgemmThreads = 384;           // both kernels: a producer warpgroup and two consumer warpgroups
+constexpr int kMaxChunks = 4;                // conv_igemm_kernel: accumulator columns in chunks of 64 (<= 256)
+constexpr int kWgradChunks = 8;              // conv_wgrad_v2_kernel: accumulator columns in chunks of 32 (<= 256)
 constexpr int kMaxStages = 6;
+constexpr int kBSlack = 1024;                // shared memory behind an activation stage that MMAs may read
 
 struct IgemmParams {
     const unsigned char* wp;     // packed weights [wgroups][mt][kc][taps_all][4096]
@@ -71,10 +72,7 @@ struct IgemmParams {
     int kt, kh, kw, pad_t, pad_h, pad_w;
     int tt, th, wt, wtb, thb;    // tile frames / rows / cols, box cols / rows
     int frame_px;                // thb * wtb: accumulator columns from one frame of the tile to the next
-    int ncols;                   // accumulator columns (multiple of 16, <= 512)
-    int n0;                      // columns of the first MMA of a tap (the second one takes ncols - n0; 0 = single MMA)
-    int epi_warps;               // epilogue warps that take part (4 or 8)
-    int nbuf;                    // accumulator buffers in TMEM: 2 when ncols <= 256 (epilogue of tile i overlaps tile i + 1)
+    int ncols;                   // accumulator columns (multiple of 16, <= 256; the MMAs compute them in chunks of 64)
     int tiles_x, tiles_y, tiles_t;
     int64_t total_tiles;         // tiles_x * tiles_y * tiles_t * mt * instances
     int ks;                      // k-steps per stage (> 1 only when kt == 1)
@@ -164,10 +162,10 @@ int pack_act(const void* x, void* x8, int split, int64_t inst, int c, int cblk, 
 // run of 16*taps elements per output channel; dgrad: one run of 128*taps elements per k): a warp copies a run into shared
 // memory with aligned 4-byte loads (no per-element index arithmetic), then every thread assembles one 16-byte image row
 // from 8 shared-memory reads and consecutive threads write consecutive rows (512 contiguous bytes per warp).
-// Rows of the 128-row weight image (= TMEM lanes of the accumulator). An epilogue warp can only read the 32 lanes of its
-// quadrant, so an m-tile with fewer than 128 output channels spreads them evenly over the four quadrants (`per` channels at
-// the start of each) instead of filling quadrant after quadrant: all epilogue warps share the store work of a 32- or
-// 64-channel layer. Channels >= 4 * per (zero rows) take the remaining rows in order.
+// Rows of the 128-row weight image (= accumulator rows). An m-tile with fewer than 128 output channels spreads them evenly
+// over the four 32-row quarters (`per` channels at the start of each) instead of filling quarter after quarter, so that
+// both consumer warpgroups and all their warps share the epilogue's store work of a 32- or 64-channel layer. Channels
+// >= 4 * per (zero rows) take the remaining rows in order.
 __host__ __device__ __forceinline__ int m_rows_per_quadrant(int channels_left)
 {
     const int cv = channels_left < kBM ? (channels_left > 0 ? channels_left : 0) : kBM;
@@ -179,6 +177,14 @@ __host__ __device__ __forceinline__ int m_row_of_channel(int ch, int per)
     if (ch < 4 * per) return (ch / per) * 32 + ch % per;
     const int r = ch - 4 * per;
     return (r / (32 - per)) * 32 + per + r % (32 - per);
+}
+
+// inverse of m_row_of_channel: the channel (relative to the m-tile) held by image row `row`
+__host__ __device__ __forceinline__ int m_channel_of_row(int row, int per)
+{
+    if (per >= 32) return row;
+    const int q = row / 32, i = row % 32;
+    return i < per ? q * per + i : 4 * per + q * (32 - per) + (i - per);
 }
 
 template <class TIn, bool SPLIT>
@@ -304,35 +310,31 @@ __device__ __forceinline__ TileCoord decode_tile(const IgemmParams& p, int64_t L
 }
 
 // Persistent: CTA b works on tiles b, b + gridDim.x, ... (pixel tile fastest, so that concurrently running CTAs share the
-// weight tiles of one (instance, m-tile) in L2). The operand ring runs across tile boundaries; with <= 256 accumulator
-// columns two TMEM buffers alternate, so the epilogue of tile i overlaps the main loop of tile i + 1.
+// weight tiles of one (instance, m-tile) in L2). The operand ring runs across tile boundaries, so the producer fetches the
+// first stages of tile i + 1 while the consumers store tile i.
+// Roles (384 threads): warp 0 = TMA producer (one lane); warpgroups 1 and 2 = MMA + epilogue for accumulator rows 0-63 and
+// 64-127 of the weight images. Each consumer holds its 64 x ncols fp32 accumulator in registers (ncols <= 256, issued as
+// chunks of 64 columns) and releases a stage once the wgmma group that read it has completed.
+template <bool BF16, int NCH>
 __global__ void __launch_bounds__(kIgemmThreads, 1) conv_igemm_kernel(const __grid_constant__ CUtensorMap tmx, const IgemmParams p)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    __shared__ uint64_t full_bar[kMaxStages], empty_bar[kMaxStages], acc_full[2], acc_empty[2];
-    __shared__ uint32_t tmem_slot;
+    __shared__ uint64_t full_bar[kMaxStages], empty_bar[kMaxStages];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~(uintptr_t)127);
 
     const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+    const int wg = __shfl_sync(0xffffffffu, (int)threadIdx.x / 128, 0);     // warpgroup index, warp-uniform to the compiler
     const int taps2 = p.kh * p.kw;
     const int kchunks = (p.kc + p.ks - 1) / p.ks;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < p.stages; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        for (int b = 0; b < 2; b++) { mbar_init(&acc_full[b], 1); mbar_init(&acc_empty[b], (uint32_t)p.epi_warps); }
+        for (int s = 0; s < p.stages; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
         fence_barrier_init();
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(&tmem_slot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = tmem_slot;
 
-    if (warp == 0) {
-        if (elect_one()) {
+    if (wg == 0) {
+        if (warp == 0 && elect_one()) {
             int it = 0;
             for (int64_t L = blockIdx.x; L < p.total_tiles; L += gridDim.x) {
                 const TileCoord c = decode_tile(p, L);
@@ -360,145 +362,110 @@ __global__ void __launch_bounds__(kIgemmThreads, 1) conv_igemm_kernel(const __gr
                 }
             }
         }
-    } else if (warp == 1) {
-        if (elect_one()) {
-            // instruction descriptors: D = f32, A and B K-major, fp16 or bf16 operands, N >> 3, M >> 4
-            const uint32_t ibase = (1u << 4) | (p.bf16 ? ((1u << 7) | (1u << 10)) : 0u) | ((uint32_t)(kBM >> 4) << 24);
-            const int na = p.n0 > 0 ? p.n0 : p.ncols, nb = p.n0 > 0 ? p.ncols - p.n0 : 0;
-            const uint32_t idesc_a = ibase | ((uint32_t)(na >> 3) << 17), idesc_b = ibase | ((uint32_t)(nb >> 3) << 17);
-            const uint32_t blk_bytes = (uint32_t)p.b_box / 2;
-            int it = 0, i = 0;
-            for (int64_t L = blockIdx.x; L < p.total_tiles; L += gridDim.x, i++) {
-                const int buf = i % p.nbuf;
-                if (i >= p.nbuf) mbar_wait(&acc_empty[buf], (uint32_t)((i / p.nbuf - 1) & 1));
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_base + (uint32_t)buf * 256;
-                bool first = true;
-                for (int kt = 0; kt < p.kt; kt++) {
-                    for (int kcix = 0; kcix < kchunks; kcix++, it++) {
-                        const int s = it % p.stages;
-                        mbar_wait(&full_bar[s], (uint32_t)((it / p.stages) & 1));
-                        tc_fence_after();
-                        const uint32_t st = smem_u32(smem + (size_t)s * p.stage_bytes);
-                        const int nks = min(p.ks, p.kc - kcix * p.ks);
-                        // descriptors as (lo, hi) words, stepped with 32-bit adds on the low word (address >> 4): the next tap's weight
-                        // image(s) + nimg * 4096 bytes, the next tap column + 16 bytes, the next tap row + wtb * 16 bytes
-                        const uint32_t a_hi = desc_hi(128), b_hi = desc_hi(128);
-                        const uint32_t a_tap = (uint32_t)(p.nimg * kATile) >> 4, b_lo_img = (uint32_t)p.b_bytes >> 4, b_nb = (uint32_t)na;
-                        // wide tiles (two MMAs per tap, columns [0, na) and [na, ncols)): all taps of one half, then the other --
-                        // consecutive MMAs keep accumulating into the same tensor-memory columns (switching them costs ~60 clocks)
-                        for (int j = 0; j < nks; j++) {
-                            const uint32_t a_base = desc_lo(st + (uint32_t)(j * taps2 * p.nimg) * kATile, 2048);
-                            const uint32_t b_base = desc_lo(st + (uint32_t)p.a_stage + (uint32_t)j * (uint32_t)p.b_step, blk_bytes);
-                            for (int half = 0; half < (nb > 0 ? 2 : 1); half++) {
-                                const uint32_t tm = tmem_d + (half ? (uint32_t)na : 0u);
-                                const uint32_t id = half ? idesc_b : idesc_a;
-                                uint32_t a_lo = a_base, b_row = b_base + (half ? b_nb : 0u);
-                                uint32_t acc = first ? 0u : 1u;
-                                for (int ky = 0; ky < p.kh; ky++, b_row += (uint32_t)p.wtb) {
-                                    uint32_t b_lo = b_row;
-                                    for (int kx = 0; kx < p.kw; kx++, b_lo++, a_lo += a_tap) {
-                                        // fp16: one product; split: hi*hi, hi*lo, lo*hi (A image hi, hi, lo; B image hi, lo, hi)
-                                        umma_f16_w(tm, a_lo, a_hi, b_lo, b_hi, id, acc);
-                                        acc = 1u;
-                                        if (p.nimg == 2) {
-                                            umma_f16_w(tm, a_lo, a_hi, b_lo + b_lo_img, b_hi, id, 1u);
-                                            umma_f16_w(tm, a_lo + (kATile >> 4), a_hi, b_lo, b_hi, id, 1u);
-                                        }
+    } else if (wg >= 1) {
+        const int cw = wg - 1;                               // accumulator rows 64 cw .. 64 cw + 63
+        const int tid = threadIdx.x % 128, wq = tid / 32;
+        const uint32_t blk_bytes = (uint32_t)p.b_box / 2;
+        const uint32_t a_hi = desc_hi(128), b_hi = desc_hi(128);
+        const uint32_t a_tap = (uint32_t)(p.nimg * kATile) >> 4, b_lo_img = (uint32_t)p.b_bytes >> 4;
+        int it = 0;
+        for (int64_t L = blockIdx.x; L < p.total_tiles; L += gridDim.x) {
+            const TileCoord c = decode_tile(p, L);
+            float acc[NCH][32];                              // NCH = ncols / 64 rounded up (columns >= ncols are computed and dropped)
+#pragma unroll
+            for (int ch = 0; ch < NCH; ch++)
+#pragma unroll
+                for (int i = 0; i < 32; i++) acc[ch][i] = 0.f;
+            int prev = -1;
+            for (int kt = 0; kt < p.kt; kt++) {
+                for (int kcix = 0; kcix < kchunks; kcix++, it++) {
+                    const int s = it % p.stages;
+                    mbar_wait(&full_bar[s], (uint32_t)((it / p.stages) & 1));
+                    wgmma_fence();
+                    const uint32_t st = smem_u32(smem + (size_t)s * p.stage_bytes);
+                    const int nks = min(p.ks, p.kc - kcix * p.ks);
+                    // descriptors as (lo, hi) words, stepped with 32-bit adds on the low word (address >> 4): the next tap's weight
+                    // image(s) + nimg * 4096 bytes, the next tap column + 16 bytes, the next tap row + wtb * 16 bytes, the next
+                    // 64 accumulator columns + 1024 bytes; this warpgroup's 64 weight rows start 1024 bytes into an image
+                    for (int j = 0; j < nks; j++) {
+                        uint32_t a_lo = desc_lo(st + (uint32_t)(j * taps2 * p.nimg) * kATile + (uint32_t)cw * 1024u, 2048);
+                        const uint32_t b_base = desc_lo(st + (uint32_t)p.a_stage + (uint32_t)j * (uint32_t)p.b_step, blk_bytes);
+                        for (int ky = 0; ky < p.kh; ky++) {
+                            for (int kx = 0; kx < p.kw; kx++, a_lo += a_tap) {
+                                const uint32_t b_lo = b_base + (uint32_t)(ky * p.wtb + kx);
+#pragma unroll
+                                for (int ch = 0; ch < NCH; ch++) {
+                                    // fp16: one product; split: hi*hi, hi*lo, lo*hi (A image hi, hi, lo; B image hi, lo, hi)
+                                    wgmma_m64n64k16<BF16, 0, 0>(acc[ch], a_lo, a_hi, b_lo + 64u * ch, b_hi);
+                                    if constexpr (BF16) {
+                                        wgmma_m64n64k16<BF16, 0, 0>(acc[ch], a_lo, a_hi, b_lo + 64u * ch + b_lo_img, b_hi);
+                                        wgmma_m64n64k16<BF16, 0, 0>(acc[ch], a_lo + (kATile >> 4), a_hi, b_lo + 64u * ch, b_hi);
                                     }
                                 }
                             }
-                            first = false;
                         }
-                        umma_commit(&empty_bar[s]);
                     }
+                    wgmma_commit();
+                    wgmma_wait<1>();                          // the group of the previous stage has completed: release its slot
+                    mbar_arrive_if(&empty_bar[prev >= 0 ? prev : 0], prev >= 0 && tid == 0);
+                    prev = s;
                 }
-                umma_commit(&acc_full[buf]);
             }
-        }
-    } else if (warp - 2 < p.epi_warps) {
-        // ---- epilogue warps: TMEM lane quadrant = warp % 4 (a warp can only read its own 32 lanes = 32 output channels of the
-        // tile); the two warps of a quadrant alternate the 32-column blocks. Each warp has a private 32 x 33 transposition
-        // buffer so that a store instruction covers 32 consecutive pixels of one channel. With short K loops (1x3x3 / 1x1x1
-        // layers, few channels) this epilogue, not the MMA loop, bounds the kernel (ncu on the 32 -> 64 layer of the low-res
-        // discriminator: tensor pipe 30 % active with ONE latency-bound warp per quadrant storing channel by channel), hence
-        // two warps per quadrant (p.epi_warps = 8) for short K loops and eight independent shared-memory reads in flight
-        // before their stores. Long K loops keep four warps: the second set's transposition buffers would cost a pipeline stage.
-        const int q = warp % 4, half = (warp - 2) / 4, nhalf = p.epi_warps / 4;
-        float* sT = reinterpret_cast<float*>(smem + (size_t)p.stages * p.stage_bytes + 512) + (warp - 2) * (32 * 33);
-        int i = 0;
-        for (int64_t L = blockIdx.x; L < p.total_tiles; L += gridDim.x, i++) {
-            const TileCoord c = decode_tile(p, L);
-            const int buf = i % p.nbuf;
-            mbar_wait(&acc_full[buf], (uint32_t)((i / p.nbuf) & 1));
-            tc_fence_after();
-            const uint32_t tmem_d = tmem_base + (uint32_t)buf * 256;
-            const int per = m_rows_per_quadrant(p.cout - c.mti * kBM);     // channels per lane quadrant (conv_pack_w_kernel's row order)
-            const int m0 = c.mti * kBM + q * per;
-            const int rows_ok = min(per, p.cout - m0);               // channels of this warp that exist (lanes 0 .. rows_ok - 1)
-            const int m_lane = m0 + lane;                            // this lane's channel while the values are in registers
-            const float b = (p.bias != nullptr && lane < rows_ok) ? __ldg(p.bias + (int64_t)(c.inst % p.wgroups) * p.cout + m_lane) : 0.f;
-            const int64_t ch0 = ((int64_t)c.inst * p.cout + m0) * p.y_cs;
-            for (int n0 = 32 * half; n0 < p.ncols && rows_ok > 0; n0 += 32 * nhalf) {
-                uint32_t acc[32];
-                tmem_ld32(tmem_d + ((uint32_t)(q * 32) << 16) + (uint32_t)n0, acc);
+            wgmma_wait<0>();
+            mbar_arrive_if(&empty_bar[prev], tid == 0);
+
+            // ---- epilogue: registers -> [bias, lrelu, gain, clamp] -> NC(T)HW global. This thread holds accumulator rows
+            // r and r + 8 (conv_pack_w_kernel's row order -> channel) and column pairs 8 j + 2 (lane % 4) of every chunk.
+            const int per = m_rows_per_quadrant(p.cout - c.mti * kBM);
+            int64_t chbase[2];
+            float bias[2];
+            bool rok[2];
 #pragma unroll
-                for (int j = 0; j < 32; j++) {
-                    float v = __uint_as_float(acc[j]);
-                    if (p.act) {
-                        v += b;
-                        if (p.act == 2) v = v < 0.f ? v * p.alpha : v;
-                        v *= p.gain;
-                        if (p.clamp >= 0.f) v = fminf(fmaxf(v, -p.clamp), p.clamp);
-                    }
-                    sT[j * 33 + lane] = v;
-                }
-                __syncwarp();
-                // lane = accumulator column n0 + lane -> (frame, row, col) of the tile
-                const int n = n0 + lane;
-                const int f = n / p.frame_px, rem = n - f * p.frame_px;
-                const int r = rem / p.wtb, cc = rem - r * p.wtb;
-                const int ot = c.t0 + f, oy = c.oy0 + r, ox = c.ox0 + cc;
-                bool ok = n < p.ncols && f < p.tt && r < p.th && cc < p.wt && ot < p.to && oy < p.ho && ox < p.wo;
-                int64_t off;
-                if (p.ostride == 1) {
-                    off = ch0 + ((int64_t)ot * p.ho + oy) * p.wo + ox;
-                } else {
-                    ok = ok && (oy % p.ostride == 0) && (ox % p.ostride == 0);
-                    off = ch0 + ((int64_t)ot * p.hos + oy / p.ostride) * p.wos + ox / p.ostride;
-                }
-                if (ok) {
-                    const float* src = sT + lane * 33;
-                    if (p.out_f32) {
-                        float* y = reinterpret_cast<float*>(p.y) + off;
-                        for (int row0 = 0; row0 < rows_ok; row0 += 8, y += 8 * p.y_cs) {
-                            float v8[8];
-#pragma unroll
-                            for (int k = 0; k < 8; k++) v8[k] = src[row0 + k];
-#pragma unroll
-                            for (int k = 0; k < 8; k++) if (row0 + k < rows_ok) y[(int64_t)k * p.y_cs] = v8[k];
-                        }
-                    } else {
-                        __half* y = reinterpret_cast<__half*>(p.y) + off;
-                        for (int row0 = 0; row0 < rows_ok; row0 += 8, y += 8 * p.y_cs) {
-                            float v8[8];
-#pragma unroll
-                            for (int k = 0; k < 8; k++) v8[k] = src[row0 + k];
-#pragma unroll
-                            for (int k = 0; k < 8; k++) if (row0 + k < rows_ok) y[(int64_t)k * p.y_cs] = __float2half_rn(v8[k]);
-                        }
-                    }
-                }
-                __syncwarp();
+            for (int h = 0; h < 2; h++) {
+                const int ch = m_channel_of_row(cw * 64 + wq * 16 + lane / 4 + 8 * h, per);
+                const int co = c.mti * kBM + ch;
+                rok[h] = ch < kBM && co < p.cout;
+                bias[h] = (p.bias != nullptr && rok[h]) ? __ldg(p.bias + (int64_t)(c.inst % p.wgroups) * p.cout + co) : 0.f;
+                chbase[h] = ((int64_t)c.inst * p.cout + co) * p.y_cs;
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&acc_empty[buf]);
+#pragma unroll
+            for (int ch = 0; ch < NCH; ch++) {
+#pragma unroll
+                for (int j = 0; j < 8; j++) {
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        // accumulator column -> (frame, row, col) of the tile
+                        const int n = ch * 64 + j * 8 + 2 * (lane % 4) + e;
+                        const int f = n / p.frame_px, rem = n - f * p.frame_px;
+                        const int r = rem / p.wtb, cc = rem - r * p.wtb;
+                        const int ot = c.t0 + f, oy = c.oy0 + r, ox = c.ox0 + cc;
+                        bool ok = n < p.ncols && f < p.tt && r < p.th && cc < p.wt && ot < p.to && oy < p.ho && ox < p.wo;
+                        int64_t off;
+                        if (p.ostride == 1) {
+                            off = ((int64_t)ot * p.ho + oy) * p.wo + ox;
+                        } else {
+                            ok = ok && (oy % p.ostride == 0) && (ox % p.ostride == 0);
+                            off = ((int64_t)ot * p.hos + oy / p.ostride) * p.wos + ox / p.ostride;
+                        }
+                        if (!ok) continue;
+#pragma unroll
+                        for (int h = 0; h < 2; h++) {
+                            if (!rok[h]) continue;
+                            float v = acc[ch][4 * j + 2 * h + e];
+                            if (p.act) {
+                                v += bias[h];
+                                if (p.act == 2) v = v < 0.f ? v * p.alpha : v;
+                                v *= p.gain;
+                                if (p.clamp >= 0.f) v = fminf(fmaxf(v, -p.clamp), p.clamp);
+                            }
+                            if (p.out_f32) reinterpret_cast<float*>(p.y)[chbase[h] + off] = v;
+                            else reinterpret_cast<__half*>(p.y)[chbase[h] + off] = __float2half_rn(v);
+                        }
+                    }
+                }
+            }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, 512);
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -601,27 +568,20 @@ int run_igemm(const void* x, const void* w, void* y, int dtype, int n, int group
     p.to = t + 2 * pad_t - kt + 1; p.ho = h + 2 * pad_h - kh + 1; p.wo = wd + 2 * pad_w - kw + 1;
     LVG_REQUIRE(p.to >= 1 && p.ho >= 1 && p.wo >= 1, "convnd: empty output");
     p.kt = kt; p.kh = kh; p.kw = kw; p.pad_t = pad_t; p.pad_h = pad_h; p.pad_w = pad_w;
-    // tile: whole rows (and, for small frames, several frames) up to 512 accumulator columns; wide images are cut into
-    // column tiles. A tile of <= 256 columns leaves room for two accumulator buffers (epilogue overlap).
-    // (short K loops -- up to ~160 MMAs per tile -- are epilogue-bound: they take <= 256 columns and alternate two accumulator
-    // buffers; measured on the sres discriminator shapes: 0.173 vs 0.200 ms at 256 -> 256 channels 64x64)
+    // tile: whole rows (and, for small frames, several frames) up to 256 accumulator columns (the register accumulator of a
+    // consumer warpgroup: 128 fp32 registers per thread); wide images are cut into column tiles. LVG_CONV_COLS lowers it.
     const char* cb_env = getenv("LVG_CONV_COLS");
     const int taps2 = kh * kw;
-    int epi_bytes = 4 * 32 * 33 * 4 + 512;              // four epilogue warps; eight when that costs neither tile size nor the second stage (below)
-    int smem_budget = 224 * 1024 - epi_bytes;
+    const int smem_budget = 224 * 1024;
     p.ostride = ostride;
     p.hos = (p.ho - 1) / ostride + 1; p.wos = (p.wo - 1) / ostride + 1;
     p.ks = (kt == 1) ? (taps2 == 1 ? 4 : (taps2 <= 3 ? 2 : 1)) : 1;
     if (p.ks > g.kc) p.ks = g.kc;
     p.a_stage = p.ks * taps2 * g.nimg * kATile;
     // the column budget shrinks until two stages fit shared memory (split precision doubles both operands of a stage)
-    // (fp32 / split precision: 256 columns whatever the K loop, since the MMA issue path costs 4 instructions per MMA: two
-    // alternating accumulators -- the epilogue of tile i under the main loop of tile i + 1 -- beat the better weight-tile
-    // amortisation of 512-column tiles on every layer class of a low-res step, 72.7 -> 69.8 ms forward, 55.6 -> 54.2 ms input
-    // gradients; the small-frame layers also get more tiles than SMs: 512 channels at 3x4 pixels 0.30 -> 0.22 ms. fp16 layers
-    // (one product per tap against the same weight bytes per tap: the weight tile weighs 1.5x more) keep 512 columns for long
-    // K loops, the configuration their super-res numbers were measured with. LVG_CONV_COLS overrides both.)
-    for (int col_budget = cb_env ? atoi(cb_env) : ((split || g.kc * kt * taps2 <= 160) ? 256 : 512);; col_budget -= 64) {
+    int col_budget0 = cb_env ? atoi(cb_env) : 256;
+    if (col_budget0 > 256) col_budget0 = 256;
+    for (int col_budget = col_budget0;; col_budget -= 64) {
         LVG_REQUIRE(col_budget >= 64, "convnd: no tile fits shared memory");
         const int max_wt = 128 - (kw - 1);                    // a TMA box row is at most 256 8-byte elements
         p.tiles_x = (p.wo + max_wt - 1) / max_wt;
@@ -651,25 +611,14 @@ int run_igemm(const void* x, const void* w, void* y, int dtype, int n, int group
         p.b_box = 2 * p.tt * p.frame_px * 16;                  // one pair of blocks as TMA writes it
         p.b_bytes = round_up(p.b_box, 128);
         p.b_step = g.nimg * p.b_bytes;
-        p.stage_bytes = round_up(p.a_stage + p.ks * p.b_step + 512, 128);      // + slack: the last taps read a few pixels past the tile
-        if (p.ncols <= 512 && 2 * p.stage_bytes <= smem_budget) break;
+        // + slack: the last taps and the columns of the last 64-column chunk past ncols read up to 50 pixels past the tile
+        p.stage_bytes = round_up(p.a_stage + p.ks * p.b_step + kBSlack, 128);
+        if (p.ncols <= 256 && 2 * p.stage_bytes <= smem_budget) break;
         if (p.th == 1 && p.tt == 1 && col_budget <= p.wtb) { LVG_REQUIRE(false, "convnd: a one-row tile does not fit shared memory"); }
     }
-    LVG_REQUIRE(p.th >= 1 && p.ncols <= 512 && p.ncols >= 16, "convnd: tile geometry");
-    // epilogue warps: eight when their extra transposition buffers cost no pipeline stage (every layer gains: the fp16
-    // 539 -> 512 layer 1.29 -> 1.17 ms), or when the K loop is short anyway (epilogue-bound layers: 32 -> 32 1x3x3 of the
-    // low-res discriminator 1.81 -> 1.22 ms); else four (the fp32 512-channel 3x3x3 layer loses a stage: 3.9 -> 6.5 ms with eight)
-    auto stages_for = [&](int budget) { int st = 2; while (st < kMaxStages && (st + 1) * p.stage_bytes <= budget) st++; return st; };
-    const int budget8 = 224 * 1024 - (kEpiWarps * 32 * 33 * 4 + 512);
-    p.epi_warps = 4;
-    if (2 * p.stage_bytes <= budget8 && (stages_for(budget8) == stages_for(smem_budget) || g.kc * kt * taps2 <= 160)) {
-        p.epi_warps = kEpiWarps;
-        epi_bytes = kEpiWarps * 32 * 33 * 4 + 512;
-        smem_budget = budget8;
-    }
-    p.nbuf = p.ncols <= 256 ? 2 : 1;
-    p.n0 = p.ncols <= 256 ? 0 : round_up(p.ncols / 2, 16);
-    p.stages = stages_for(smem_budget);
+    LVG_REQUIRE(p.th >= 1 && p.ncols <= 256 && p.ncols >= 16, "convnd: tile geometry");
+    p.stages = 2;
+    while (p.stages < kMaxStages && (p.stages + 1) * p.stage_bytes <= smem_budget) p.stages++;
     // Short K loops (few input channels, 1x1 / 1x3x3 kernels): when the ring can be cut to a multiple of the stages one tile
     // takes, slot s sees the same (kt, k-chunk) on every tile -- with one weight set for the whole launch (no groups, one
     // m-tile) the weight images stay where the first pass put them and only the activation tiles stream (the weight images
@@ -729,12 +678,16 @@ int run_igemm(const void* x, const void* w, void* y, int dtype, int n, int group
         const int rc = encode_map(&tm, x8, wd, h, t, inst * g.nblk, wd, (int64_t)h * wd, thw, p.wtb, p.thb, p.tt, 2);
         if (rc) return rc;
     }
-    const size_t smem = (size_t)p.stages * p.stage_bytes + epi_bytes + 128;
-    LVG_CUDA(cudaFuncSetAttribute(conv_igemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const size_t smem = (size_t)p.stages * p.stage_bytes + 128;
+    void (*const kerns[2][kMaxChunks])(const CUtensorMap, const IgemmParams) = {
+        {conv_igemm_kernel<false, 1>, conv_igemm_kernel<false, 2>, conv_igemm_kernel<false, 3>, conv_igemm_kernel<false, 4>},
+        {conv_igemm_kernel<true, 1>, conv_igemm_kernel<true, 2>, conv_igemm_kernel<true, 3>, conv_igemm_kernel<true, 4>}};
+    void (*kern)(const CUtensorMap, const IgemmParams) = kerns[split][(p.ncols + 63) / 64 - 1];
+    LVG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const char* cta_env = getenv("LVG_CONV_CTAS");          // experiments: fewer persistent CTAs than SMs
     const int max_ctas = cta_env ? atoi(cta_env) : num_sms();
     int64_t ctas = p.total_tiles < max_ctas ? p.total_tiles : max_ctas;
-    conv_igemm_kernel<<<(unsigned)ctas, kIgemmThreads, smem, s>>>(tm, p);
+    kern<<<(unsigned)ctas, kIgemmThreads, smem, s>>>(tm, p);
     LVG_LAUNCH_CHECK();
     return LVG_OK;
 }
@@ -808,7 +761,7 @@ extern "C" int lvg_convnd_dgrad(const void* dy, const void* w, void* dx, int dty
 // Weight gradient:  dW[g][co][ci][kt][ky][kx] = sum over samples and output pixels of dy[co][pix] * x[ci][pix + tap]
 //
 // GEMM view per CTA (group g, 128-channel tile of co, NT-channel tile of ci, tap row (kt, ky)):
-//   D_kx[co][ci] += A[co][k] * B_kx[ci][k],   K = output pixels, the kw taps of the row as kw accumulators in TMEM.
+//   D_kx[co][ci] += A[co][k] * B_kx[ci][k],   K = output pixels, the kw taps of the row as kw register accumulators.
 // Both operands come from the SAME channel-block-of-8 tensors the forward kernels use, now as MN-major operands: a pixel
 // is a 16-byte row (8 channels) and the pixel index runs linearly at 16 bytes over a stage tile of RH rows x PS columns,
 // PS = (segment width + kw - 1) rounded up to 16. The dy tile is loaded through a tensor map whose W extent is clipped to
@@ -839,21 +792,24 @@ struct WgradV2Params {
     int nsplit;
     int a_bytes, b_bytes, stage_bytes, stages;      // per stage: one A (B) operand image; a stage holds split+1 of each
     int64_t split_stride;        // elements between fp32 partials
-    int tap_major;               // MMA order inside a stage: tap outermost, K steps innermost (else K step outermost, taps innermost)
-    int mrows;                   // M of the MMA: 128, or 64 (cout <= 64): accumulator row 16 j + i then sits in TMEM lane 32 j + i
+    int mrows;                   // output-channel rows computed: 128, or 64 (cout <= 64: one consumer warpgroup)
     int tail_bytes;              // shared memory behind the stage ring that the MMAs may read (kx-shifted last rows; the 128 - 8 * ablk rows without data)
 };
 
 struct WgradMaps { CUtensorMap a[4]; CUtensorMap b; };     // dy8 clipped to each column segment; x8
 
-__global__ void __launch_bounds__(kThreads, 1) conv_wgrad_v2_kernel(const __grid_constant__ WgradMaps maps, const WgradV2Params p)
+// Roles (384 threads): warp 0 = TMA producer (one lane); warpgroups 1 and 2 = MMA + epilogue for output channels 0-63 and
+// 64-127 of the m-tile (only the first when mrows = 64). A consumer holds the khc * kw accumulators of NT columns each in
+// registers (<= 256 columns, issued as chunks of 32 input channels).
+template <bool BF16, int NCH>
+__global__ void __launch_bounds__(kIgemmThreads, 1) conv_wgrad_v2_kernel(const __grid_constant__ WgradMaps maps, const WgradV2Params p)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    __shared__ uint64_t full_bar[kMaxStages], empty_bar[kMaxStages], acc_bar;
-    __shared__ uint32_t tmem_slot;
+    __shared__ uint64_t full_bar[kMaxStages], empty_bar[kMaxStages];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~(uintptr_t)127);
 
     const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+    const int wg = __shfl_sync(0xffffffffu, (int)threadIdx.x / 128, 0);
     int bx = blockIdx.x;
     const int sp = bx % p.nsplit; bx /= p.nsplit;
     int ky0 = 0;
@@ -863,6 +819,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgrad_v2_kernel(const __grid
     const int mti = blockIdx.y, g = blockIdx.z;
     const int NT = p.nt;
     const int nop = p.split ? 2 : 1;                              // operand images per stage and side
+    const int consumers = p.mrows / 64;
 
     // stages of this CTA: (sample, frame, segment, row block), range [s0, s1)
     const int rblocks = (p.ho + p.rh - 1) / p.rh;
@@ -871,26 +828,18 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgrad_v2_kernel(const __grid
     const int s0 = (int)((int64_t)total * sp / p.nsplit), s1 = (int)((int64_t)total * (sp + 1) / p.nsplit);
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < p.stages; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(&acc_bar, 1);
+        for (int s = 0; s < p.stages; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], (uint32_t)consumers); }
         fence_barrier_init();
     }
     // zero the slack behind the stage buffers (the kx-shifted reads of the last block run 32 bytes past its end; the dy
     // values they meet are zero, and zero * garbage must not become NaN)
     // (uninitialised shared memory may hold NaN patterns: clear all of it once)
-    for (int i = threadIdx.x; i < (p.stages * p.stage_bytes + p.tail_bytes) / 16; i += kThreads) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0u, 0u, 0u, 0u);
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(&tmem_slot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
+    for (int i = threadIdx.x; i < (p.stages * p.stage_bytes + p.tail_bytes) / 16; i += kIgemmThreads) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0u, 0u, 0u, 0u);
     fence_proxy_async();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_d = tmem_slot;
 
-    if (warp == 0) {
-        if (elect_one()) {
+    if (wg == 0) {
+        if (warp == 0 && elect_one()) {
             for (int s = s0; s < s1; s++) {
                 const int it = s - s0, slot = it % p.stages;
                 if (it >= p.stages) mbar_wait(&empty_bar[slot], (uint32_t)((it / p.stages - 1) & 1));
@@ -910,120 +859,74 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgrad_v2_kernel(const __grid
                 }
             }
         }
-    } else if (warp == 1) {
-        if (elect_one()) {
-            // instruction descriptor: D = f32, A and B MN-major (bits 15, 16), N >> 3, M >> 4
-            const uint32_t idesc = (1u << 4) | (p.bf16 ? ((1u << 7) | (1u << 10)) : 0u) | (1u << 15) | (1u << 16) | ((uint32_t)(NT >> 3) << 17) |
-                                   ((uint32_t)(p.mrows >> 4) << 24);
-            bool first = true;
-            for (int s = s0; s < s1; s++) {
-                const int it = s - s0, slot = it % p.stages;
-                const int seg = (s / rblocks) % p.nseg;
-                const int rb = s % rblocks;
-                const int rows = min(p.rh, p.ho - rb * p.rh);
-                const int ksteps = (rows * p.ps[seg] + 15) / 16;                 // (a trailing half step reads the zero-filled next row)
-                const uint32_t blk_a = (uint32_t)(p.rh * p.ps[seg] * 16);                    // bytes of one channel block of the dy tile
-                const uint32_t blk_b = (uint32_t)((p.rh + p.khc - 1) * p.ps[seg] * 16);      // ... of the x tile (kh - 1 halo rows when folded)
-                const uint32_t ky_step = (uint32_t)(p.ps[seg] * 16);                          // one tap row down = one tile row further
-                mbar_wait(&full_bar[slot], (uint32_t)((it / p.stages) & 1));
-                tc_fence_after();
-                const uint32_t a0 = smem_u32(smem + (size_t)slot * p.stage_bytes);
-                const uint32_t b0 = a0 + (uint32_t)(nop * p.a_bytes);
-                // descriptors as (lo, hi) words: a K step is +16 on the low word (256 bytes >> 4), a tap column +1, a tap row
-                // + ky_step >> 4 -- the loop below is all this thread does, and its instruction count per MMA bounds the kernel
-                const uint32_t a_hi = desc_hi(blk_a), b_hi = desc_hi(blk_b);
-                const uint32_t ky16 = ky_step >> 4;
-                if (p.tap_major) {
-                    // K steps innermost: consecutive MMAs accumulate into the SAME tensor-memory columns (one tap's accumulator)
-                    uint32_t tcol = tmem_d;
-                    for (int kyi = 0; kyi < p.khc; kyi++) {
-                        for (int kx = 0; kx < p.kw; kx++, tcol += (uint32_t)NT) {
-                            uint32_t acc = first ? 0u : 1u;
-                            for (int term = 0; term < (p.split ? 3 : 1); term++) {
-                                uint32_t a_lo = desc_lo(a0 + (term == 1 ? (uint32_t)p.a_bytes : 0u), 128);     // hi*hi, lo*hi, hi*lo
-                                uint32_t b_lo = desc_lo(b0 + (term == 2 ? (uint32_t)p.b_bytes : 0u), 128) + (uint32_t)kyi * ky16 + (uint32_t)kx;
-                                for (int k = 0; k < ksteps; k++, a_lo += 16, b_lo += 16) { umma_f16_w(tcol, a_lo, a_hi, b_lo, b_hi, idesc, acc); acc = 1u; }
-                            }
-                        }
-                    }
-                    first = false;
-                } else {
-                    for (int term = 0; term < (p.split ? 3 : 1); term++) {
-                        uint32_t a_lo = desc_lo(a0 + (term == 1 ? (uint32_t)p.a_bytes : 0u), 128);     // hi*hi, lo*hi, hi*lo
-                        uint32_t b_lo = desc_lo(b0 + (term == 2 ? (uint32_t)p.b_bytes : 0u), 128);
-                        uint32_t acc = first ? 0u : 1u;
-                        for (int k = 0; k < ksteps; k++, a_lo += 16, b_lo += 16) {
-                            uint32_t b_row = b_lo, tcol = tmem_d;
-                            for (int kyi = 0; kyi < p.khc; kyi++, b_row += ky16) {
-                                uint32_t b_tap = b_row;
-                                for (int kx = 0; kx < p.kw; kx++, b_tap++, tcol += (uint32_t)NT) umma_f16_w(tcol, a_lo, a_hi, b_tap, b_hi, idesc, acc);
-                            }
-                            acc = 1u;
-                        }
-                        first = false;
-                    }
-                }
-                umma_commit(&empty_bar[slot]);
-            }
-            umma_commit(&acc_bar);
-        }
-    }
-    // ---- epilogue, 32 input channels at a time: TMEM -> shared [co][ci * kw + kx] (fp32) -> global rows of kw-runs
-    float* tile = reinterpret_cast<float*>(smem);
-    const int row_pitch = 32 * p.kw + 1;
-    if (warp >= 2) {
-        mbar_wait(&acc_bar, 0);
-        tc_fence_after();
-    }
-    __syncthreads();                       // every stage buffer is free from here on
-    {
-        const int taps = p.kt * p.kh * p.kw;
-        const int ci0 = nti * NT, co0 = mti * kBM;
-        const bool any = s1 > s0;
-        for (int kc0 = 0; kc0 < p.khc * ((NT + 31) / 32); kc0++) {
-            const int kyi = kc0 / ((NT + 31) / 32), c0 = (kc0 - kyi * ((NT + 31) / 32)) * 32;      // tap row of this CTA, first of 32 input channels
-            const int tap0 = (kt * p.kh + ky0 + kyi) * p.kw;
-            if (warp >= 2) {
-                const int q = warp % 4;
-                const bool m64 = p.mrows == 64;
-                const int r = m64 ? q * 16 + (lane & 15) : q * 32 + lane;        // accumulator row held by this lane (M = 64: lanes 16-31 hold none)
-                const bool holds = !m64 || lane < 16;
-                for (int kx = 0; kx < p.kw; kx++) {
-                    uint32_t acc[32];
-                    tmem_ld32(tmem_d + ((uint32_t)(q * 32) << 16) + (uint32_t)((kyi * p.kw + kx) * NT + c0), acc);
-                    if (holds) {
+    } else if (wg >= 1 && wg - 1 < consumers) {
+        const int cw = wg - 1;
+        const int tid = threadIdx.x % 128, wq = tid / 32;
+        const int cpt = NT / 32;                                   // 32-channel chunks per tap
+        float acc[NCH][16];                                        // NCH = khc * kw * NT / 32 accumulator chunks
 #pragma unroll
-                        for (int j = 0; j < 32; j++) tile[r * row_pitch + j * p.kw + kx] = any ? __uint_as_float(acc[j]) : 0.f;
+        for (int ch = 0; ch < NCH; ch++)
+#pragma unroll
+            for (int i = 0; i < 16; i++) acc[ch][i] = 0.f;
+        int prev = -1;
+        for (int s = s0; s < s1; s++) {
+            const int it = s - s0, slot = it % p.stages;
+            const int seg = (s / rblocks) % p.nseg;
+            const int rb = s % rblocks;
+            const int rows = min(p.rh, p.ho - rb * p.rh);
+            const int ksteps = (rows * p.ps[seg] + 15) / 16;                 // (a trailing half step reads the zero-filled next row)
+            const uint32_t blk_a = (uint32_t)(p.rh * p.ps[seg] * 16);                    // bytes of one channel block of the dy tile
+            const uint32_t blk_b = (uint32_t)((p.rh + p.khc - 1) * p.ps[seg] * 16);      // ... of the x tile (kh - 1 halo rows when folded)
+            const uint32_t ky16 = (uint32_t)p.ps[seg];                                   // one tap row down = one tile row further (>> 4)
+            mbar_wait(&full_bar[slot], (uint32_t)((it / p.stages) & 1));
+            wgmma_fence();
+            const uint32_t a0 = smem_u32(smem + (size_t)slot * p.stage_bytes) + (uint32_t)cw * 8u * blk_a;
+            const uint32_t b0 = smem_u32(smem + (size_t)slot * p.stage_bytes) + (uint32_t)(nop * p.a_bytes);
+            // descriptors as (lo, hi) words: a K step is +16 on the low word (256 bytes >> 4), a tap column +1, a tap row
+            // + ps, the next 32 input channels + 4 blocks of the x tile
+            const uint32_t a_hi = desc_hi(blk_a), b_hi = desc_hi(blk_b);
+            const uint32_t chunk16 = (4u * blk_b) >> 4;
+            for (int term = 0; term < (p.split ? 3 : 1); term++) {
+                const uint32_t a_lo0 = desc_lo(a0 + (term == 1 ? (uint32_t)p.a_bytes : 0u), 128);     // hi*hi, lo*hi, hi*lo
+                const uint32_t b_lo0 = desc_lo(b0 + (term == 2 ? (uint32_t)p.b_bytes : 0u), 128);
+                for (int k = 0; k < ksteps; k++) {
+#pragma unroll
+                    for (int ch = 0; ch < NCH; ch++) {
+                        const int tap = ch / cpt, c = ch - tap * cpt;
+                        const int kyi = tap / p.kw, kx = tap - kyi * p.kw;
+                        wgmma_m64n32k16<BF16, 1, 1>(acc[ch], a_lo0 + 16u * k, a_hi,
+                                                    b_lo0 + 16u * k + (uint32_t)kyi * ky16 + (uint32_t)kx + (uint32_t)c * chunk16, b_hi);
                     }
                 }
             }
-            __syncthreads();
-            const int ci_n = min(32, min(NT - c0, p.cin - ci0 - c0));
-            const int per_row = ci_n * p.kw;
-            if (per_row > 0) {
-                for (int r = warp; r < p.mrows; r += kThreads / 32) {
-                    const int co = co0 + r;
-                    if (co >= p.cout) break;
-                    const int64_t base = (((int64_t)g * p.cout + co) * p.cin + ci0 + c0) * taps + tap0;
-                    const float* src = tile + r * row_pitch;
-                    if (p.nsplit > 1) {
-                        float* dst = reinterpret_cast<float*>(p.dw) + (int64_t)sp * p.split_stride + base;
-                        for (int j = lane; j < per_row; j += 32) { const int ci = j / p.kw, kx = j - ci * p.kw; dst[ci * taps + kx] = src[j]; }
-                    } else if (p.out_f32) {
-                        float* dst = reinterpret_cast<float*>(p.dw) + base;
-                        for (int j = lane; j < per_row; j += 32) { const int ci = j / p.kw, kx = j - ci * p.kw; dst[ci * taps + kx] = src[j]; }
-                    } else {
-                        __half* dst = reinterpret_cast<__half*>(p.dw) + base;
-                        for (int j = lane; j < per_row; j += 32) { const int ci = j / p.kw, kx = j - ci * p.kw; dst[ci * taps + kx] = __float2half_rn(src[j]); }
-                    }
-                }
+            wgmma_commit();
+            wgmma_wait<1>();                              // the group of the previous stage has completed: release its slot
+            mbar_arrive_if(&empty_bar[prev >= 0 ? prev : 0], prev >= 0 && tid == 0);
+            prev = slot;
+        }
+        wgmma_wait<0>();
+
+        // ---- epilogue: registers -> dW[g][co][ci][kt][ky][kx] (or the fp32 partial sums of split `sp`)
+        const int taps = p.kt * p.kh * p.kw;
+        const int ci0 = nti * NT;
+#pragma unroll
+        for (int ch = 0; ch < NCH; ch++) {
+            const int tap = ch / cpt, c = ch - tap * cpt;
+            const int kyi = tap / p.kw, kx = tap - kyi * p.kw;
+            const int tapg = (kt * p.kh + ky0 + kyi) * p.kw + kx;
+#pragma unroll
+            for (int i = 0; i < 16; i++) {
+                const int co = mti * kBM + cw * 64 + wq * 16 + lane / 4 + 8 * ((i / 2) % 2);
+                const int cil = c * 32 + (i / 4) * 8 + 2 * (lane % 4) + i % 2;
+                if (co >= p.cout || cil >= NT || ci0 + cil >= p.cin) continue;
+                const int64_t off = (((int64_t)g * p.cout + co) * p.cin + ci0 + cil) * taps + tapg;
+                const float v = acc[ch][i];
+                if (p.nsplit > 1) reinterpret_cast<float*>(p.dw)[(int64_t)sp * p.split_stride + off] = v;
+                else if (p.out_f32) reinterpret_cast<float*>(p.dw)[off] = v;
+                else reinterpret_cast<__half*>(p.dw)[off] = __float2half_rn(v);
             }
-            __syncthreads();
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_d, 512);
 }
 
 template <class TOut>
@@ -1057,20 +960,15 @@ WgradPlan wgrad_plan(int dtype, int n, int groups, int cin, int cout, int t, int
     q.split = dtype == LVG_F32;
     q.cpad_a = wgrad_cpad_a(cout);
     q.ablk = q.cpad_a < kBM ? q.cpad_a / 8 : 16;
-    // M of the MMA. This kernel's MN-major MMAs are paced by their shared-memory operand reads (~64 clocks for 128 dy rows +
-    // N / 2 for the x columns, measured); with at most 64 output channels M = 64 halves the dy part. Accumulator rows
-    // 16 j .. 16 j + 15 then sit in TMEM lanes 32 j .. 32 j + 15 (probed on B200: profiles/r02_probe_m64_tmem_lanes.txt).
+    // rows of the accumulator: with at most 64 output channels one consumer warpgroup (M = 64) does all the work
     q.mrows = (q.cpad_a <= 64 && env_flag("LVG_WGRAD_M64", 1)) ? 64 : kBM;
     q.cpad_b = round_up(cin, 16);
     // Few input channels (<= 32): ONE CTA takes all kh tap rows -- the x tile carries kh - 1 halo rows and a tap row is a
     // start-address shift of one tile row, like kx is a shift of one pixel -- so dy and x are fetched once per (kt, n-tile)
-    // instead of once per (kt, ky). The kh * kw accumulators of NT columns each must fit the 512 TMEM columns, so NT <= 48:
-    // measured (B200, profiles/r02_lres_conv_table.txt), an MN-major MMA of this kernel costs ~(64 + N / 2) clocks whatever
-    // the issue rate -- 32 input channels: 2.56 vs 3.07 ms folded (same MMA count, a third of the operand traffic); 64 input
-    // channels would need two n-tiles of 32 = twice the MMAs: 6.5 vs 4.2 ms, hence the limit (LVG_WGRAD_FOLD_CIN).
-    q.khc = (kh > 1 && cin <= env_flag("LVG_WGRAD_FOLD_CIN", 32) && env_flag("LVG_WGRAD_FOLD", 1)) ? kh : 1;
-    int nt_cap = (512 / (q.khc * kw)) / 16 * 16;
-    if (nt_cap > 256) nt_cap = 256;
+    // instead of once per (kt, ky), where the kh * kw accumulators of 32 columns each fit the 256 register columns of a
+    // consumer warpgroup (kh * kw <= 8).
+    q.khc = (kh > 1 && kh * kw * 32 <= 256 && cin <= env_flag("LVG_WGRAD_FOLD_CIN", 32) && env_flag("LVG_WGRAD_FOLD", 1)) ? kh : 1;
+    int nt_cap = (256 / (q.khc * kw)) / 32 * 32;
     if (q.split && nt_cap > 128) nt_cap = 128;
     // column segments (a TMA box row is at most 128 pixels incl. the kw - 1 halo) and the common tile pitch
     q.nseg = (wo + 128 - kw) / (129 - kw);
@@ -1086,10 +984,10 @@ WgradPlan wgrad_plan(int dtype, int n, int groups, int cin, int cout, int t, int
     }
     {   // the smallest stage (1 or 2 rows) must leave room for two stages
         const int min_rows = q.ps % 16 != 0 ? 2 : 1;
-        while (nt_cap > 16 && 2 * stage_of(min_rows, nt_cap) > 200 * 1024) nt_cap -= 16;
+        while (nt_cap > 32 && 2 * stage_of(min_rows, nt_cap) > 200 * 1024) nt_cap -= 32;
     }
     q.ntiles = (q.cpad_b + nt_cap - 1) / nt_cap;
-    q.nt = round_up((q.cpad_b + q.ntiles - 1) / q.ntiles, 16);
+    q.nt = round_up((q.cpad_b + q.ntiles - 1) / q.ntiles, 32);          // the MMAs take the input channels 32 at a time
     q.cpad_b = q.nt * q.ntiles;
     q.mt = (q.cpad_a + kBM - 1) / kBM;
     const int64_t inst = (int64_t)n * groups;
@@ -1114,17 +1012,14 @@ WgradPlan wgrad_plan(int dtype, int n, int groups, int cin, int cout, int t, int
     }
     q.stages = 2;
     while (q.stages < kMaxStages && (q.stages + 1) * q.stage_bytes + q.tail_bytes <= 220 * 1024) q.stages++;
-    const size_t tile_bytes = (size_t)kBM * (32 * kw + 1) * 4;
-    q.smem = (size_t)q.stages * q.stage_bytes + q.tail_bytes;
-    if (tile_bytes > q.smem) q.smem = tile_bytes;
-    q.smem += 128;
+    q.smem = (size_t)q.stages * q.stage_bytes + q.tail_bytes + 128;
     // Split the pixel range over `nsplit` CTAs per output tile. One CTA per SM is resident, so the kernel runs in waves of
     // num_sms CTAs: choose the split that minimises waves x (stages per CTA + a fixed per-CTA cost of ~4 stages: clearing
-    // shared memory, the TMEM -> global epilogue) -- e.g. 3 output tiles: 49 splits = 147 CTAs = one wave of 470 stages
-    // instead of 64 splits = 192 CTAs = two waves of 360. Partial sums are capped at 256 MB.
+    // shared memory, the register -> global epilogue) -- e.g. with 132 SMs and 3 output tiles: 44 splits = 132 CTAs = one
+    // wave instead of 64 splits = 192 CTAs = two waves. Partial sums are capped at 256 MB.
     const int64_t ctas = (int64_t)q.ntiles * (kh / q.khc) * kt * q.mt * groups;
     const int64_t stages = (int64_t)n * to * q.nseg * ((ho + q.rh - 1) / q.rh);
-    const int sms = 148;
+    const int sms = num_sms();
     int64_t cap = 160;
     if (cap > stages) cap = stages;
     while (cap > 1 && cap * q.dw_elems * 4 > (256ll << 20)) cap--;
@@ -1179,18 +1074,10 @@ int run_wgrad(const void* x, const void* dy, void* dw, int dtype, int n, int gro
     for (int j = 0; j < 4; j++) { p.seg_w[j] = q.seg_w[j]; p.seg_x0[j] = q.seg_x0[j]; p.ps[j] = q.ps; }
     p.rh = q.rh; p.khc = q.khc; p.ablk = q.ablk;
     p.mrows = q.mrows;
-    // MMA order inside a stage. Switching the accumulator (another tap's TMEM columns) between two MMAs costs ~60 clocks on
-    // B200 whatever M and N are (measured: the 32 -> 32 layer of the low-res discriminator 2.63 -> 1.66 ms with the K steps
-    // innermost); with a single K step per stage there is nothing to keep together and the K-outermost order pipelines better
-    // (512 channels at 3x4 pixels: 0.36 vs 0.46 ms).
-    {
-        const int e = env_flag("LVG_WGRAD_TAP_MAJOR", -1);
-        p.tap_major = e >= 0 ? e : (q.rh * q.ps / 16 >= 2 ? 1 : 0);
-    }
     p.a_bytes = q.a_stage; p.b_bytes = q.b_stage; p.stage_bytes = q.stage_bytes; p.stages = q.stages; p.tail_bytes = q.tail_bytes;
     const size_t smem = q.smem;
     LVG_REQUIRE(smem <= 227 * 1024, "convnd_wgrad: stage does not fit shared memory (%zu bytes)", smem);
-    LVG_REQUIRE(q.khc * kw * q.nt <= 512, "convnd_wgrad: accumulators exceed tensor memory");
+    LVG_REQUIRE(q.khc * kw * q.nt <= 32 * kWgradChunks && q.nt % 32 == 0, "convnd_wgrad: accumulators exceed the register budget");
     p.nsplit = q.nsplit;
     p.split_stride = q.dw_elems;
     p.dw = q.nsplit > 1 ? (void*)part : dw;
@@ -1206,9 +1093,14 @@ int run_wgrad(const void* x, const void* dy, void* dw, int dtype, int n, int gro
         const int rc = encode_map(&maps.b, x8, wd, h, t, inst * p.nblk_b, wd, (int64_t)h * wd, thw_b, p.ps[0], p.rh + q.khc - 1, 1, q.nt / 8);
         if (rc) return rc;
     }
-    LVG_CUDA(cudaFuncSetAttribute(conv_wgrad_v2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+#define LVG_WGRAD_KERNELS(B) {conv_wgrad_v2_kernel<B, 1>, conv_wgrad_v2_kernel<B, 2>, conv_wgrad_v2_kernel<B, 3>, conv_wgrad_v2_kernel<B, 4>, \
+                              conv_wgrad_v2_kernel<B, 5>, conv_wgrad_v2_kernel<B, 6>, conv_wgrad_v2_kernel<B, 7>, conv_wgrad_v2_kernel<B, 8>}
+    void (*const kerns[2][kWgradChunks])(const WgradMaps, const WgradV2Params) = {LVG_WGRAD_KERNELS(false), LVG_WGRAD_KERNELS(true)};
+#undef LVG_WGRAD_KERNELS
+    void (*kern)(const WgradMaps, const WgradV2Params) = kerns[q.split][q.khc * kw * q.nt / 32 - 1];
+    LVG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     dim3 grid((unsigned)(q.ntiles * kt * (kh / q.khc) * q.nsplit), (unsigned)q.mt, (unsigned)groups);
-    conv_wgrad_v2_kernel<<<grid, kThreads, smem, s>>>(maps, p);
+    kern<<<grid, kIgemmThreads, smem, s>>>(maps, p);
     LVG_LAUNCH_CHECK();
     if (q.nsplit > 1) {
         int64_t blocks = (q.dw_elems + 255) / 256;
@@ -1292,9 +1184,9 @@ extern "C" int lvg_convnd_plan(int mode, int dtype, int n, int groups, int cin, 
     g_plan_only = nullptr;
     if (rc) return rc;
     const int v[48] = {p.wgroups, p.cout, p.mt, p.kc, p.nblk, p.nimg, p.lo_blk, p.to, p.ho, p.wo, p.kt, p.kh, p.kw, p.pad_t, p.pad_h, p.pad_w,
-                       p.tt, p.th, p.wt, p.wtb, p.thb, p.frame_px, p.ncols, p.n0, p.epi_warps, p.nbuf, p.tiles_x, p.tiles_y, p.tiles_t,
+                       p.tt, p.th, p.wt, p.wtb, p.thb, p.frame_px, p.ncols, p.tiles_x, p.tiles_y, p.tiles_t,
                        (int)p.total_tiles, p.ks, p.stages, p.a_resident, p.a_stage, p.b_step, p.b_bytes, p.b_box, p.stage_bytes, p.ostride, p.hos, p.wos,
-                       0, 0, 0, 0, 0, 0, 0};
+                       0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
     for (int i = 0; i < 48; i++) out[i] = v[i];
     return LVG_OK;
 }

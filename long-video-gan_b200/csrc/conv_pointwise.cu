@@ -4,9 +4,8 @@
 // skip connections: generator_lres.py:544-592, discriminator_lres.py:135-213). They are HBM-bound by a wide margin
 // (<= 8192 multiply-adds per pixel against 8 bytes per channel and pixel), and the tensor-core engine is the wrong tool for
 // them: it re-tiles the input into bf16 hi/lo channel blocks first (one extra read + write of the tensor), pads the
-// 3..64 output channels to a 128-row MMA and runs three products per term. Measured on B200 (tools/lres_conv_table.py):
-// 64->64 over (8, 160, 36, 64): 1.15 ms on the engine vs 0.23 ms of pure traffic; 3->32 over (8, 128, 64, 64): 1.32 ms
-// vs 0.09 ms. These kernels read x once, write y once, and multiply in exact fp32:
+// 3..64 output channels to a 128-row MMA and runs three products per term (tools/lres_conv_table.py compares the two per
+// layer). These kernels read x once, write y once, and multiply in exact fp32:
 //   forward         y[n][co][p] = sum_ci W[co][ci] * x[n][ci][p]
 //   input gradient  the same kernel on dy with the transposed weight view
 //   weight gradient dW[co][ci]  = sum_{n,p} dy[n][co][p] * x[n][ci][p]   (per-CTA partials + the engine's fold kernel)
@@ -20,7 +19,7 @@ namespace {
 constexpr int kPwThreads = 256;
 constexpr int kPwCiChunk = 64;          // input channels staged per pass
 
-__device__ __forceinline__ float2 pw_fma2(float2 a, float2 b, float2 c) { return __ffma2_rn(a, b, c); }
+__device__ __forceinline__ float2 pw_fma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 
 // CO_T output channels per thread (even), CT channel threads; a CTA covers PXT = (256 / CT) * 4 pixels of one sample.
 // ws: weights [ci][COP] (COP = CO_T * CT, zero padded), xs: [ci chunk][PXT].
@@ -212,14 +211,10 @@ bool pw_enabled()
     return v == 1;
 }
 
-// Channel limits from measurements on B200 (tools/lres_conv_table.py, batch 8): forward / input gradient win up to
-// cin * cout = 4096 (64->64 over 2.9 M pixels: 0.73 vs 1.15 ms; 3->32: 0.15 vs 1.32 ms; at 64->128 the engine is ahead:
-// 0.44 vs 0.58 ms); the weight-gradient kernel (shared-memory bound: 8 LDS.128 per 32 packed FMAs and row pitches that
-// collide in the banks) wins only for a handful of channel pairs (3->32: 0.59 vs 1.24 ms, 64->3: 0.68 vs 1.13 ms) and
-// loses from 32->64 on (2.7 vs 1.4 ms).
-// The weight gradient takes this path only on request (LVG_POINTWISE_WGRAD=1): since the engine's weight gradient keeps its K
-// steps together per accumulator it is the faster one even for 3 -> 32 and 64 -> 3 channels (0.40 vs 0.60 ms, 0.47 vs 0.71 ms on
-// B200, tools/lres_conv_table.py with LVG_POINTWISE=0); forward / input gradient stay here (0.15 vs 0.67 ms at 3 -> 32).
+// Channel limits: forward / input gradient take these kernels up to cin * cout = 4096, where the engine's re-tiling and
+// padding cost more than the layer's traffic. The weight-gradient kernel (shared-memory bound: 8 LDS.128 per 32 FMA pairs,
+// row pitches that collide in the banks) runs only on request (LVG_POINTWISE_WGRAD=1); the engine's weight gradient is
+// the default. These limits have not been re-measured on the H100 (tools/lres_conv_table.py compares both paths).
 bool pw_wgrad_enabled()
 {
     const char* e = getenv("LVG_POINTWISE_WGRAD");      // read per call: tests switch it

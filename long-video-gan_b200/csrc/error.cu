@@ -23,5 +23,5 @@ extern "C" int64_t lvg_launch_count(void) { return (int64_t)lvg::launches(); }
 extern "C" int lvg_abi_version(void) { return LVG_ABI_VERSION; }
 extern "C" const char* lvg_last_error(void) { return lvg::g_err; }
 extern "C" const char* lvg_build_info(void) {
-    return "liblvg_ops sm_100a nvcc " __DATE__;
+    return "liblvg_ops sm_90a nvcc " __DATE__;
 }

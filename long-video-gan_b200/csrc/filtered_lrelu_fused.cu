@@ -345,8 +345,8 @@ Cfg pick(int fu_w, int fu_h, int fd_w, int fd_h, int up, int down)
     return CFG_NONE;
 }
 
-// Output tile height. 64x24 tiles fit three CTAs per SM (66 KB, <= 85 registers) and measured 12-18 % faster than
-// 64x32 (two CTAs) on the up2/down2 layers; the up4 configuration has a larger halo and is faster with 64x32.
+// Output tile height. 64x24 tiles fit three CTAs per SM (66 KB, <= 85 registers) against two of 64x32; the up4
+// configuration has a larger halo, for which the taller tile pads fewer rows.
 // An image that a single 32-row tile covers keeps the tall tile. LVG_FL_TOH=24|32 overrides (experiments).
 int tile_rows(int up, int oh)
 {
@@ -354,8 +354,7 @@ int tile_rows(int up, int oh)
     if (forced < 0) { const char* e = getenv("LVG_FL_TOH"); forced = e ? atoi(e) : 0; }
     if (forced == 24 || forced == 32) return forced;
     (void)up;
-    // fewest padded rows wins, ties go to the 24-row tile (3 CTAs per SM). Measured on B200 (fp16, NT = 64): L10 (up 4, 92 rows)
-    // 8.65 ms with 24 vs 9.74 with 32; L3 (38 rows) 0.85 vs 1.06; L5 (56 rows) 2.45 vs 2.30; 16-row tiles lose everywhere.
+    // fewest padded rows wins, ties go to the 24-row tile (3 CTAs per SM); LVG_FL_TOH forces one for measurements
     const int pad24 = (oh + 23) / 24 * 24, pad32 = (oh + 31) / 32 * 32;
     return pad32 < pad24 ? 32 : 24;
 }

@@ -1,9 +1,9 @@
 // Fused filtered leaky ReLU, third formulation: every shared-memory access is a 128-bit (or 64-bit)
-// access and every FMA is a packed f32x2 FMA whose two lanes sit in one aligned register pair as loaded.
+// access and FMAs come in pairs whose two lanes sit in one aligned register pair as loaded.
 //
-// Why: the previous kernel (scalar LDS/STS, per-sample sign codes through a byte tile) issued ~19 K warp
-// instructions per 64x24 tile of which 12 % were FMAs (ncu, profiles/r02_ncu_prof_fl.md). Here the per-tile
-// instruction count is ~3x lower and the kernel is bounded by shared-memory bandwidth / the FMA pipe instead.
+// Why: a formulation with scalar LDS/STS and per-sample sign codes through a byte tile spends most of its instructions on
+// addressing and shared-memory traffic, not on FMAs; here the per-tile instruction count is several times lower and the
+// kernel is bounded by shared-memory bandwidth / the FMA pipe instead.
 //
 // Semantics (torch_utils/ops/filtered_lrelu.cu:139-1099, filtered_lrelu.py:121-153 of the reference):
 //   t[U] = up^2 * sum_s gu[s] * z[U + s - pad0],  z = zero-stuffed (x + b), zero outside the image
@@ -87,7 +87,7 @@ FL_HD int imax(int a, int b) { return a > b ? a : b; }
 FL_HD int fdiv_floor(int a, int b) { int q = a / b; return (a % b != 0 && ((a < 0) != (b < 0))) ? q - 1 : q; }
 FL_HD int fdiv_ceil(int a, int b) { return fdiv_floor(a + b - 1, b); }
 
-// ---- memory and arithmetic primitives (device: vector LDS/STS and FFMA2; host: plain C with alignment asserts)
+// ---- memory and arithmetic primitives (device: vector LDS/STS and paired FMAs; host: plain C with alignment asserts)
 FL_HD float4 lds4(const float* p)
 {
 #ifdef FLV3_HOST_EMU
@@ -116,31 +116,22 @@ FL_HD void sts2(float* p, float a, float b)
 #endif
     *reinterpret_cast<float2*>(p) = make_float2(a, b);
 }
-FL_HD float2 fma2(float2 a, float2 b, float2 c)
-{
-#ifdef FLV3_HOST_EMU
-    return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
-#else
-    return __ffma2_rn(a, b, c);
-#endif
-}
+FL_HD float2 fma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 template <class T> FL_HD float ld_as_float(const T* p);
 template <> FL_HD float ld_as_float<float>(const float* p) { return *p; }
 template <> FL_HD float ld_as_float<__half>(const __half* p) { return __half2float(*p); }
-// x + bias in fp32 (fp16 tensors: one mixed-precision add, SASS FHADD)
+// x + bias in fp32
 FL_HD float ld_plus(const float* p, float bias) { return *p + bias; }
 FL_HD float ld_plus(const __half* p, float bias)
 {
 #ifdef FLV3_HOST_EMU
     return __half2float(*p) + bias;
 #else
-    float r;
-    asm("add.rn.f32.f16 %0, %1, %2;" : "=f"(r) : "h"(__half_as_ushort(*p)), "f"(bias));
-    return r;
+    return __half2float(*p) + bias;
 #endif
 }
 // x[i] + bias with the element address formed by ONE wide multiply-add (the compiler otherwise spends four
-// instructions per 64-bit element address) and, for fp16, the conversion folded into the add
+// instructions per 64-bit element address)
 FL_HD float ld_plus_at(const float* p, int i, float bias)
 {
 #ifdef FLV3_HOST_EMU
@@ -158,7 +149,7 @@ FL_HD float ld_plus_at(const __half* p, int i, float bias)
     return __half2float(p[i]) + bias;
 #else
     float r;
-    asm("{ .reg .b64 a; .reg .b16 h; mad.wide.s32 a, %1, 2, %2; ld.global.nc.b16 h, [a]; add.rn.f32.f16 %0, h, %3; }"
+    asm("{ .reg .b64 a; .reg .b16 h; .reg .f32 v; mad.wide.s32 a, %1, 2, %2; ld.global.nc.b16 h, [a]; cvt.f32.f16 v, h; add.rn.f32 %0, v, %3; }"
         : "=f"(r) : "r"(i), "l"(p), "f"(bias));
     return r;
 #endif
@@ -172,14 +163,7 @@ FL_HD void st_byte_if(uint8_t* q, bool ok, unsigned v)
     asm volatile("{ .reg .pred p; setp.ne.s32 p, %1, 0; @p st.global.u8 [%0], %2; }" :: "l"(q), "r"((int)ok), "r"(v) : "memory");
 #endif
 }
-FL_HD float2 mul2(float2 a, float2 b)
-{
-#ifdef FLV3_HOST_EMU
-    return make_float2(a.x * b.x, a.y * b.y);
-#else
-    return __fmul2_rn(a, b);
-#endif
-}
+FL_HD float2 mul2(float2 a, float2 b) { return make_float2(a.x * b.x, a.y * b.y); }
 // bits 2k of the result = sign bits of v[k] (k < 4); higher bits are garbage the caller masks away.
 // Two byte permutes gather the four top bytes, one multiply moves bit 8k+7 to bit 32+2k.
 FL_HD unsigned sign_bits4(float v0, float v1, float v2, float v3)

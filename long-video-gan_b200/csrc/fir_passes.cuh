@@ -5,7 +5,7 @@
 // keeps the (compile-time sized) filter in registers and lets each thread
 // produce a short run of outputs from one contiguous window of inputs, so a
 // shared-memory load feeds ~4-5 FMAs instead of 1 (LDS issue rate is 1/4 of the
-// FMA rate on sm_100, so this is what keeps the FMA pipe, not the LSU, busy).
+// FMA rate, so this is what keeps the FMA pipe, not the LSU, busy).
 //
 // Up-sampling passes work on the phase-aligned up-sampled axis: position
 // a = UP*q + r (q = "group", r = phase) is
@@ -220,16 +220,14 @@ __device__ __forceinline__ void down_y(const float* __restrict__ in, int pin, in
 }
 
 // ===========================================================================================
-// Packed variants: every thread produces TWO outputs per FMA instruction with the f32x2 form
-// (SASS FFMA2). A plain 3-register FFMA on sm_100 needs two issue cycles whenever two of its
-// sources share a register-bank parity; the packed form moves 64-bit register pairs and runs at
-// the full FP32 rate, and it halves the instruction count of the inner loops.
+// Paired variants: every thread produces TWO outputs per coefficient load, as two scalar FMAs
+// (sm_90 has no packed f32x2 FMA), which halves the shared-memory reads of the inner loops.
 // The two outputs of a pair lie along the axis that is NOT being filtered:
 //   y passes: columns L and L + 32 of a 64-column span (lane L; all accesses stay stride-1 32-bit)
 //   x passes: rows r and r + RW of the same warp item (two conflict-free 32-bit loads)
 // Coefficients are held as (g, g) pairs.
 
-__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return __ffma2_rn(a, b, c); }
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 
 template <int UP, int F, int R, int NTHREADS>
 __device__ __forceinline__ void up_x2(const float* __restrict__ in, int pin, float* __restrict__ out, int pout,

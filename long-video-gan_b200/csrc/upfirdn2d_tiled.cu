@@ -441,8 +441,7 @@ int launch_tiled(TiledParams& p, cudaStream_t s)
     }
     const int64_t blocks = p.pb > 1 ? (p.planes + p.pb - 1) / p.pb : p.planes * p.tiles_x * p.tiles_y;
     if (blocks > INT32_MAX) return LVG_UNSUPPORTED;
-    // (A persistent grid that prefetched the next work item's vectors into registers measured 5-60 % slower on
-    //  B200 -- more live registers, fewer resident CTAs -- and was dropped: one CTA per work item.)
+    // (one CTA per work item: a persistent grid prefetching the next item's vectors costs live registers and resident CTAs)
     auto k = upfirdn2d_tiled_kernel<T, KX, SX, FX, KY, SY, FY>;
     if (smem > 48 * 1024) LVG_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     k<<<(unsigned)blocks, kThreads, smem, s>>>(p);

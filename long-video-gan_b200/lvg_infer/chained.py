@@ -3,7 +3,7 @@
 The reference's ``generate.py:56-88`` runs the low-res generator over the whole sequence, then walks
 ``sres_G.sample_video_segments`` ONE 16-frame segment at a time at batch 1 (``generator_sres.py:662-681``) and finally
 ``torch.cat``s every high-res segment on the device (4096 frames at 256x144 fp32 = 1.8 GB) before the encoder sees the first
-frame. On a B200 a single segment leaves most of the 148 SMs idle (the 64-channel layers launch fewer CTAs than there are
+frame. A single segment leaves most of the SMs idle (the 64-channel layers launch fewer CTAs than there are
 SMs) and the device-side concatenation is what bounds the video length.
 
 ``generate_video`` keeps the reference's arithmetic -- same ``latent_z`` for every segment, same windows with

@@ -1,4 +1,4 @@
-"""Drop-in ``torch_utils`` package holding the B200-native ``torch_utils.ops``.
+"""Drop-in ``torch_utils`` package holding the H100-native ``torch_utils.ops``.
 
 Only the operator path (``torch_utils.ops`` and the plugin loader
 ``torch_utils.custom_ops``) lives here. When this directory is placed on

@@ -1,4 +1,4 @@
-"""Plugin loader for the sm_100a operator library (replaces the JIT loader).
+"""Plugin loader for the sm_90a operator library (replaces the JIT loader).
 
 The reference builds three pybind11 modules at first use
 (``torch_utils/custom_ops.py:59-157`` -> ``torch.utils.cpp_extension.load``).
@@ -566,7 +566,7 @@ class Conv2dPlugin:
 
 
 class ConvNdPlugin:
-    """TMA-fed tcgen05 implicit-GEMM convolution for 1-D / 2-D / 3-D NC(T)HW tensors, fp16 or fp32 (bf16 hi/lo split),
+    """TMA-fed wgmma implicit-GEMM convolution for 1-D / 2-D / 3-D NC(T)HW tensors, fp16 or fp32 (bf16 hi/lo split),
     stride 1: forward (optionally with the bias_act epilogue fused), input gradient, weight gradient. No reference
     plugin: the reference hands these to cuDNN (conv2d_gradfix.py:37-45, generator_lres.py:119, discriminator_lres.py:121,172)."""
 
@@ -699,7 +699,7 @@ _PLUGIN_CLASSES = {
 
 def get_plugin(module_name, sources=None, headers=None, source_dir=None, **build_kwargs):
     """Same call shape as the reference loader (custom_ops.py:59); sources/headers/build flags
-    are accepted and ignored because the library is prebuilt for sm_100a."""
+    are accepted and ignored because the library is prebuilt for sm_90a."""
     if module_name not in _plugins:
         if module_name not in _PLUGIN_CLASSES:
             raise RuntimeError(f'unknown plugin "{module_name}"')

@@ -1,1 +1,1 @@
-"""B200-native drop-in for LongVideoGAN's ``torch_utils.ops`` operator set."""
+"""H100-native drop-in for LongVideoGAN's ``torch_utils.ops`` operator set."""

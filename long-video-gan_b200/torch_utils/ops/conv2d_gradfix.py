@@ -4,7 +4,7 @@ Same functions and module switches as the reference (conv2d_gradfix.py:22-45):
 ``enabled``, ``weight_gradients_disabled``, ``no_weight_gradients()``. In the
 reference the custom autograd path is inert on torch >= 1.11 (:49-58) and every
 call lands in cuDNN. Here this module is the tensor-core boundary: CUDA calls
-inside the envelope of the tcgen05 implicit-GEMM kernel (csrc/conv2d_tc.cu;
+inside the envelope of the wgmma implicit-GEMM kernel (csrc/conv2d_tc.cu;
 grouped "modulated" 3x3 / 1x1 convolutions in fp16) are routed to it through
 ``_native`` below; everything else goes to ``torch.nn.functional``.
 """
@@ -17,7 +17,7 @@ enabled = False                     # kept for API compatibility (train_lres.py:
 weight_gradients_disabled = False   # forcefully skip weight gradients (R1 penalty, see no_weight_gradients)
 
 # Native convolution backend: None = library convolution only (what the reference does). `install_native()`
-# binds the tcgen05 kernel; `LVG_NATIVE_CONV=0` in the environment keeps it off.
+# binds the wgmma engine; `LVG_NATIVE_CONV=0` in the environment keeps it off.
 _native = None
 
 
@@ -123,11 +123,10 @@ class _Conv2dDgrad(torch.autograd.Function):
 
 
 class _Conv2dWgrad(torch.autograd.Function):
-    """dw = sum over samples and pixels of dy (x) shifted x: lvg_conv2d_wgrad (tcgen05, pixels as the GEMM K axis).
+    """dw = sum over samples and pixels of dy (x) shifted x: lvg_conv2d_wgrad (wgmma, pixels as the GEMM K axis).
     LVG_NATIVE_WGRAD = 1: always the native kernel (what the GPU tests set); 0: always ATen / cuDNN; unset ("auto"):
-    native where it measured faster than cuDNN on B200 -- few input channels per group (<= 64: 3.4x on the 27-channel
-    first layer) -- and ATen for the wide layers, where the round-1 kernel reaches 300-440 TFLOP/s against cuDNN's
-    360-740 (profiles/r01_microbench.txt)."""
+    native for few input channels per group (<= 64), where cuDNN's grouped weight gradient is far off the tensor-core
+    rate, and ATen for the wide layers. The split has not been re-measured on the H100."""
 
     @staticmethod
     def forward(ctx, dy, x, w_shape, padding, groups):

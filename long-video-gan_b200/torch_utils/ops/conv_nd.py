@@ -1,4 +1,4 @@
-"""1-D / 2-D / 3-D grouped convolution on the TMA-fed tcgen05 engine (csrc/conv_igemm.cu), with autograd of any order.
+"""1-D / 2-D / 3-D grouped convolution on the TMA-fed wgmma engine (csrc/conv_igemm.cu), with autograd of any order.
 
 Not a module of the reference's ``torch_utils.ops`` -- the reference calls ``torch.nn.functional.conv1d / conv2d / conv3d``
 (cuDNN) directly at these sites:
@@ -191,7 +191,7 @@ def conv_transpose2d(input, weight, bias=None, stride=1, padding=0, output_paddi
 
 class _ConvBiasAct(torch.autograd.Function):
     """conv -> bias_act in ONE kernel: the convolution's epilogue adds the bias, applies linear / lrelu, gain and clamp while
-    the accumulators leave tensor memory (no write + re-read of the pre-activation tensor). Backward: the activation
+    the accumulators leave the registers (no write + re-read of the pre-activation tensor). Backward: the activation
     gradient from the saved output (bias_act semantics, bias_act.py:91-120), then the convolution gradients."""
 
     @staticmethod

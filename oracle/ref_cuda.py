@@ -2,7 +2,7 @@
 
 `load()` imports the UNMODIFIED reference `torch_utils` package staged at oracle/_ref/src (see build_ref.py) under
 the alias `lvgref_torch_utils`, so it can live in one process with this repository's `torch_utils`, and replaces its
-JIT step (`custom_ops.get_plugin`, custom_ops.py:59-157) with a loader of the three plugins prebuilt for sm_100a in
+JIT step (`custom_ops.get_plugin`, custom_ops.py:59-157) with a loader of the three plugins prebuilt for sm_90a in
 oracle/_ref/*.so. Everything above the plugins -- `bias_act.py:126-207`, `upfirdn2d.py:217-273`,
 `filtered_lrelu.py:159-272` (the autograd.Functions, sign-tensor plumbing, fallbacks) -- is the reference's code,
 running its kernels. Only tests/, tools/microbench.py (--ref-cuda) and bench.py's reference legs may use this.
@@ -51,7 +51,7 @@ def patch_custom_ops(custom_ops_module):
 def load():
     """-> namespace with bias_act, upfirdn2d, filtered_lrelu, conv2d_resample, conv2d_gradfix (reference modules)."""
     if not available():
-        raise RuntimeError('oracle/_ref is not built (python oracle/build_ref.py in the authoring container)')
+        raise RuntimeError('oracle/_ref is not built (python oracle/build_ref.py where a reference checkout is present)')
     if ALIAS not in sys.modules:
         sys.modules.setdefault('imageio', types.ModuleType('imageio'))
         if SRC not in sys.path:

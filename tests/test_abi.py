@@ -30,7 +30,7 @@ def test_library_exports_every_declared_symbol():
 def test_version_and_error_string():
     lib = custom_ops.load_library()
     assert lib.lvg_abi_version() == 1
-    assert b'sm_100a' in lib.lvg_build_info()
+    assert b'sm_90a' in lib.lvg_build_info()
     assert isinstance(lib.lvg_last_error(), bytes)
 
 

@@ -1,4 +1,4 @@
-"""The tcgen05 implicit-GEMM convolution (conv2d_gradfix.conv2d -> lvg_conv2d_fprop / lvg_conv2d_dgrad)
+"""The wgmma implicit-GEMM convolution (conv2d_gradfix.conv2d -> lvg_conv2d_fprop / lvg_conv2d_dgrad)
 against torch's own convolution evaluated in fp32 on the same fp16-rounded operands."""
 import numpy as np
 import pytest

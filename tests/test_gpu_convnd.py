@@ -1,4 +1,4 @@
-"""The TMA-fed tcgen05 implicit-GEMM convolution engine (csrc/conv_igemm.cu) through the C ABI, against torch's own
+"""The TMA-fed wgmma implicit-GEMM convolution engine (csrc/conv_igemm.cu) through the C ABI, against torch's own
 convolutions in float64 on the same inputs: 1-D / 2-D / 3-D, fp16 and fp32 (bf16 hi/lo split), forward with and
 without the fused bias_act epilogue, input gradient, weight gradient (with and without split-K, one and two column
 segments). Shapes follow the call sites: conv2d_gradfix.py:37-45 (generator_sres.py:63-65, conv2d_resample.py:29-41),

@@ -1,6 +1,6 @@
 """Drop-in rule ON CUDA: the reference's own `model/*` (unmodified, staged at oracle/_ref/src) runs forward + backward
 (+ an R1-style double backward) on cuda twice -- once over this repository's `torch_utils.ops` (package directory ahead
-on PYTHONPATH, the documented drop-in), once over the reference's own ops and its own CUDA plugins built for sm_100a
+on PYTHONPATH, the documented drop-in), once over the reference's own ops and its own CUDA plugins built for sm_90a
 (oracle #2) -- and the networks' outputs and parameter gradients agree to the north_star tolerances."""
 import os
 import subprocess
@@ -41,7 +41,7 @@ def test_resolution(runs):
 
 
 # low-res networks (all fp32): ours -- torch_utils.ops kernels AND the F.conv3d / F.conv1d calls on the tensor-core engine
-# (bf16 hi/lo split products, fp32 accumulation in tensor memory) -- against the reference on its own CUDA ops and cuDNN in
+# (bf16 hi/lo split products, fp32 accumulation) -- against the reference on its own CUDA ops and cuDNN in
 # strict fp32. (key, max-norm tolerance, L2 tolerance). The activations stay inside the north_star's 1e-3; through ~30
 # convolution layers (up to 13824 products per output) and the backward pass the engine's ~1e-5..7e-5 per-layer error
 # shows up as ~1e-2 in the parameter gradients and in the R1 input gradient -- the price of leaving the SIMT fp32 path

@@ -1,5 +1,5 @@
 """Oracle #2: this repository's CUDA ops against the REFERENCE'S OWN CUDA ops (its three plugins built unmodified for
-sm_100a into oracle/_ref by oracle/build_ref.py, driven by its own Python wrappers bias_act.py:126-207,
+sm_90a into oracle/_ref by oracle/build_ref.py, driven by its own Python wrappers bias_act.py:126-207,
 upfirdn2d.py:217-273, filtered_lrelu.py:159-272) on identical random inputs, on the call signatures the networks
 make (SURVEY Appendix A; real spatial sizes, batch reduced). This is the comparison the north_star states its
 tolerances for: 1e-3 relative fp32 activations, 1e-2 gradients -- checked ELEMENT-WISE here
@@ -241,7 +241,7 @@ CR = [
 @pytest.mark.parametrize('name,xs,ws,kw,dtype', CR, ids=[c[0] for c in CR])
 def test_conv2d_resample_vs_reference_cuda(ref, name, xs, ws, kw, dtype):
     # The reference's conv is cuDNN (conv2d_gradfix.py:37-45 -> F.conv2d; fp32 with TF32 off as train_sres.py sets it);
-    # ours is the tcgen05 kernel where native. Tolerance: fp16 operands, fp32 accumulation on both sides.
+    # ours is the wgmma engine where native. Tolerance: fp16 operands, fp32 accumulation on both sides.
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
     kw = dict(kw)

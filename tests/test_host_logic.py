@@ -204,7 +204,7 @@ def test_conv2d_resample(name):
 
 
 class _TorchConvNative:
-    """Stand-in for the tcgen05 convolution plugin: same methods, torch arithmetic (CPU). Counts the calls."""
+    """Stand-in for the convolution plugin: same methods, torch arithmetic (CPU). Counts the calls."""
 
     def __init__(self):
         self.calls = dict(fprop=0, dgrad=0, wgrad=0)

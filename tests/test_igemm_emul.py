@@ -4,10 +4,10 @@ with the tiling the library itself plans (`lvg_convnd_plan`, host arithmetic of 
 What is replayed in numpy: the persistent tile loop and its decode order, the TMA boxes over the channel-block tensor X8
 with hardware zero fill (halo rows / columns / frames), the stage layout in shared memory, a filter tap as a shift of the
 linear pixel index (ky * tile_width + kx), the MMA over ALL accumulator columns including the halo columns that straddle
-rows and frames, the row order of the weight images (channels of a partial m-tile spread over the four TMEM lane quadrants),
-and the epilogue's map from (TMEM lane, column) to (channel, frame, row, column) with the stride lattice of strided
+rows and frames (in the kernel's 64-column chunks), the row order of the weight images (channels of a partial m-tile spread
+over the four 32-row quarters), and the epilogue's map from (accumulator row, column) to (channel, frame, row, column) with the stride lattice of strided
 convolutions -- against torch.nn.functional convolutions in float64. Checked besides the values: every read stays inside the
-stage buffer (+ its 512-byte slack), every output element is written exactly once, the shared-memory budget, and the
+stage buffer (+ its slack), every output element is written exactly once, the shared-memory budget, and the
 slot-invariance the resident weight images rely on. Not covered: descriptor bit fields, the instruction itself, the weight
 re-tiling kernel's byte layout (the -m gpu tests do). Reference call sites: conv2d_gradfix.py:37-45, generator_lres.py:119,578,
 discriminator_lres.py:121,172."""
@@ -21,7 +21,7 @@ import torch.nn.functional as F
 from torch_utils import custom_ops
 
 FIELDS = ['wgroups', 'rows', 'mt', 'kc', 'nblk', 'nimg', 'lo_blk', 'to', 'ho', 'wo', 'kt', 'kh', 'kw', 'pad_t', 'pad_h', 'pad_w', 'tt', 'th',
-          'wt', 'wtb', 'thb', 'frame_px', 'ncols', 'n0', 'epi_warps', 'nbuf', 'tiles_x', 'tiles_y', 'tiles_t', 'total_tiles', 'ks', 'stages',
+          'wt', 'wtb', 'thb', 'frame_px', 'ncols', 'tiles_x', 'tiles_y', 'tiles_t', 'total_tiles', 'ks', 'stages',
           'a_resident', 'a_stage', 'b_step', 'b_bytes', 'b_box', 'stage_bytes', 'ostride', 'hos', 'wos']
 
 
@@ -58,8 +58,9 @@ def emulate(X, A, q, n, groups, ck, cm, garbage):
     os_ = q['ostride']
     cpad = q['kc'] * 16
     assert fpx == thb * wtb and q['b_box'] == 2 * tt * fpx * 16 and q['b_bytes'] >= q['b_box'] and q['b_bytes'] % 128 == 0
-    assert ncols % 16 == 0 and 16 <= ncols <= 512 and (q['nbuf'] == 2) == (ncols <= 256) and wtb <= 128 and thb <= 256 and tt <= 256
-    assert q['stages'] >= 2 and q['stages'] * q['stage_bytes'] + q['epi_warps'] * 32 * 33 * 4 + 512 + 128 <= 227 * 1024
+    assert ncols % 16 == 0 and 16 <= ncols <= 256 and wtb <= 128 and thb <= 256 and tt <= 256
+    assert q['stages'] >= 2 and q['stages'] * q['stage_bytes'] + 128 <= 227 * 1024
+    mma_cols = -(-ncols // 64) * 64                         # the MMAs run in chunks of 64 columns; columns >= ncols are dropped
     kchunks = -(-q['kc'] // q['ks'])
     if q['a_resident']:
         assert q['stages'] % (kt * kchunks) == 0 and groups == 1 and q['mt'] == 1
@@ -78,7 +79,7 @@ def emulate(X, A, q, n, groups, ck, cm, garbage):
         Xp = np.zeros((cpad, T, H, W))
         Xp[:ck] = X[nn, g * ck:(g + 1) * ck]
         per = rows_per_quadrant(cm - mti * 128)
-        D = np.zeros((128, ncols))
+        D = np.zeros((128, mma_cols))
         for ktap in range(kt):
             for kcix in range(kchunks):
                 k0 = kcix * q['ks']
@@ -110,9 +111,9 @@ def emulate(X, A, q, n, groups, ck, cm, garbage):
                                 kv = min(16, ck - kk)
                                 if kv > 0:
                                     Am[row_of_channel(ch, per), :kv] = A[g, mti * 128 + ch, kk:kk + kv, ktap, ky, kx]
-                            idx = j * step_px + (np.arange(16) // 8)[None, :] * blk_px + np.arange(ncols)[:, None] + ky * wtb + kx
+                            idx = j * step_px + (np.arange(16) // 8)[None, :] * blk_px + np.arange(mma_cols)[:, None] + ky * wtb + kx
                             assert idx.max() < stage_b_px, 'tap read past the stage buffer'
-                            Bm = smem[idx, (np.arange(16) % 8)[None, :]]            # [ncols][16]
+                            Bm = smem[idx, (np.arange(16) % 8)[None, :]]            # [mma_cols][16]
                             D += Am @ Bm.T
         for qd in range(4):
             m0 = mti * 128 + qd * per

@@ -82,7 +82,7 @@ def emulate(x, dy, cin, cout, groups, k3, pad3, q, garbage):
     a_px, b_px = q['a_stage'] // 16, q['b_stage'] // 16
     assert a_px == ablk * rh * ps and b_px == (NT // 8) * (rh + khc - 1) * ps
     assert q['stages'] >= 2 and q['stages'] * q['stage_bytes'] + q['tail_bytes'] + 128 <= q['smem'] <= 227 * 1024
-    assert khc * kw * NT <= 512 and rh + khc - 1 <= 256 and ps <= 128 and ablk <= 16 and NT // 8 <= 256
+    assert khc * kw * NT <= 256 and NT % 32 == 0 and rh + khc - 1 <= 256 and ps <= 128 and ablk <= 16 and NT // 8 <= 256
     smem_px = q['stages'] * stage_px + tail_px
     dw = np.zeros((groups * cout, cin, kt, kh, kw))
     rblocks = -(-Ho // rh)
@@ -169,7 +169,7 @@ def test_wgrad_kernel_addressing_replayed_on_cpu(case, dtype_code, monkeypatch):
         q = plan(dtype_code, n, groups, cin, cout, T, H, W, *k3, *pad3)
         if q['pointwise']:
             continue
-        assert q['khc'] == (k3[1] if (fold and k3[1] > 1 and cin <= 64) else 1)
+        assert q['khc'] == (k3[1] if (fold and k3[1] > 1 and cin <= 64 and k3[1] * k3[2] * 32 <= 256) else 1)
         assert q['ablk'] == (-(-cout // 16) * 2 if (compact and cout < 128) else 16)
         assert q['mrows'] == (64 if (compact and cout <= 64) else 128)
         g = torch.Generator().manual_seed(5)
@@ -185,8 +185,8 @@ def test_wgrad_kernel_addressing_replayed_on_cpu(case, dtype_code, monkeypatch):
 
 
 def test_wgrad_plans_of_the_lowres_networks_fit_the_hardware(monkeypatch):
-    """Every conv3d signature of one low-res G+D pass (workloads/lres_step.json), batch 8: the plan's shared memory, TMEM
-    columns and TMA boxes are inside the limits, and the few-channel layers are folded."""
+    """Every conv3d signature of one low-res G+D pass (workloads/lres_step.json), batch 8: the plan's shared memory, register
+    accumulator columns and TMA boxes are inside the limits, and the few-channel layers are folded where their accumulators fit."""
     import json
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     wl = json.load(open(os.path.join(root, 'workloads', 'lres_step.json')))
@@ -201,6 +201,6 @@ def test_wgrad_plans_of_the_lowres_networks_fit_the_hardware(monkeypatch):
             continue
         seen += 1
         assert q['smem'] <= 227 * 1024 and q['stages'] >= 2, (c, q)
-        assert q['khc'] * ws[4] * q['nt'] <= 512 and q['rh'] + q['khc'] - 1 <= 256 and q['ps'] <= 128, (c, q)
-        assert q['khc'] == (ws[3] if ws[3] > 1 and ws[1] <= 32 else 1), (c, q)
+        assert q['khc'] * ws[4] * q['nt'] <= 256 and q['nt'] % 32 == 0 and q['rh'] + q['khc'] - 1 <= 256 and q['ps'] <= 128, (c, q)
+        assert q['khc'] == (ws[3] if ws[3] > 1 and ws[1] <= 32 and ws[3] * ws[4] * 32 <= 256 else 1), (c, q)
     assert seen >= 10

@@ -1,4 +1,4 @@
-"""Timing of the TMA-fed tcgen05 convolution engine against cuDNN (torch.nn.functional / aten::convolution_backward) on
+"""Timing of the TMA-fed wgmma convolution engine against cuDNN (torch.nn.functional / aten::convolution_backward) on
 the convolution shapes of the two training configurations. CUDA events, L2 flushed, median of 7.
     python tools/bench_convnd.py [filter] > profiles/r02_convnd.txt"""
 import math

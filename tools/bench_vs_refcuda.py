@@ -1,5 +1,5 @@
 """Per-op timing of this repository's CUDA ops NEXT TO the reference's own CUDA ops (oracle/_ref, built unmodified for
-sm_100a by oracle/build_ref.py) on the same B200, same inputs, at the full sizes of the two training configurations
+sm_90a by oracle/build_ref.py) on the same H100, same inputs, at the full sizes of the two training configurations
 (lres per-GPU batch 8; sres NT = 64). Forward, and forward+backward through autograd (dx [+db]) -- the public API on
 both sides. CUDA events, L2 flushed between iterations, median of 10.
 

@@ -16,5 +16,5 @@ for n in fl:filtered_lrelu_v3 wgrad:conv_wgrad_v2 igemm:conv_igemm adam:adam_ste
   src=${n%%:*}; dst=${n##*:}
   [ -f $O/r_$src.ncu-rep ] && python tools/ncu_summary.py $O/r_$src.ncu-rep > profiles/${R}_ncu_$dst.md
 done
-cuobjdump -sass long-video-gan_b200/liblvg_ops.so | grep -oE "\b(UTCHMMA|UTCQMMA|UTCBAR|UTMALDG|UTMASTG|UBLKCP|LDTM|STTM|UTCCP|FFMA2|FMUL2|FHADD|LDS\.128|STS\.128)\b[.A-Z0-9_]*" | sed 's/\..*//' | sort | uniq -c | sort -rn > profiles/${R}_sass_mnemonics.txt
+cuobjdump -sass long-video-gan_b200/liblvg_ops.so | grep -oE "\b(HGMMA|WARPGROUP|UTMALDG|UTMASTG|UBLKCP|SYNCS|FFMA|LDS\.128|STS\.128)\b[.A-Z0-9_]*" | sed 's/\..*//' | sort | uniq -c | sort -rn > profiles/${R}_sass_mnemonics.txt
 ls -la profiles | tail -25
