@@ -277,6 +277,28 @@ int lvg_convnd_backward(const void* x, const void* dy, const void* w, void* dx, 
                         int stride, void* workspace, int64_t workspace_bytes, void* stream);
 
 /*
+ * Modulated convolution with one shared weight (groups = 1, stride 1), fp16 or fp32 (bf16 hi/lo split):
+ *   y[n][co][ot] = d[n][co][ot] * sum_{ci,taps} w[co][ci][taps] * a[n][ci][t] * x[n][ci][t][...]
+ * -- the style modulation / demodulation of modulated_conv2d (generator_sres.py:28-67, as N*T samples of 2-D images) and
+ * temporal_modulated_conv3d (generator_lres.py:83-125) without per-sample weights. a [n][cin][t] (required) scales x while
+ * it is re-tiled, d [n][cout][to] (NULL = none) the fp32 accumulators; t = 1 for 2-D. Argument order as lvg_convnd_fprop
+ * with groups = 1. `workspace`: lvg_modconv_workspace bytes (forward and backward), 16-byte aligned; -1 / LVG_UNSUPPORTED
+ * outside the envelope of lvg_convnd_backward (kh * kw <= 9, kw <= 3, kt <= 7, 0 <= pad <= k - 1).
+ * Backward: dx = a * conv^T(d * dy, w), dw = sum_n conv_w(a * x, d * dy) (NULL = skipped), da[n][ci][t] = sum_hw
+ * conv^T(d * dy, w) * x (NULL = skipped), dyy[n][co][ot] = sum_hw dy * y (NULL = skipped; needs y and d; the gradient of d
+ * is dyy / d). d * dy is re-tiled once for both gradients when cout < 128 or a multiple of 128.
+ */
+int64_t lvg_modconv_workspace(int dtype, int n, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw,
+                              int pad_t, int pad_h, int pad_w);
+int lvg_modconv_fprop(const void* x, const void* w, const float* a, const float* d, void* y, int dtype, int n, int cin,
+                      int cout, int t, int h, int wd, int kt, int kh, int kw, int pad_t, int pad_h, int pad_w,
+                      void* workspace, int64_t workspace_bytes, void* stream);
+int lvg_modconv_backward(const void* x, const void* w, const float* a, const float* d, const void* y, const void* dy,
+                         void* dx, void* dw, float* da, float* dyy, int dtype, int n, int cin, int cout, int t, int h,
+                         int wd, int kt, int kh, int kw, int pad_t, int pad_h, int pad_w, void* workspace,
+                         int64_t workspace_bytes, void* stream);
+
+/*
  * Depthwise long FIR along the last axis (cross-correlation, no padding), fp32:
  *   y[n][g][t] = sum_k w[g][k] * x[n][g][t + k],   x [n][groups][lin], w [groups][k], y [n][groups][lin - k + 1]
  * -- BlurredNoise.blur of the low-res generator: F.conv1d(noise, blur_filters [128, 1, 5000], groups = 128)

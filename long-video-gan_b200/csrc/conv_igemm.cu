@@ -28,6 +28,7 @@
 // Roles (384 threads): warp 0 = TMA producer (one lane), warpgroups 1-2 = wgmma consumers, each with its 64 accumulator rows
 // in registers and its own epilogue ([bias, lrelu, gain, clamp] -> NC(T)HW global). Stages hand over through full/empty mbarriers.
 
+#include <algorithm>
 #include <cuda.h>
 #include <stdlib.h>
 #include <cuda_bf16.h>
@@ -82,6 +83,7 @@ struct IgemmParams {
     int a_stage, b_step, b_bytes, b_box, stage_bytes;    // bytes: A per stage, B stride per k-step / per pair of blocks, TMA payload of a pair, whole stage
     int64_t y_cs;                // output channel stride (= to*hos*wos)
     int ostride, hos, wos;       // output decimation (strided convolution): only rows / columns divisible by ostride are stored
+    const float* out_scale;      // per-(instance, output channel, output frame) factor [inst][cout][to] on the accumulator, or nullptr
 };
 
 // ------------------------------------------------------------------------------------------------ re-tiling passes
@@ -93,9 +95,11 @@ __device__ __forceinline__ float bf16_val(unsigned short b) { return __uint_as_f
 // 16-byte writes. SPLIT: fp32 in, bf16 hi blocks [0, cblk) and lo blocks [cblk, 2 cblk) out.
 // Dilation (gradients of strided convolutions): input pixel (t, i, j) of an ih x iw image lands at (t, i*dil, j*dil) of
 // the oh x ow output image, which the caller has zeroed.
-struct PackGeom { int64_t thw_in, thw_out; int ih, iw, oh, ow, dil; };
+// `scale` (modulated convolutions): every element is multiplied by scale[instance][channel][frame] in fp32 before it is
+// rounded to fp16 / split into bf16 halves; nullptr = the elements are copied as they are.
+struct PackGeom { int64_t thw_in, thw_out; int ih, iw, oh, ow, dil; const float* scale; };
 
-template <class TIn, bool SPLIT>
+template <class TIn, bool SPLIT, bool SCALE>
 __global__ void __launch_bounds__(256) conv_pack_act_kernel(const TIn* __restrict__ x, uint4* __restrict__ y, int64_t inst, int c,
                                                              int cblk, PackGeom gm)
 {
@@ -109,6 +113,13 @@ __global__ void __launch_bounds__(256) conv_pack_act_kernel(const TIn* __restric
         const int64_t in = r / cblk;
         const int c0 = blk * 8;
         const TIn* src = x + ((int64_t)in * c + c0) * thw + p;
+        const float* sc = nullptr;           // this pixel's factor of channel c0 (channel stride: frames)
+        int64_t frames = 1;
+        if constexpr (SCALE) {
+            const int64_t hw = (int64_t)gm.ih * gm.iw;
+            frames = thw / hw;
+            sc = gm.scale + ((int64_t)in * c + c0) * frames + p / hw;
+        }
         int64_t po = p;
         if (gm.dil > 1) {
             const int j = (int)(p % gm.iw);
@@ -121,12 +132,18 @@ __global__ void __launch_bounds__(256) conv_pack_act_kernel(const TIn* __restric
             alignas(16) unsigned short v[8];
 #pragma unroll
             for (int j = 0; j < 8; j++) v[j] = (c0 + j < c) ? __half_as_ushort(__ldg(reinterpret_cast<const __half*>(src) + (int64_t)j * thw)) : (unsigned short)0;
+            if constexpr (SCALE) {
+#pragma unroll
+                for (int j = 0; j < 8; j++)
+                    if (c0 + j < c) v[j] = __half_as_ushort(__float2half_rn(__half2float(__ushort_as_half(v[j])) * __ldg(sc + j * frames)));
+            }
             y[((int64_t)in * nblk + blk) * gm.thw_out + po] = *reinterpret_cast<const uint4*>(v);
         } else {
             alignas(16) unsigned short hi[8], lo[8];
 #pragma unroll
             for (int j = 0; j < 8; j++) {
-                const float f = (c0 + j < c) ? __ldg(reinterpret_cast<const float*>(src) + (int64_t)j * thw) : 0.f;
+                float f = (c0 + j < c) ? __ldg(reinterpret_cast<const float*>(src) + (int64_t)j * thw) : 0.f;
+                if constexpr (SCALE) { if (c0 + j < c) f *= __ldg(sc + j * frames); }
                 hi[j] = bf16_bits(f);
                 lo[j] = bf16_bits(f - bf16_val(hi[j]));
             }
@@ -137,17 +154,22 @@ __global__ void __launch_bounds__(256) conv_pack_act_kernel(const TIn* __restric
 }
 
 // launches the re-tiling of one activation tensor (zeroing the target first when it is dilated)
-int pack_act(const void* x, void* x8, int split, int64_t inst, int c, int cblk, int t, int ih, int iw, int oh, int ow, int dil, cudaStream_t s)
+int pack_act(const void* x, void* x8, int split, int64_t inst, int c, int cblk, int t, int ih, int iw, int oh, int ow, int dil, cudaStream_t s,
+             const float* scale = nullptr)
 {
     PackGeom gm;
     gm.thw_in = (int64_t)t * ih * iw; gm.thw_out = (int64_t)t * oh * ow; gm.ih = ih; gm.iw = iw; gm.oh = oh; gm.ow = ow; gm.dil = dil;
+    gm.scale = scale;
     if (dil > 1) LVG_CUDA(cudaMemsetAsync(x8, 0, (size_t)(inst * (split ? 2 : 1) * cblk * gm.thw_out * 16), s));
     const int64_t total = inst * cblk * gm.thw_in;
     int64_t blocks = (total + 255) / 256;
     const int64_t cap = (int64_t)num_sms() * 64;
     if (blocks > cap) blocks = cap;
-    if (split) conv_pack_act_kernel<float, true><<<(unsigned)blocks, 256, 0, s>>>((const float*)x, (uint4*)x8, inst, c, cblk, gm);
-    else conv_pack_act_kernel<__half, false><<<(unsigned)blocks, 256, 0, s>>>((const __half*)x, (uint4*)x8, inst, c, cblk, gm);
+    // (the scaled variants are separate instantiations: the unscaled re-tiling stays the plain copy it was)
+    if (split && scale) conv_pack_act_kernel<float, true, true><<<(unsigned)blocks, 256, 0, s>>>((const float*)x, (uint4*)x8, inst, c, cblk, gm);
+    else if (split) conv_pack_act_kernel<float, true, false><<<(unsigned)blocks, 256, 0, s>>>((const float*)x, (uint4*)x8, inst, c, cblk, gm);
+    else if (scale) conv_pack_act_kernel<__half, false, true><<<(unsigned)blocks, 256, 0, s>>>((const __half*)x, (uint4*)x8, inst, c, cblk, gm);
+    else conv_pack_act_kernel<__half, false, false><<<(unsigned)blocks, 256, 0, s>>>((const __half*)x, (uint4*)x8, inst, c, cblk, gm);
     LVG_LAUNCH_CHECK();
     return LVG_OK;
 }
@@ -315,7 +337,7 @@ __device__ __forceinline__ TileCoord decode_tile(const IgemmParams& p, int64_t L
 // Roles (384 threads): warp 0 = TMA producer (one lane); warpgroups 1 and 2 = MMA + epilogue for accumulator rows 0-63 and
 // 64-127 of the weight images. Each consumer holds its 64 x ncols fp32 accumulator in registers (ncols <= 256, issued as
 // chunks of 64 columns) and releases a stage once the wgmma group that read it has completed.
-template <bool BF16, int NCH>
+template <bool BF16, int NCH, bool OSCALE>
 __global__ void __launch_bounds__(kIgemmThreads, 1) conv_igemm_kernel(const __grid_constant__ CUtensorMap tmx, const IgemmParams p)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -420,6 +442,7 @@ __global__ void __launch_bounds__(kIgemmThreads, 1) conv_igemm_kernel(const __gr
             int64_t chbase[2];
             float bias[2];
             bool rok[2];
+            const float* osc[2];
 #pragma unroll
             for (int h = 0; h < 2; h++) {
                 const int ch = m_channel_of_row(cw * 64 + wq * 16 + lane / 4 + 8 * h, per);
@@ -427,6 +450,7 @@ __global__ void __launch_bounds__(kIgemmThreads, 1) conv_igemm_kernel(const __gr
                 rok[h] = ch < kBM && co < p.cout;
                 bias[h] = (p.bias != nullptr && rok[h]) ? __ldg(p.bias + (int64_t)(c.inst % p.wgroups) * p.cout + co) : 0.f;
                 chbase[h] = ((int64_t)c.inst * p.cout + co) * p.y_cs;
+                osc[h] = OSCALE ? p.out_scale + ((int64_t)c.inst * p.cout + co) * p.to : nullptr;
             }
 #pragma unroll
             for (int ch = 0; ch < NCH; ch++) {
@@ -452,6 +476,7 @@ __global__ void __launch_bounds__(kIgemmThreads, 1) conv_igemm_kernel(const __gr
                         for (int h = 0; h < 2; h++) {
                             if (!rok[h]) continue;
                             float v = acc[ch][4 * j + 2 * h + e];
+                            if constexpr (OSCALE) v *= __ldg(osc[h] + ot);
                             if (p.act) {
                                 v += bias[h];
                                 if (p.act == 2) v = v < 0.f ? v * p.alpha : v;
@@ -540,8 +565,10 @@ thread_local IgemmParams* g_plan_only = nullptr;
 int run_igemm(const void* x, const void* w, void* y, int dtype, int n, int groups, int ck, int cm, int t, int h, int wd, int kt, int kh,
               int kw, int pad_t, int pad_h, int pad_w, int64_t w_gs, int64_t w_sm, int64_t w_sk, int flip, const float* bias, int act,
               float alpha, float gain, float clamp, int xin_h, int xin_w, int dil, int ostride, const unsigned char* x8_pre, void* workspace,
-              int64_t workspace_bytes, cudaStream_t s)
+              int64_t workspace_bytes, cudaStream_t s, const float* in_scale = nullptr, const float* out_scale = nullptr)
 {
+    // `in_scale` [n][ck][t] multiplies x while it is re-tiled (not with x8_pre: the caller re-tiled it), `out_scale`
+    // [n][cm][to] the accumulators in the epilogue (groups == 1: instance = sample)
     // `x8_pre` != nullptr: x is already re-tiled there (lvg_convnd_backward shares dy8 with the weight gradient); the workspace
     // then only holds the packed weights
     const int split = dtype == LVG_F32 ? 1 : 0;
@@ -561,7 +588,7 @@ int run_igemm(const void* x, const void* w, void* y, int dtype, int n, int group
 
     IgemmParams p;
     memset(&p, 0, sizeof(p));
-    p.wp = wp; p.y = y; p.bias = bias; p.act = act; p.alpha = alpha; p.gain = gain; p.clamp = clamp;
+    p.wp = wp; p.y = y; p.bias = bias; p.act = act; p.alpha = alpha; p.gain = gain; p.clamp = clamp; p.out_scale = out_scale;
     p.out_f32 = split; p.bf16 = split;
     p.wgroups = groups; p.cout = cm; p.mt = g.mt; p.kc = g.kc; p.nblk = g.nblk;
     p.nimg = g.nimg; p.lo_blk = g.cblk;
@@ -639,7 +666,7 @@ int run_igemm(const void* x, const void* w, void* y, int dtype, int n, int group
 
     // re-tile the operands
     {
-        const int rc = x8_pre ? LVG_OK : pack_act(x, x8, split, inst, ck, g.cblk, t, xin_h, xin_w, h, wd, dil, s);
+        const int rc = x8_pre ? LVG_OK : pack_act(x, x8, split, inst, ck, g.cblk, t, xin_h, xin_w, h, wd, dil, s, in_scale);
         if (rc) return rc;
         const int64_t wblocks = (int64_t)groups * g.mt * g.kc;
         LVG_REQUIRE(wblocks < (1ll << 31), "convnd: too many weight tiles");
@@ -679,10 +706,13 @@ int run_igemm(const void* x, const void* w, void* y, int dtype, int n, int group
         if (rc) return rc;
     }
     const size_t smem = (size_t)p.stages * p.stage_bytes + 128;
-    void (*const kerns[2][kMaxChunks])(const CUtensorMap, const IgemmParams) = {
-        {conv_igemm_kernel<false, 1>, conv_igemm_kernel<false, 2>, conv_igemm_kernel<false, 3>, conv_igemm_kernel<false, 4>},
-        {conv_igemm_kernel<true, 1>, conv_igemm_kernel<true, 2>, conv_igemm_kernel<true, 3>, conv_igemm_kernel<true, 4>}};
-    void (*kern)(const CUtensorMap, const IgemmParams) = kerns[split][(p.ncols + 63) / 64 - 1];
+    // (the output-scaled epilogue is a separate instantiation: the unscaled one stays as it was)
+    void (*const kerns[2][2][kMaxChunks])(const CUtensorMap, const IgemmParams) = {
+        {{conv_igemm_kernel<false, 1, false>, conv_igemm_kernel<false, 2, false>, conv_igemm_kernel<false, 3, false>, conv_igemm_kernel<false, 4, false>},
+         {conv_igemm_kernel<true, 1, false>, conv_igemm_kernel<true, 2, false>, conv_igemm_kernel<true, 3, false>, conv_igemm_kernel<true, 4, false>}},
+        {{conv_igemm_kernel<false, 1, true>, conv_igemm_kernel<false, 2, true>, conv_igemm_kernel<false, 3, true>, conv_igemm_kernel<false, 4, true>},
+         {conv_igemm_kernel<true, 1, true>, conv_igemm_kernel<true, 2, true>, conv_igemm_kernel<true, 3, true>, conv_igemm_kernel<true, 4, true>}}};
+    void (*kern)(const CUtensorMap, const IgemmParams) = kerns[out_scale != nullptr][split][(p.ncols + 63) / 64 - 1];
     LVG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const char* cta_env = getenv("LVG_CONV_CTAS");          // experiments: fewer persistent CTAs than SMs
     const int max_ctas = cta_env ? atoi(cta_env) : num_sms();
@@ -1042,7 +1072,7 @@ WgradPlan wgrad_plan(int dtype, int n, int groups, int cin, int cout, int t, int
 // the weight-gradient launch; `dy8_pre` != nullptr: dy is already re-tiled (the tensor the input gradient of the same call read)
 int run_wgrad(const void* x, const void* dy, void* dw, int dtype, int n, int groups, int cin, int cout, int t, int h, int wd, int kt, int kh,
               int kw, int pad_t, int pad_h, int pad_w, int stride, const unsigned char* dy8_pre, void* workspace, int64_t workspace_bytes,
-              cudaStream_t s)
+              cudaStream_t s, const float* x_scale = nullptr, const float* dy_scale = nullptr)
 {
     const int to = t + 2 * pad_t - kt + 1, ho = h + 2 * pad_h - kh + 1, wo = wd + 2 * pad_w - kw + 1;
     const WgradPlan q = wgrad_plan(dtype, n, groups, cin, cout, t, h, wd, to, ho, wo, kt, kh, kw);
@@ -1057,9 +1087,10 @@ int run_wgrad(const void* x, const void* dy, void* dw, int dtype, int n, int gro
     const int64_t thw_a = (int64_t)to * ho * wo, thw_b = (int64_t)t * h * wd;
     {
         // dy of a strided convolution is spread over every stride-th pixel of the stride-1 output grid (zeros between)
-        int rc = dy8_pre ? LVG_OK : pack_act(dy, dy8, q.split, inst, cout, q.cpad_a / 8, to, (ho - 1) / stride + 1, (wo - 1) / stride + 1, ho, wo, stride, s);
+        int rc = dy8_pre ? LVG_OK : pack_act(dy, dy8, q.split, inst, cout, q.cpad_a / 8, to, (ho - 1) / stride + 1, (wo - 1) / stride + 1, ho, wo, stride, s,
+                                             dy_scale);
         if (rc) return rc;
-        rc = pack_act(x, x8, q.split, inst, cin, q.cpad_b / 8, t, h, wd, h, wd, 1, s);
+        rc = pack_act(x, x8, q.split, inst, cin, q.cpad_b / 8, t, h, wd, h, wd, 1, s, x_scale);   // x_scale [n][cin][t]: x is modulated
         if (rc) return rc;
     }
     WgradV2Params p;
@@ -1273,4 +1304,175 @@ extern "C" int lvg_convnd_backward(const void* x, const void* dy, const void* w,
     // (stream order: the weight gradient's re-tiling of x overwrites the packed weights only after the input gradient read them)
     return run_wgrad(x, dy, dw, dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, stride, dy8, rest,
                      workspace_bytes - dy8_room, s);
+}
+
+// =================================================================================================
+// Modulated convolution  y = d (.) conv(a (.) x, w)  with one weight tensor shared by every sample (groups = 1, stride 1):
+// a [n][cin][t] scales x while it is re-tiled (conv_pack_act_kernel), d [n][cout][to] the accumulators in the epilogue
+// (conv_igemm_kernel). The per-sample weights of the reference's grouped formulation (generator_sres.py:44-60) and the
+// modulated activation copies (generator_lres.py:117-123) are never formed.
+// Backward: dy is re-tiled with the factor d for both gradients; dgrad writes dx' = conv^T(d dy, w) into dx, and one
+// streaming pass (modconv_rowdot_kernel) turns it into dx = a dx' while it sums da = sum_hw dx' x. The gradient of d comes
+// from sum_hw dy y (= d sum_hw dy conv(a x, w)), a second pass of the same kernel; the caller divides by d.
+
+namespace lvg {
+namespace {
+
+__device__ __forceinline__ float to_f32(float v) { return v; }
+__device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
+__device__ __forceinline__ void from_f32(float& o, float v) { o = v; }
+__device__ __forceinline__ void from_f32(__half& o, float v) { o = __float2half_rn(v); }
+
+// r[row] = sum_i u[row][i] * v[row][i] over rows of `len` contiguous elements (fp32 accumulation); scale != nullptr:
+// u[row][i] *= scale[row] in place (after it was read). One CTA per row; VEC elements per 16-byte load when rows are aligned.
+template <class T, int VEC>
+__global__ void __launch_bounds__(256) modconv_rowdot_kernel(T* __restrict__ u, const T* __restrict__ v, const float* __restrict__ scale,
+                                                             float* __restrict__ r, int64_t rows, int64_t len)
+{
+    __shared__ float red[8];
+    for (int64_t row = blockIdx.x; row < rows; row += gridDim.x) {
+        T* ur = u + row * len;
+        const T* vr = v + row * len;
+        const float sc = scale != nullptr ? __ldg(scale + row) : 1.f;
+        float acc = 0.f;
+        for (int64_t i = (int64_t)threadIdx.x * VEC; i < len; i += 256 * VEC) {
+            alignas(16) T ue[VEC], ve[VEC];
+            if constexpr (VEC > 1) {
+                *reinterpret_cast<uint4*>(ue) = *reinterpret_cast<const uint4*>(ur + i);
+                *reinterpret_cast<uint4*>(ve) = __ldg(reinterpret_cast<const uint4*>(vr + i));
+            } else {
+                ue[0] = ur[i];
+                ve[0] = vr[i];
+            }
+#pragma unroll
+            for (int j = 0; j < VEC; j++) {
+                const float uf = to_f32(ue[j]);
+                acc += uf * to_f32(ve[j]);
+                from_f32(ue[j], uf * sc);
+            }
+            if (scale != nullptr) {
+                if constexpr (VEC > 1) *reinterpret_cast<uint4*>(ur + i) = *reinterpret_cast<const uint4*>(ue);
+                else ur[i] = ue[0];
+            }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+        if (threadIdx.x % 32 == 0) red[threadIdx.x / 32] = acc;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            float s = 0.f;
+            for (int k = 0; k < 8; k++) s += red[k];
+            if (r != nullptr) r[row] = s;
+        }
+        __syncthreads();
+    }
+}
+
+int modconv_rowdot(void* u, const void* v, const float* scale, float* r, int dtype, int64_t rows, int64_t len, cudaStream_t s)
+{
+    int64_t blocks = rows;
+    const int64_t cap = (int64_t)num_sms() * 8;
+    if (blocks > cap) blocks = cap;
+    if (blocks < 1) return LVG_OK;
+    const int es = dtype == LVG_F32 ? 4 : 2;
+    const bool vec = aligned16(u) && aligned16(v) && (len * es) % 16 == 0;
+    if (dtype == LVG_F32) {
+        if (vec) modconv_rowdot_kernel<float, 4><<<(unsigned)blocks, 256, 0, s>>>((float*)u, (const float*)v, scale, r, rows, len);
+        else modconv_rowdot_kernel<float, 1><<<(unsigned)blocks, 256, 0, s>>>((float*)u, (const float*)v, scale, r, rows, len);
+    } else {
+        if (vec) modconv_rowdot_kernel<__half, 8><<<(unsigned)blocks, 256, 0, s>>>((__half*)u, (const __half*)v, scale, r, rows, len);
+        else modconv_rowdot_kernel<__half, 1><<<(unsigned)blocks, 256, 0, s>>>((__half*)u, (const __half*)v, scale, r, rows, len);
+    }
+    LVG_LAUNCH_CHECK();
+    return LVG_OK;
+}
+
+// forward and backward run on the engine alone (never the streaming 1x1x1 kernels, which take no factors)
+bool modconv_in_envelope(int dtype, int n, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw, int pad_t, int pad_h, int pad_w)
+{
+    return cin >= 1 && cout >= 1 && pad_t <= kt - 1 && pad_h <= kh - 1 && pad_w <= kw - 1 &&
+           wgrad_in_envelope(dtype, n, 1, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, 1);
+}
+
+inline int64_t round256(int64_t b) { return (b + 255) / 256 * 256; }
+
+}  // namespace
+}  // namespace lvg
+
+extern "C" int64_t lvg_modconv_workspace(int dtype, int n, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw, int pad_t, int pad_h,
+                                         int pad_w)
+{
+    if (!modconv_in_envelope(dtype, n, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w)) return -1;
+    const int split = dtype == LVG_F32;
+    const int taps = kt * kh * kw;
+    const int to = t + 2 * pad_t - kt + 1, ho = h + 2 * pad_h - kh + 1, wo = wd + 2 * pad_w - kw + 1;
+    const Geometry gf = geometry(split, n, 1, cin, cout, (int64_t)t * h * wd, taps);          // forward
+    const Geometry gd = geometry(split, n, 1, cout, cin, (int64_t)to * ho * wo, taps);        // input gradient
+    const WgradPlan q = wgrad_plan(dtype, n, 1, cin, cout, t, h, wd, to, ho, wo, kt, kh, kw);
+    const int64_t sep = std::max(std::max(gf.act_bytes + gf.w_bytes, gd.act_bytes + gd.w_bytes), q.a_bytes + q.b_bytes + q.part_bytes);
+    const int64_t shared = round256(gd.act_bytes) + std::max(round256(gd.w_bytes) + 256, round256(q.b_bytes) + q.part_bytes + 768);
+    return std::max(sep, shared) + 1024;
+}
+
+extern "C" int lvg_modconv_fprop(const void* x, const void* w, const float* a, const float* d, void* y, int dtype, int n, int cin, int cout, int t,
+                                 int h, int wd, int kt, int kh, int kw, int pad_t, int pad_h, int pad_w, void* workspace, int64_t workspace_bytes,
+                                 void* stream)
+{
+    LVG_REQUIRE(x && w && a && y, "modconv_fprop: x, w, a, y must not be NULL");
+    if (!modconv_in_envelope(dtype, n, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w)) {
+        set_error("modconv_fprop: outside the tensor-core kernel's envelope");
+        return LVG_UNSUPPORTED;
+    }
+    const int taps = kt * kh * kw;
+    return run_igemm(x, w, y, dtype, n, 1, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, (int64_t)cout * cin * taps, (int64_t)cin * taps,
+                     taps, 0, nullptr, 0, 0.f, 1.f, -1.f, h, wd, 1, 1, nullptr, workspace, workspace_bytes, (cudaStream_t)stream, a, d);
+}
+
+extern "C" int lvg_modconv_backward(const void* x, const void* w, const float* a, const float* d, const void* y, const void* dy, void* dx, void* dw,
+                                    float* da, float* dyy, int dtype, int n, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw,
+                                    int pad_t, int pad_h, int pad_w, void* workspace, int64_t workspace_bytes, void* stream)
+{
+    LVG_REQUIRE(x && w && a && dy && dx, "modconv_backward: x, w, a, dy, dx must not be NULL");
+    LVG_REQUIRE(!dyy || (y && d), "modconv_backward: sum(dy * y) needs y and d");
+    LVG_REQUIRE(workspace && aligned16(workspace), "modconv_backward: workspace must be 16-byte aligned and not NULL");
+    if (!modconv_in_envelope(dtype, n, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w)) {
+        set_error("modconv_backward: outside the tensor-core kernel's envelope");
+        return LVG_UNSUPPORTED;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    const int split = dtype == LVG_F32 ? 1 : 0;
+    const int taps = kt * kh * kw;
+    const int to = t + 2 * pad_t - kt + 1, ho = h + 2 * pad_h - kh + 1, wo = wd + 2 * pad_w - kw + 1;
+    int rc;
+    if (dyy) {
+        rc = modconv_rowdot(const_cast<void*>(dy), y, nullptr, dyy, dtype, (int64_t)n * cout * to, (int64_t)ho * wo, s);
+        if (rc) return rc;
+    }
+    const Geometry gd = geometry(split, n, 1, cout, cin, (int64_t)to * ho * wo, taps);
+    const int64_t w_gs = (int64_t)cout * cin * taps;
+    if (wgrad_cpad_a(cout) == round_up(cout, 16)) {
+        // one re-tiling of d dy serves both gradients (layout as lvg_convnd_backward: [dy8][dgrad weights | x8, partial sums])
+        const int64_t dy8_room = round256(gd.act_bytes);
+        const int64_t wp_room = round256(gd.w_bytes) + 256;
+        LVG_REQUIRE(workspace_bytes >= dy8_room + wp_room, "modconv_backward: workspace too small");
+        unsigned char* dy8 = reinterpret_cast<unsigned char*>(workspace);
+        unsigned char* rest = dy8 + dy8_room;
+        rc = pack_act(dy, dy8, split, n, cout, gd.cblk, to, ho, wo, ho, wo, 1, s, d);
+        if (rc) return rc;
+        rc = run_igemm(dy, w, dx, dtype, n, 1, cout, cin, to, ho, wo, kt, kh, kw, kt - 1 - pad_t, kh - 1 - pad_h, kw - 1 - pad_w, w_gs, taps,
+                       (int64_t)cin * taps, 1, nullptr, 0, 0.f, 1.f, -1.f, ho, wo, 1, 1, dy8, rest, wp_room, s);
+        if (rc) return rc;
+        rc = modconv_rowdot(dx, x, a, da, dtype, (int64_t)n * cin * t, (int64_t)h * wd, s);
+        if (rc) return rc;
+        return dw ? run_wgrad(x, dy, dw, dtype, n, 1, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, 1, dy8, rest, workspace_bytes - dy8_room, s, a)
+                  : LVG_OK;
+    }
+    // output channels that are neither < 128 nor a multiple of 128: the two gradients tile d dy differently, each re-tiles it
+    rc = run_igemm(dy, w, dx, dtype, n, 1, cout, cin, to, ho, wo, kt, kh, kw, kt - 1 - pad_t, kh - 1 - pad_h, kw - 1 - pad_w, w_gs, taps,
+                   (int64_t)cin * taps, 1, nullptr, 0, 0.f, 1.f, -1.f, ho, wo, 1, 1, nullptr, workspace, workspace_bytes, s, d);
+    if (rc) return rc;
+    rc = modconv_rowdot(dx, x, a, da, dtype, (int64_t)n * cin * t, (int64_t)h * wd, s);
+    if (rc) return rc;
+    return dw ? run_wgrad(x, dy, dw, dtype, n, 1, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, 1, nullptr, workspace, workspace_bytes, s, a, d)
+              : LVG_OK;
 }

@@ -73,6 +73,9 @@ _SIGNATURES = {
     'lvg_convnd_wgrad_plan': (_c_int, [_c_int] * 14 + [ctypes.POINTER(_c_int), _c_int]),
     'lvg_convnd_backward_workspace': (_c_i64, [_c_int] * 14),
     'lvg_convnd_backward': (_c_int, [_c_void_p] * 5 + [_c_int] * 15 + [_c_void_p, _c_i64, _c_void_p]),
+    'lvg_modconv_workspace': (_c_i64, [_c_int] * 13),
+    'lvg_modconv_fprop': (_c_int, [_c_void_p] * 5 + [_c_int] * 13 + [_c_void_p, _c_i64, _c_void_p]),
+    'lvg_modconv_backward': (_c_int, [_c_void_p] * 10 + [_c_int] * 13 + [_c_void_p, _c_i64, _c_void_p]),
 }
 
 LVG_UNSUPPORTED = -1
@@ -685,6 +688,61 @@ class ConvNdPlugin:
         if rc == LVG_UNSUPPORTED:
             raise RuntimeError('convnd_backward: ' + self._lib.lvg_last_error().decode())
         return dx, dw
+
+    def _modconv_args(self, x, w, padding):
+        a, sp, k, pad = self._args(tuple(x.shape), tuple(w.shape), padding, 1, x.dtype)
+        del a[2]                                            # groups = 1
+        return a, sp, k, pad
+
+    def modconv_supported(self, x, w, padding):
+        """Inside the envelope of lvg_modconv_fprop / lvg_modconv_backward (given supported(x, w, 1, padding, 1, 1))."""
+        return self._lib.lvg_modconv_workspace(*self._modconv_args(x, w, padding)[0]) >= 0
+
+    @staticmethod
+    def _factor(f, shape, what):
+        if f.dtype != torch.float32 or tuple(f.shape) != tuple(shape):
+            raise RuntimeError(f'{what}: expected a float32 tensor of shape {list(shape)}, got {f.dtype} {list(f.shape)}')
+        return f.contiguous()
+
+    def modconv_fprop(self, x, w, a, d, padding):
+        """y = d * conv(a * x, w), groups = 1, stride 1: a [N, Cin, T] scales x, d [N, Cout, To] (or None) the output;
+        T = To = 1 for 2-D tensors."""
+        x, w = x.contiguous(), w.contiguous()
+        args, sp, k, pad = self._modconv_args(x, w, padding)
+        out_sp = [s + 2 * p - kk + 1 for s, p, kk in zip(sp, pad, k)]
+        a = self._factor(a, (x.shape[0], x.shape[1], sp[0]), 'modconv_fprop: a')
+        if d is not None:
+            d = self._factor(d, (x.shape[0], w.shape[0], out_sp[0]), 'modconv_fprop: d')
+        y = torch.empty([x.shape[0], w.shape[0]] + out_sp[3 - (x.ndim - 2):], dtype=x.dtype, device=x.device)
+        ws = self._workspace(x.device, self._lib.lvg_modconv_workspace(*args))
+        with _DeviceGuard(x):
+            rc = _check(self._lib.lvg_modconv_fprop(_ptr(x), _ptr(w), _ptr(a), _ptr(d), _ptr(y), *args, _ptr(ws), ws.numel(), _stream(x)),
+                        'modconv_fprop')
+        if rc == LVG_UNSUPPORTED:
+            raise RuntimeError('modconv_fprop: ' + self._lib.lvg_last_error().decode())
+        return y
+
+    def modconv_backward(self, x, w, a, d, y, dy, padding, want_dw=True):
+        """Gradients of y = d * conv(a * x, w) in one call: (dx, dw or None, da [N, Cin, T], sum_hw dy * y [N, Cout, To] or
+        None when d is None)."""
+        x, w, dy = x.contiguous(), w.contiguous(), dy.contiguous()
+        args, sp, k, pad = self._modconv_args(x, w, padding)
+        a = self._factor(a, (x.shape[0], x.shape[1], sp[0]), 'modconv_backward: a')
+        dx = torch.empty_like(x)
+        dw = torch.empty_like(w) if want_dw else None
+        da = torch.empty(a.shape, dtype=torch.float32, device=x.device)
+        dyy = None
+        if d is not None:
+            d = self._factor(d, (x.shape[0], w.shape[0], dy.shape[2] if dy.ndim == 5 else 1), 'modconv_backward: d')
+            y = y.contiguous()
+            dyy = torch.empty(d.shape, dtype=torch.float32, device=x.device)
+        ws = self._workspace(x.device, self._lib.lvg_modconv_workspace(*args))
+        with _DeviceGuard(x):
+            rc = _check(self._lib.lvg_modconv_backward(_ptr(x), _ptr(w), _ptr(a), _ptr(d), _ptr(y) if d is not None else None, _ptr(dy), _ptr(dx),
+                                                       _ptr(dw), _ptr(da), _ptr(dyy), *args, _ptr(ws), ws.numel(), _stream(x)), 'modconv_backward')
+        if rc == LVG_UNSUPPORTED:
+            raise RuntimeError('modconv_backward: ' + self._lib.lvg_last_error().decode())
+        return dx, dw, da, dyy
 
 
 _PLUGIN_CLASSES = {
