@@ -22,8 +22,9 @@
 // GEMM view per instance:  D[co][pix] = sum_{kt} sum_{ci} sum_{ky,kx} W[co][ci][kt][ky][kx] * X[ci][t + kt][y + ky][x + kx]
 //   M = 128 output channels (two warpgroups of 64), N = TH x (WT + kw - 1) pixels (<= 256 register columns),
 //   K = 16 channels per MMA; the K loop runs over (kt, 16-channel step), every stage issues kh*kw MMAs (one per tap).
-// Weights are re-tiled per call into 128 x 16 K-major images per (m-tile, k-step, tap) (conv_pack_w_kernel) and arrive
-// with one cp.async.bulk per stage.
+//   GEMMs with M <= 64 run in 64-row mode: M = 64, and the two warpgroups split the N columns.
+// Weights are re-tiled per call into 128 x 16 (64-row mode: 64 x 16) K-major images per (m-tile, k-step, tap)
+// (conv_pack_w_kernel) and arrive with one cp.async.bulk per stage.
 //
 // Roles (384 threads): warp 0 = TMA producer (one lane), warpgroups 1-2 = wgmma consumers, each with its 64 accumulator rows
 // in registers and its own epilogue ([bias, lrelu, gain, clamp] -> NC(T)HW global). Stages hand over through full/empty mbarriers.
@@ -50,15 +51,14 @@ namespace {
 using namespace tc;
 
 constexpr int kBM = 128;
-constexpr int kATile = kBM * 16 * 2;          // one 128 x 16 weight image: 4096 bytes
+constexpr int kATile = kBM * 16 * 2;          // one 128 x 16 weight image: 4096 bytes (64-row mode: 2048)
 constexpr int kIgemmThreads = 384;           // both kernels: a producer warpgroup and two consumer warpgroups
-constexpr int kMaxChunks = 4;                // conv_igemm_kernel: accumulator columns in chunks of 64 (<= 256)
-constexpr int kWgradChunks = 8;              // conv_wgrad_v2_kernel: accumulator columns in chunks of 32 (<= 256)
+constexpr int kWidths = 16;                  // conv_igemm_kernel: MMA widths 16, 32, ..., 256 columns
 constexpr int kMaxStages = 6;
 constexpr int kBSlack = 1024;                // shared memory behind an activation stage that MMAs may read
 
 struct IgemmParams {
-    const unsigned char* wp;     // packed weights [wgroups][mt][kc][taps_all][4096]
+    const unsigned char* wp;     // packed weights [wgroups][mt][kc][taps_all][a_img]
     void* y;
     const float* bias;           // per output channel (group-local index g*cout + co), or nullptr
     int act;                     // 0 = none, 1 = (x + b) * gain clamped, 2 = lrelu(x + b, alpha) * gain clamped
@@ -73,7 +73,10 @@ struct IgemmParams {
     int kt, kh, kw, pad_t, pad_h, pad_w;
     int tt, th, wt, wtb, thb;    // tile frames / rows / cols, box cols / rows
     int frame_px;                // thb * wtb: accumulator columns from one frame of the tile to the next
-    int ncols;                   // accumulator columns (multiple of 16, <= 256; the MMAs compute them in chunks of 64)
+    int ncols;                   // accumulator columns of the tile (multiple of 16, <= 256)
+    int m64;                     // 64-row mode (cout <= 64): 64-row weight images, both consumers read the same A and split the columns
+    int ncw;                     // MMA width of a consumer: ncols, or in 64-row mode ncols / 2 rounded up to 16
+    int a_img;                   // bytes of one weight image: 4096 (128 rows), 2048 (64 rows)
     int tiles_x, tiles_y, tiles_t;
     int64_t total_tiles;         // tiles_x * tiles_y * tiles_t * mt * instances
     int ks;                      // k-steps per stage (> 1 only when kt == 1)
@@ -184,6 +187,8 @@ int pack_act(const void* x, void* x8, int split, int64_t inst, int c, int cblk, 
 // run of 16*taps elements per output channel; dgrad: one run of 128*taps elements per k): a warp copies a run into shared
 // memory with aligned 4-byte loads (no per-element index arithmetic), then every thread assembles one 16-byte image row
 // from 8 shared-memory reads and consecutive threads write consecutive rows (512 contiguous bytes per warp).
+// 64-row mode (GEMMs with at most 64 rows): 64 x 16 images of 2048 bytes, byte offset(m, k) = (k/8)*1024 + (m/8)*128 +
+// (m%8)*16 + (k%8)*2, row = channel; both consumer warpgroups read the whole image.
 // Rows of the 128-row weight image (= accumulator rows). An m-tile with fewer than 128 output channels spreads them evenly
 // over the four 32-row quarters (`per` channels at the start of each) instead of filling quarter after quarter, so that
 // both consumer warpgroups and all their warps share the epilogue's store work of a 32- or 64-channel layer. Channels
@@ -212,7 +217,7 @@ __host__ __device__ __forceinline__ int m_channel_of_row(int row, int per)
 template <class TIn, bool SPLIT>
 __global__ void __launch_bounds__(256) conv_pack_w_kernel(const TIn* __restrict__ w, unsigned char* __restrict__ wp, int m_total, int k_total,
                                                            int kpad, int taps, int64_t gstride, int64_t sm, int64_t sk, int flip, int mt, int kc,
-                                                           int rows_per_pass, int rows_per_cta)
+                                                           int rows_per_pass, int rows_per_cta, int img_rows)
 {
     extern __shared__ uint32_t sw32[];               // [runs][pitch] words, then the runs' element offsets
     constexpr int ES = (int)sizeof(TIn);
@@ -230,15 +235,16 @@ __global__ void __launch_bounds__(256) conv_pack_w_kernel(const TIn* __restrict_
     const int pitch = ((run_el * ES + 2 + 3) / 4) | 1;
     const int max_runs = mrows ? R : 16;
     int* s_off = reinterpret_cast<int*>(sw32 + (size_t)max_runs * pitch);
-    unsigned char* dst0 = wp + ((((int64_t)g * mt + mti) * kc + kci) * taps) * (int64_t)(NIMG * kATile);
+    const int img = img_rows * 32;                   // bytes of one image
+    unsigned char* dst0 = wp + ((((int64_t)g * mt + mti) * kc + kci) * taps) * (int64_t)(NIMG * img);
     const int kvalid = max(0, min(16, k_total - k0));
     const int per = m_rows_per_quadrant(m_total - mti * kBM);
     // blockIdx.y = chunk of rows_per_cta image rows (small layers have only a handful of (group, m-tile, k-step) blocks: the
     // row chunks spread their latency-bound staging over more SMs)
-    const int row_end = min(kBM, ((int)blockIdx.y + 1) * rows_per_cta);
+    const int row_end = min(img_rows, ((int)blockIdx.y + 1) * rows_per_cta);
     for (int r0 = (int)blockIdx.y * rows_per_cta; r0 < row_end; r0 += R) {
         const int Rn = min(R, row_end - r0);
-        const int m0 = mti * kBM + r0;
+        const int m0 = mti * img_rows + r0;
         const int mvalid = max(0, min(Rn, m_total - m0));
         const int len = mrows ? kvalid * taps : mvalid * taps;             // valid elements of a run
         const int nruns = len > 0 ? (mrows ? mvalid : kvalid) : 0;
@@ -291,9 +297,10 @@ __global__ void __launch_bounds__(256) conv_pack_w_kernel(const TIn* __restrict_
                     v[j] = ES == 2 ? hbits : __half_as_ushort(__float2half_rn(f));
                 }
             }
-            unsigned char* dimg = dst0 + (size_t)tap * (NIMG * kATile) + k8 * 2048 + m_row_of_channel(r0 + mrow, per) * 16;
+            const int row = img_rows == kBM ? m_row_of_channel(r0 + mrow, per) : r0 + mrow;
+            unsigned char* dimg = dst0 + (size_t)tap * (NIMG * img) + k8 * (img / 2) + row * 16;
             *reinterpret_cast<uint4*>(dimg) = *reinterpret_cast<const uint4*>(v);
-            if constexpr (SPLIT) *reinterpret_cast<uint4*>(dimg + kATile) = *reinterpret_cast<const uint4*>(vlo);
+            if constexpr (SPLIT) *reinterpret_cast<uint4*>(dimg + img) = *reinterpret_cast<const uint4*>(vlo);
         }
         __syncthreads();
     }
@@ -335,9 +342,11 @@ __device__ __forceinline__ TileCoord decode_tile(const IgemmParams& p, int64_t L
 // weight tiles of one (instance, m-tile) in L2). The operand ring runs across tile boundaries, so the producer fetches the
 // first stages of tile i + 1 while the consumers store tile i.
 // Roles (384 threads): warp 0 = TMA producer (one lane); warpgroups 1 and 2 = MMA + epilogue for accumulator rows 0-63 and
-// 64-127 of the weight images. Each consumer holds its 64 x ncols fp32 accumulator in registers (ncols <= 256, issued as
-// chunks of 64 columns) and releases a stage once the wgmma group that read it has completed.
-template <bool BF16, int NCH, bool OSCALE>
+// 64-127 of the weight images, each over all ncols columns (NW = ncols). 64-row mode (at most 64 output rows): both read
+// the same 64-row images, warpgroup 1 takes columns [0, NW), warpgroup 2 [NW, 2 NW) (NW = ncols / 2 rounded up to 16;
+// columns >= ncols are computed and dropped). Each consumer holds its 64 x NW fp32 accumulator in registers, issues one
+// m64nNWk16 per tap and product, and releases a stage once the wgmma group that read it has completed.
+template <bool BF16, int NW, bool OSCALE>
 __global__ void __launch_bounds__(kIgemmThreads, 1) conv_igemm_kernel(const __grid_constant__ CUtensorMap tmx, const IgemmParams p)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -360,7 +369,7 @@ __global__ void __launch_bounds__(kIgemmThreads, 1) conv_igemm_kernel(const __gr
             int it = 0;
             for (int64_t L = blockIdx.x; L < p.total_tiles; L += gridDim.x) {
                 const TileCoord c = decode_tile(p, L);
-                const unsigned char* wpg = p.wp + (((int64_t)(c.inst % p.wgroups) * p.mt + c.mti) * p.kc) * (int64_t)(p.kt * taps2) * (p.nimg * kATile);
+                const unsigned char* wpg = p.wp + (((int64_t)(c.inst % p.wgroups) * p.mt + c.mti) * p.kc) * (int64_t)(p.kt * taps2) * (p.nimg * p.a_img);
                 const int blk0 = c.inst * p.nblk;
                 for (int kt = 0; kt < p.kt; kt++) {
                     for (int kcix = 0; kcix < kchunks; kcix++, it++) {
@@ -370,10 +379,10 @@ __global__ void __launch_bounds__(kIgemmThreads, 1) conv_igemm_kernel(const __gr
                         const int k0 = kcix * p.ks;
                         const int nks = min(p.ks, p.kc - k0);
                         const bool load_a = !p.a_resident || it < p.stages;
-                        const uint32_t a_bytes = load_a ? (uint32_t)(nks * taps2 * p.nimg * kATile) : 0u;
+                        const uint32_t a_bytes = load_a ? (uint32_t)(nks * taps2 * p.nimg * p.a_img) : 0u;
                         mbar_expect_tx(&full_bar[s], a_bytes + (uint32_t)(nks * p.nimg * p.b_box));
                         // A: kt == 1 -> the nks steps' tiles are contiguous; kt > 1 -> ks == 1, the taps of this kt are contiguous
-                        if (load_a) bulk_copy_g2s(st, wpg + ((int64_t)k0 * p.kt + kt) * (int64_t)taps2 * (p.nimg * kATile), a_bytes, &full_bar[s]);
+                        if (load_a) bulk_copy_g2s(st, wpg + ((int64_t)k0 * p.kt + kt) * (int64_t)taps2 * (p.nimg * p.a_img), a_bytes, &full_bar[s]);
                         for (int j = 0; j < nks; j++) {
                             const int kb = (k0 + j) * 2;
                             for (int im = 0; im < p.nimg; im++)
@@ -385,19 +394,20 @@ __global__ void __launch_bounds__(kIgemmThreads, 1) conv_igemm_kernel(const __gr
             }
         }
     } else if (wg >= 1) {
-        const int cw = wg - 1;                               // accumulator rows 64 cw .. 64 cw + 63
+        const int cw = wg - 1;
         const int tid = threadIdx.x % 128, wq = tid / 32;
         const uint32_t blk_bytes = (uint32_t)p.b_box / 2;
         const uint32_t a_hi = desc_hi(128), b_hi = desc_hi(128);
-        const uint32_t a_tap = (uint32_t)(p.nimg * kATile) >> 4, b_lo_img = (uint32_t)p.b_bytes >> 4;
+        const uint32_t a_tap = (uint32_t)(p.nimg * p.a_img) >> 4, a_lo_img = (uint32_t)p.a_img >> 4, b_lo_img = (uint32_t)p.b_bytes >> 4;
+        // 128-row images: this warpgroup's 64 rows start 1024 bytes into an image; 64-row mode: its columns start NW pixels in
+        const uint32_t a_row0 = p.m64 ? 0u : (uint32_t)cw * 1024u;
+        const int col0 = p.m64 ? cw * NW : 0;
         int it = 0;
         for (int64_t L = blockIdx.x; L < p.total_tiles; L += gridDim.x) {
             const TileCoord c = decode_tile(p, L);
-            float acc[NCH][32];                              // NCH = ncols / 64 rounded up (columns >= ncols are computed and dropped)
+            float acc[NW / 2];
 #pragma unroll
-            for (int ch = 0; ch < NCH; ch++)
-#pragma unroll
-                for (int i = 0; i < 32; i++) acc[ch][i] = 0.f;
+            for (int i = 0; i < NW / 2; i++) acc[i] = 0.f;
             int prev = -1;
             for (int kt = 0; kt < p.kt; kt++) {
                 for (int kcix = 0; kcix < kchunks; kcix++, it++) {
@@ -407,22 +417,19 @@ __global__ void __launch_bounds__(kIgemmThreads, 1) conv_igemm_kernel(const __gr
                     const uint32_t st = smem_u32(smem + (size_t)s * p.stage_bytes);
                     const int nks = min(p.ks, p.kc - kcix * p.ks);
                     // descriptors as (lo, hi) words, stepped with 32-bit adds on the low word (address >> 4): the next tap's weight
-                    // image(s) + nimg * 4096 bytes, the next tap column + 16 bytes, the next tap row + wtb * 16 bytes, the next
-                    // 64 accumulator columns + 1024 bytes; this warpgroup's 64 weight rows start 1024 bytes into an image
+                    // image(s) + nimg * a_img bytes, the next tap column + 16 bytes, the next tap row + wtb * 16 bytes, the next
+                    // accumulator column + 16 bytes. A's LBO (the second 8-channel half) is half an image.
                     for (int j = 0; j < nks; j++) {
-                        uint32_t a_lo = desc_lo(st + (uint32_t)(j * taps2 * p.nimg) * kATile + (uint32_t)cw * 1024u, 2048);
-                        const uint32_t b_base = desc_lo(st + (uint32_t)p.a_stage + (uint32_t)j * (uint32_t)p.b_step, blk_bytes);
+                        uint32_t a_lo = desc_lo(st + (uint32_t)(j * taps2 * p.nimg * p.a_img) + a_row0, (uint32_t)p.a_img / 2);
+                        const uint32_t b_base = desc_lo(st + (uint32_t)p.a_stage + (uint32_t)j * (uint32_t)p.b_step, blk_bytes) + (uint32_t)col0;
                         for (int ky = 0; ky < p.kh; ky++) {
                             for (int kx = 0; kx < p.kw; kx++, a_lo += a_tap) {
                                 const uint32_t b_lo = b_base + (uint32_t)(ky * p.wtb + kx);
-#pragma unroll
-                                for (int ch = 0; ch < NCH; ch++) {
-                                    // fp16: one product; split: hi*hi, hi*lo, lo*hi (A image hi, hi, lo; B image hi, lo, hi)
-                                    wgmma_m64n64k16<BF16, 0, 0>(acc[ch], a_lo, a_hi, b_lo + 64u * ch, b_hi);
-                                    if constexpr (BF16) {
-                                        wgmma_m64n64k16<BF16, 0, 0>(acc[ch], a_lo, a_hi, b_lo + 64u * ch + b_lo_img, b_hi);
-                                        wgmma_m64n64k16<BF16, 0, 0>(acc[ch], a_lo + (kATile >> 4), a_hi, b_lo + 64u * ch, b_hi);
-                                    }
+                                // fp16: one product; split: hi*hi, hi*lo, lo*hi (A image hi, hi, lo; B image hi, lo, hi)
+                                wgmma_m64nNk16<BF16, NW, 0, 0>(acc, a_lo, a_hi, b_lo, b_hi);
+                                if constexpr (BF16) {
+                                    wgmma_m64nNk16<BF16, NW, 0, 0>(acc, a_lo, a_hi, b_lo + b_lo_img, b_hi);
+                                    wgmma_m64nNk16<BF16, NW, 0, 0>(acc, a_lo + a_lo_img, a_hi, b_lo, b_hi);
                                 }
                             }
                         }
@@ -437,7 +444,7 @@ __global__ void __launch_bounds__(kIgemmThreads, 1) conv_igemm_kernel(const __gr
             mbar_arrive_if(&empty_bar[prev], tid == 0);
 
             // ---- epilogue: registers -> [bias, lrelu, gain, clamp] -> NC(T)HW global. This thread holds accumulator rows
-            // r and r + 8 (conv_pack_w_kernel's row order -> channel) and column pairs 8 j + 2 (lane % 4) of every chunk.
+            // r and r + 8 (conv_pack_w_kernel's row order -> channel) and column pairs col0 + 8 j + 2 (lane % 4).
             const int per = m_rows_per_quadrant(p.cout - c.mti * kBM);
             int64_t chbase[2];
             float bias[2];
@@ -445,7 +452,8 @@ __global__ void __launch_bounds__(kIgemmThreads, 1) conv_igemm_kernel(const __gr
             const float* osc[2];
 #pragma unroll
             for (int h = 0; h < 2; h++) {
-                const int ch = m_channel_of_row(cw * 64 + wq * 16 + lane / 4 + 8 * h, per);
+                const int row = wq * 16 + lane / 4 + 8 * h;
+                const int ch = p.m64 ? row : m_channel_of_row(cw * 64 + row, per);
                 const int co = c.mti * kBM + ch;
                 rok[h] = ch < kBM && co < p.cout;
                 bias[h] = (p.bias != nullptr && rok[h]) ? __ldg(p.bias + (int64_t)(c.inst % p.wgroups) * p.cout + co) : 0.f;
@@ -453,39 +461,36 @@ __global__ void __launch_bounds__(kIgemmThreads, 1) conv_igemm_kernel(const __gr
                 osc[h] = OSCALE ? p.out_scale + ((int64_t)c.inst * p.cout + co) * p.to : nullptr;
             }
 #pragma unroll
-            for (int ch = 0; ch < NCH; ch++) {
+            for (int j = 0; j < NW / 8; j++) {
 #pragma unroll
-                for (int j = 0; j < 8; j++) {
+                for (int e = 0; e < 2; e++) {
+                    // accumulator column -> (frame, row, col) of the tile
+                    const int n = col0 + j * 8 + 2 * (lane % 4) + e;
+                    const int f = n / p.frame_px, rem = n - f * p.frame_px;
+                    const int r = rem / p.wtb, cc = rem - r * p.wtb;
+                    const int ot = c.t0 + f, oy = c.oy0 + r, ox = c.ox0 + cc;
+                    bool ok = n < p.ncols && f < p.tt && r < p.th && cc < p.wt && ot < p.to && oy < p.ho && ox < p.wo;
+                    int64_t off;
+                    if (p.ostride == 1) {
+                        off = ((int64_t)ot * p.ho + oy) * p.wo + ox;
+                    } else {
+                        ok = ok && (oy % p.ostride == 0) && (ox % p.ostride == 0);
+                        off = ((int64_t)ot * p.hos + oy / p.ostride) * p.wos + ox / p.ostride;
+                    }
+                    if (!ok) continue;
 #pragma unroll
-                    for (int e = 0; e < 2; e++) {
-                        // accumulator column -> (frame, row, col) of the tile
-                        const int n = ch * 64 + j * 8 + 2 * (lane % 4) + e;
-                        const int f = n / p.frame_px, rem = n - f * p.frame_px;
-                        const int r = rem / p.wtb, cc = rem - r * p.wtb;
-                        const int ot = c.t0 + f, oy = c.oy0 + r, ox = c.ox0 + cc;
-                        bool ok = n < p.ncols && f < p.tt && r < p.th && cc < p.wt && ot < p.to && oy < p.ho && ox < p.wo;
-                        int64_t off;
-                        if (p.ostride == 1) {
-                            off = ((int64_t)ot * p.ho + oy) * p.wo + ox;
-                        } else {
-                            ok = ok && (oy % p.ostride == 0) && (ox % p.ostride == 0);
-                            off = ((int64_t)ot * p.hos + oy / p.ostride) * p.wos + ox / p.ostride;
+                    for (int h = 0; h < 2; h++) {
+                        if (!rok[h]) continue;
+                        float v = acc[4 * j + 2 * h + e];
+                        if constexpr (OSCALE) v *= __ldg(osc[h] + ot);
+                        if (p.act) {
+                            v += bias[h];
+                            if (p.act == 2) v = v < 0.f ? v * p.alpha : v;
+                            v *= p.gain;
+                            if (p.clamp >= 0.f) v = fminf(fmaxf(v, -p.clamp), p.clamp);
                         }
-                        if (!ok) continue;
-#pragma unroll
-                        for (int h = 0; h < 2; h++) {
-                            if (!rok[h]) continue;
-                            float v = acc[ch][4 * j + 2 * h + e];
-                            if constexpr (OSCALE) v *= __ldg(osc[h] + ot);
-                            if (p.act) {
-                                v += bias[h];
-                                if (p.act == 2) v = v < 0.f ? v * p.alpha : v;
-                                v *= p.gain;
-                                if (p.clamp >= 0.f) v = fminf(fmaxf(v, -p.clamp), p.clamp);
-                            }
-                            if (p.out_f32) reinterpret_cast<float*>(p.y)[chbase[h] + off] = v;
-                            else reinterpret_cast<__half*>(p.y)[chbase[h] + off] = __float2half_rn(v);
-                        }
+                        if (p.out_f32) reinterpret_cast<float*>(p.y)[chbase[h] + off] = v;
+                        else reinterpret_cast<__half*>(p.y)[chbase[h] + off] = __float2half_rn(v);
                     }
                 }
             }
@@ -538,6 +543,7 @@ inline int env_flag(const char* name, int dflt)
 
 struct Geometry {
     int cpad, cblk, nblk, nimg, kc, mt;
+    int m64, a_img;              // 64-row mode, bytes of one weight image
     int64_t act_bytes, w_bytes;
 };
 
@@ -551,8 +557,11 @@ Geometry geometry(int split, int64_t inst, int groups, int ck, int cm, int64_t t
     g.nimg = split ? 2 : 1;
     g.kc = g.cpad / 16;
     g.mt = (cm + kBM - 1) / kBM;
+    // at most 64 rows: 64-row weight images (half the A bytes per stage, no all-zero MMA rows)
+    g.m64 = cm <= 64 && env_flag("LVG_CONV_M64", 1) ? 1 : 0;
+    g.a_img = g.m64 ? kATile / 2 : kATile;
     g.act_bytes = inst * g.nblk * thw * 16;
-    g.w_bytes = (int64_t)groups * g.mt * g.kc * taps * g.nimg * kATile;
+    g.w_bytes = (int64_t)groups * g.mt * g.kc * taps * g.nimg * g.a_img;
     return g;
 }
 
@@ -592,6 +601,7 @@ int run_igemm(const void* x, const void* w, void* y, int dtype, int n, int group
     p.out_f32 = split; p.bf16 = split;
     p.wgroups = groups; p.cout = cm; p.mt = g.mt; p.kc = g.kc; p.nblk = g.nblk;
     p.nimg = g.nimg; p.lo_blk = g.cblk;
+    p.m64 = g.m64; p.a_img = g.a_img;
     p.to = t + 2 * pad_t - kt + 1; p.ho = h + 2 * pad_h - kh + 1; p.wo = wd + 2 * pad_w - kw + 1;
     LVG_REQUIRE(p.to >= 1 && p.ho >= 1 && p.wo >= 1, "convnd: empty output");
     p.kt = kt; p.kh = kh; p.kw = kw; p.pad_t = pad_t; p.pad_h = pad_h; p.pad_w = pad_w;
@@ -604,7 +614,7 @@ int run_igemm(const void* x, const void* w, void* y, int dtype, int n, int group
     p.hos = (p.ho - 1) / ostride + 1; p.wos = (p.wo - 1) / ostride + 1;
     p.ks = (kt == 1) ? (taps2 == 1 ? 4 : (taps2 <= 3 ? 2 : 1)) : 1;
     if (p.ks > g.kc) p.ks = g.kc;
-    p.a_stage = p.ks * taps2 * g.nimg * kATile;
+    p.a_stage = p.ks * taps2 * g.nimg * g.a_img;
     // the column budget shrinks until two stages fit shared memory (split precision doubles both operands of a stage)
     int col_budget0 = cb_env ? atoi(cb_env) : 256;
     if (col_budget0 > 256) col_budget0 = 256;
@@ -638,12 +648,14 @@ int run_igemm(const void* x, const void* w, void* y, int dtype, int n, int group
         p.b_box = 2 * p.tt * p.frame_px * 16;                  // one pair of blocks as TMA writes it
         p.b_bytes = round_up(p.b_box, 128);
         p.b_step = g.nimg * p.b_bytes;
-        // + slack: the last taps and the columns of the last 64-column chunk past ncols read up to 50 pixels past the tile
+        // + slack: the last taps and (64-row mode) the columns of the second warpgroup past ncols read up to 50 pixels past
+        // the tile
         p.stage_bytes = round_up(p.a_stage + p.ks * p.b_step + kBSlack, 128);
         if (p.ncols <= 256 && 2 * p.stage_bytes <= smem_budget) break;
         if (p.th == 1 && p.tt == 1 && col_budget <= p.wtb) { LVG_REQUIRE(false, "convnd: a one-row tile does not fit shared memory"); }
     }
     LVG_REQUIRE(p.th >= 1 && p.ncols <= 256 && p.ncols >= 16, "convnd: tile geometry");
+    p.ncw = p.m64 ? round_up(p.ncols / 2, 16) : p.ncols;
     p.stages = 2;
     while (p.stages < kMaxStages && (p.stages + 1) * p.stage_bytes <= smem_budget) p.stages++;
     // Short K loops (few input channels, 1x1 / 1x3x3 kernels): when the ring can be cut to a multiple of the stages one tile
@@ -672,29 +684,30 @@ int run_igemm(const void* x, const void* w, void* y, int dtype, int n, int group
         LVG_REQUIRE(wblocks < (1ll << 31), "convnd: too many weight tiles");
         // rows of m per pass: <= ~64 KB of staging (16 * rows * taps elements either way)
         const int es = split ? 4 : 2;
+        const int img_rows = g.m64 ? 64 : kBM;
         int rpp = (int)((64 * 1024) / (16 * taps * es + 16)) / 8 * 8;
-        if (rpp > kBM) rpp = kBM;
+        if (rpp > img_rows) rpp = img_rows;
         if (rpp < 8) rpp = 8;
         const bool mrows = w_sk < w_sm;
         const int run_el = mrows ? 16 * taps : rpp * taps;
         const int pitch = ((run_el * es + 2 + 3) / 4) | 1;
         const int max_runs = mrows ? rpp : 16;
         const size_t wsm = ((size_t)max_runs * pitch + max_runs + 4) * 4;
-        // row chunks per 128-row image: enough CTAs for two per SM (1, 2, 4 or 8 chunks of 128 / chunks rows)
+        // row chunks per image: enough CTAs for two per SM (1, 2, 4 or 8 chunks of img_rows / chunks rows)
         int chunks = 1;
         {
             const char* e = getenv("LVG_PACKW_CHUNKS");       // experiments
             if (e && atoi(e) >= 1) chunks = atoi(e) >= 8 ? 8 : (atoi(e) >= 4 ? 4 : (atoi(e) >= 2 ? 2 : 1));
             else while (chunks < 8 && wblocks * chunks < 2 * (int64_t)num_sms()) chunks *= 2;
         }
-        const int rows_per_cta = kBM / chunks;
+        const int rows_per_cta = img_rows / chunks;
         const dim3 wgrid((unsigned)wblocks, (unsigned)chunks);
         if (split) {
             LVG_CUDA(cudaFuncSetAttribute(conv_pack_w_kernel<float, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsm));
-            conv_pack_w_kernel<float, true><<<wgrid, 256, wsm, s>>>((const float*)w, wp, cm, ck, g.cpad, taps, w_gs, w_sm, w_sk, flip, g.mt, g.kc, rpp, rows_per_cta);
+            conv_pack_w_kernel<float, true><<<wgrid, 256, wsm, s>>>((const float*)w, wp, cm, ck, g.cpad, taps, w_gs, w_sm, w_sk, flip, g.mt, g.kc, rpp, rows_per_cta, img_rows);
         } else {
             LVG_CUDA(cudaFuncSetAttribute(conv_pack_w_kernel<__half, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsm));
-            conv_pack_w_kernel<__half, false><<<wgrid, 256, wsm, s>>>((const __half*)w, wp, cm, ck, g.cpad, taps, w_gs, w_sm, w_sk, flip, g.mt, g.kc, rpp, rows_per_cta);
+            conv_pack_w_kernel<__half, false><<<wgrid, 256, wsm, s>>>((const __half*)w, wp, cm, ck, g.cpad, taps, w_gs, w_sm, w_sk, flip, g.mt, g.kc, rpp, rows_per_cta, img_rows);
         }
         LVG_LAUNCH_CHECK();
     }
@@ -706,13 +719,17 @@ int run_igemm(const void* x, const void* w, void* y, int dtype, int n, int group
         if (rc) return rc;
     }
     const size_t smem = (size_t)p.stages * p.stage_bytes + 128;
-    // (the output-scaled epilogue is a separate instantiation: the unscaled one stays as it was)
-    void (*const kerns[2][2][kMaxChunks])(const CUtensorMap, const IgemmParams) = {
-        {{conv_igemm_kernel<false, 1, false>, conv_igemm_kernel<false, 2, false>, conv_igemm_kernel<false, 3, false>, conv_igemm_kernel<false, 4, false>},
-         {conv_igemm_kernel<true, 1, false>, conv_igemm_kernel<true, 2, false>, conv_igemm_kernel<true, 3, false>, conv_igemm_kernel<true, 4, false>}},
-        {{conv_igemm_kernel<false, 1, true>, conv_igemm_kernel<false, 2, true>, conv_igemm_kernel<false, 3, true>, conv_igemm_kernel<false, 4, true>},
-         {conv_igemm_kernel<true, 1, true>, conv_igemm_kernel<true, 2, true>, conv_igemm_kernel<true, 3, true>, conv_igemm_kernel<true, 4, true>}}};
-    void (*kern)(const CUtensorMap, const IgemmParams) = kerns[out_scale != nullptr][split][(p.ncols + 63) / 64 - 1];
+    // one instantiation per MMA width (the output-scaled epilogue is a separate one: the unscaled one stays as it was)
+#define LVG_IGEMM_WIDTHS(B, S)                                                                                                     \
+    {conv_igemm_kernel<B, 16, S>,  conv_igemm_kernel<B, 32, S>,  conv_igemm_kernel<B, 48, S>,  conv_igemm_kernel<B, 64, S>,        \
+     conv_igemm_kernel<B, 80, S>,  conv_igemm_kernel<B, 96, S>,  conv_igemm_kernel<B, 112, S>, conv_igemm_kernel<B, 128, S>,       \
+     conv_igemm_kernel<B, 144, S>, conv_igemm_kernel<B, 160, S>, conv_igemm_kernel<B, 176, S>, conv_igemm_kernel<B, 192, S>,       \
+     conv_igemm_kernel<B, 208, S>, conv_igemm_kernel<B, 224, S>, conv_igemm_kernel<B, 240, S>, conv_igemm_kernel<B, 256, S>}
+    void (*const kerns[2][2][kWidths])(const CUtensorMap, const IgemmParams) = {
+        {LVG_IGEMM_WIDTHS(false, false), LVG_IGEMM_WIDTHS(true, false)}, {LVG_IGEMM_WIDTHS(false, true), LVG_IGEMM_WIDTHS(true, true)}};
+#undef LVG_IGEMM_WIDTHS
+    LVG_REQUIRE(p.ncw % 16 == 0 && p.ncw >= 16 && p.ncw <= 16 * kWidths, "convnd: MMA width %d", p.ncw);
+    void (*kern)(const CUtensorMap, const IgemmParams) = kerns[out_scale != nullptr][split][p.ncw / 16 - 1];
     LVG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const char* cta_env = getenv("LVG_CONV_CTAS");          // experiments: fewer persistent CTAs than SMs
     const int max_ctas = cta_env ? atoi(cta_env) : num_sms();
@@ -829,9 +846,10 @@ struct WgradV2Params {
 struct WgradMaps { CUtensorMap a[4]; CUtensorMap b; };     // dy8 clipped to each column segment; x8
 
 // Roles (384 threads): warp 0 = TMA producer (one lane); warpgroups 1 and 2 = MMA + epilogue for output channels 0-63 and
-// 64-127 of the m-tile (only the first when mrows = 64). A consumer holds the khc * kw accumulators of NT columns each in
-// registers (<= 256 columns, issued as chunks of 32 input channels).
-template <bool BF16, int NCH>
+// 64-127 of the m-tile (only the first when mrows = 64). A consumer holds the TAPS = khc * kw accumulators of NT columns
+// each in registers (TAPS * NT <= 256) and issues one m64nNTk16 per tap and k step: the x-tile descriptor steps over the
+// NT / 8 channel blocks with its stride byte offset.
+template <bool BF16, int TAPS, int NT>
 __global__ void __launch_bounds__(kIgemmThreads, 1) conv_wgrad_v2_kernel(const __grid_constant__ WgradMaps maps, const WgradV2Params p)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -847,7 +865,6 @@ __global__ void __launch_bounds__(kIgemmThreads, 1) conv_wgrad_v2_kernel(const _
     const int kt = bx % p.kt;
     const int nti = bx / p.kt;
     const int mti = blockIdx.y, g = blockIdx.z;
-    const int NT = p.nt;
     const int nop = p.split ? 2 : 1;                              // operand images per stage and side
     const int consumers = p.mrows / 64;
 
@@ -892,12 +909,11 @@ __global__ void __launch_bounds__(kIgemmThreads, 1) conv_wgrad_v2_kernel(const _
     } else if (wg >= 1 && wg - 1 < consumers) {
         const int cw = wg - 1;
         const int tid = threadIdx.x % 128, wq = tid / 32;
-        const int cpt = NT / 32;                                   // 32-channel chunks per tap
-        float acc[NCH][16];                                        // NCH = khc * kw * NT / 32 accumulator chunks
+        float acc[TAPS][NT / 2];
 #pragma unroll
-        for (int ch = 0; ch < NCH; ch++)
+        for (int tap = 0; tap < TAPS; tap++)
 #pragma unroll
-            for (int i = 0; i < 16; i++) acc[ch][i] = 0.f;
+            for (int i = 0; i < NT / 2; i++) acc[tap][i] = 0.f;
         int prev = -1;
         for (int s = s0; s < s1; s++) {
             const int it = s - s0, slot = it % p.stages;
@@ -913,19 +929,16 @@ __global__ void __launch_bounds__(kIgemmThreads, 1) conv_wgrad_v2_kernel(const _
             const uint32_t a0 = smem_u32(smem + (size_t)slot * p.stage_bytes) + (uint32_t)cw * 8u * blk_a;
             const uint32_t b0 = smem_u32(smem + (size_t)slot * p.stage_bytes) + (uint32_t)(nop * p.a_bytes);
             // descriptors as (lo, hi) words: a K step is +16 on the low word (256 bytes >> 4), a tap column +1, a tap row
-            // + ps, the next 32 input channels + 4 blocks of the x tile
+            // + ps; the stride byte offset of the x tile (one channel block) spans the NT / 8 blocks of the n-tile
             const uint32_t a_hi = desc_hi(blk_a), b_hi = desc_hi(blk_b);
-            const uint32_t chunk16 = (4u * blk_b) >> 4;
             for (int term = 0; term < (p.split ? 3 : 1); term++) {
                 const uint32_t a_lo0 = desc_lo(a0 + (term == 1 ? (uint32_t)p.a_bytes : 0u), 128);     // hi*hi, lo*hi, hi*lo
                 const uint32_t b_lo0 = desc_lo(b0 + (term == 2 ? (uint32_t)p.b_bytes : 0u), 128);
                 for (int k = 0; k < ksteps; k++) {
 #pragma unroll
-                    for (int ch = 0; ch < NCH; ch++) {
-                        const int tap = ch / cpt, c = ch - tap * cpt;
+                    for (int tap = 0; tap < TAPS; tap++) {
                         const int kyi = tap / p.kw, kx = tap - kyi * p.kw;
-                        wgmma_m64n32k16<BF16, 1, 1>(acc[ch], a_lo0 + 16u * k, a_hi,
-                                                    b_lo0 + 16u * k + (uint32_t)kyi * ky16 + (uint32_t)kx + (uint32_t)c * chunk16, b_hi);
+                        wgmma_m64nNk16<BF16, NT, 1, 1>(acc[tap], a_lo0 + 16u * k, a_hi, b_lo0 + 16u * k + (uint32_t)kyi * ky16 + (uint32_t)kx, b_hi);
                     }
                 }
             }
@@ -940,17 +953,16 @@ __global__ void __launch_bounds__(kIgemmThreads, 1) conv_wgrad_v2_kernel(const _
         const int taps = p.kt * p.kh * p.kw;
         const int ci0 = nti * NT;
 #pragma unroll
-        for (int ch = 0; ch < NCH; ch++) {
-            const int tap = ch / cpt, c = ch - tap * cpt;
+        for (int tap = 0; tap < TAPS; tap++) {
             const int kyi = tap / p.kw, kx = tap - kyi * p.kw;
             const int tapg = (kt * p.kh + ky0 + kyi) * p.kw + kx;
 #pragma unroll
-            for (int i = 0; i < 16; i++) {
+            for (int i = 0; i < NT / 2; i++) {
                 const int co = mti * kBM + cw * 64 + wq * 16 + lane / 4 + 8 * ((i / 2) % 2);
-                const int cil = c * 32 + (i / 4) * 8 + 2 * (lane % 4) + i % 2;
-                if (co >= p.cout || cil >= NT || ci0 + cil >= p.cin) continue;
+                const int cil = (i / 4) * 8 + 2 * (lane % 4) + i % 2;
+                if (co >= p.cout || ci0 + cil >= p.cin) continue;
                 const int64_t off = (((int64_t)g * p.cout + co) * p.cin + ci0 + cil) * taps + tapg;
-                const float v = acc[ch][i];
+                const float v = acc[tap][i];
                 if (p.nsplit > 1) reinterpret_cast<float*>(p.dw)[(int64_t)sp * p.split_stride + off] = v;
                 else if (p.out_f32) reinterpret_cast<float*>(p.dw)[off] = v;
                 else reinterpret_cast<__half*>(p.dw)[off] = __float2half_rn(v);
@@ -1069,6 +1081,42 @@ WgradPlan wgrad_plan(int dtype, int n, int groups, int cin, int cout, int t, int
     return q;
 }
 
+// The (taps per CTA, NT) pairs wgrad_plan can return: NT a multiple of 32 with taps * NT <= 256 (kw <= 3, and kh * kw <= 8
+// when the tap rows are folded), NT <= 128 with split operands. nullptr for anything else.
+typedef void (*WgradKernel)(const WgradMaps, const WgradV2Params);
+template <bool B>
+WgradKernel wgrad_kernel_of(int taps, int nt)
+{
+    switch (taps * 1000 + nt) {
+    case 1032: return conv_wgrad_v2_kernel<B, 1, 32>;
+    case 1064: return conv_wgrad_v2_kernel<B, 1, 64>;
+    case 1096: return conv_wgrad_v2_kernel<B, 1, 96>;
+    case 1128: return conv_wgrad_v2_kernel<B, 1, 128>;
+    case 2032: return conv_wgrad_v2_kernel<B, 2, 32>;
+    case 2064: return conv_wgrad_v2_kernel<B, 2, 64>;
+    case 2096: return conv_wgrad_v2_kernel<B, 2, 96>;
+    case 2128: return conv_wgrad_v2_kernel<B, 2, 128>;
+    case 3032: return conv_wgrad_v2_kernel<B, 3, 32>;
+    case 3064: return conv_wgrad_v2_kernel<B, 3, 64>;
+    case 4032: return conv_wgrad_v2_kernel<B, 4, 32>;
+    case 4064: return conv_wgrad_v2_kernel<B, 4, 64>;
+    case 5032: return conv_wgrad_v2_kernel<B, 5, 32>;
+    case 6032: return conv_wgrad_v2_kernel<B, 6, 32>;
+    case 7032: return conv_wgrad_v2_kernel<B, 7, 32>;
+    case 8032: return conv_wgrad_v2_kernel<B, 8, 32>;
+    }
+    if constexpr (!B) {
+        switch (taps * 1000 + nt) {
+        case 1160: return conv_wgrad_v2_kernel<B, 1, 160>;
+        case 1192: return conv_wgrad_v2_kernel<B, 1, 192>;
+        case 1224: return conv_wgrad_v2_kernel<B, 1, 224>;
+        case 1256: return conv_wgrad_v2_kernel<B, 1, 256>;
+        }
+    }
+    return nullptr;
+}
+WgradKernel wgrad_kernel(int split, int taps, int nt) { return split ? wgrad_kernel_of<true>(taps, nt) : wgrad_kernel_of<false>(taps, nt); }
+
 // the weight-gradient launch; `dy8_pre` != nullptr: dy is already re-tiled (the tensor the input gradient of the same call read)
 int run_wgrad(const void* x, const void* dy, void* dw, int dtype, int n, int groups, int cin, int cout, int t, int h, int wd, int kt, int kh,
               int kw, int pad_t, int pad_h, int pad_w, int stride, const unsigned char* dy8_pre, void* workspace, int64_t workspace_bytes,
@@ -1108,7 +1156,6 @@ int run_wgrad(const void* x, const void* dy, void* dw, int dtype, int n, int gro
     p.a_bytes = q.a_stage; p.b_bytes = q.b_stage; p.stage_bytes = q.stage_bytes; p.stages = q.stages; p.tail_bytes = q.tail_bytes;
     const size_t smem = q.smem;
     LVG_REQUIRE(smem <= 227 * 1024, "convnd_wgrad: stage does not fit shared memory (%zu bytes)", smem);
-    LVG_REQUIRE(q.khc * kw * q.nt <= 32 * kWgradChunks && q.nt % 32 == 0, "convnd_wgrad: accumulators exceed the register budget");
     p.nsplit = q.nsplit;
     p.split_stride = q.dw_elems;
     p.dw = q.nsplit > 1 ? (void*)part : dw;
@@ -1124,11 +1171,8 @@ int run_wgrad(const void* x, const void* dy, void* dw, int dtype, int n, int gro
         const int rc = encode_map(&maps.b, x8, wd, h, t, inst * p.nblk_b, wd, (int64_t)h * wd, thw_b, p.ps[0], p.rh + q.khc - 1, 1, q.nt / 8);
         if (rc) return rc;
     }
-#define LVG_WGRAD_KERNELS(B) {conv_wgrad_v2_kernel<B, 1>, conv_wgrad_v2_kernel<B, 2>, conv_wgrad_v2_kernel<B, 3>, conv_wgrad_v2_kernel<B, 4>, \
-                              conv_wgrad_v2_kernel<B, 5>, conv_wgrad_v2_kernel<B, 6>, conv_wgrad_v2_kernel<B, 7>, conv_wgrad_v2_kernel<B, 8>}
-    void (*const kerns[2][kWgradChunks])(const WgradMaps, const WgradV2Params) = {LVG_WGRAD_KERNELS(false), LVG_WGRAD_KERNELS(true)};
-#undef LVG_WGRAD_KERNELS
-    void (*kern)(const WgradMaps, const WgradV2Params) = kerns[q.split][q.khc * kw * q.nt / 32 - 1];
+    void (*const kern)(const WgradMaps, const WgradV2Params) = wgrad_kernel(q.split, q.khc * kw, q.nt);
+    LVG_REQUIRE(kern != nullptr, "convnd_wgrad: no kernel for %d taps x %d columns (split %d)", q.khc * kw, q.nt, q.split);
     LVG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     dim3 grid((unsigned)(q.ntiles * kt * (kh / q.khc) * q.nsplit), (unsigned)q.mt, (unsigned)groups);
     kern<<<grid, kIgemmThreads, smem, s>>>(maps, p);
@@ -1217,7 +1261,7 @@ extern "C" int lvg_convnd_plan(int mode, int dtype, int n, int groups, int cin, 
     const int v[48] = {p.wgroups, p.cout, p.mt, p.kc, p.nblk, p.nimg, p.lo_blk, p.to, p.ho, p.wo, p.kt, p.kh, p.kw, p.pad_t, p.pad_h, p.pad_w,
                        p.tt, p.th, p.wt, p.wtb, p.thb, p.frame_px, p.ncols, p.tiles_x, p.tiles_y, p.tiles_t,
                        (int)p.total_tiles, p.ks, p.stages, p.a_resident, p.a_stage, p.b_step, p.b_bytes, p.b_box, p.stage_bytes, p.ostride, p.hos, p.wos,
-                       0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+                       p.m64, p.ncw, 0, 0, 0, 0, 0, 0, 0, 0};
     for (int i = 0; i < 48; i++) out[i] = v[i];
     return LVG_OK;
 }

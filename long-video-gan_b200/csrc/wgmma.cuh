@@ -77,56 +77,52 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// D[64 x 64] += A[64 x 16] * B[16 x 64], fp16 or bf16 operands from shared memory, fp32 accumulators in registers, issued by
-// the whole warpgroup. TA / TB: 0 = K-major, 1 = MN-major. Fragment of thread t (warp w = t / 32 of the warpgroup, lane l):
-// d[4 j + r] = D[16 w + l / 4 + 8 (r / 2)][8 j + 2 (l % 4) + r % 2].
-template <bool BF16, int TA, int TB>
-__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi)
+// D[64 x N] += A[64 x 16] * B[16 x N], N = 16, 32, ..., 256, fp16 or bf16 operands from shared memory, fp32 accumulators in
+// registers, issued by the whole warpgroup. TA / TB: 0 = K-major, 1 = MN-major. Fragment of thread t (warp w = t / 32 of the
+// warpgroup, lane l): d[4 j + r] = D[16 w + l / 4 + 8 (r / 2)][8 j + 2 (l % 4) + r % 2], j < N / 8 -- the concatenation of
+// the fragments of N / 8 consecutive 8-column slices, whatever N is.
+#define LVG_D8(i)                                                                                                            \
+    "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+// NS: N as a string; REGS: the accumulator list; A0 .. SC: operand numbers of a_lo, a_hi, b_lo, b_hi, TA, TB, scale-d
+#define LVG_WGMMA_ASM(NS, TYPE, REGS, A0, A1, B0, B1, TA_, TB_, SC)                                                           \
+    "{\n .reg .b64 da, db;\n .reg .pred p;\n setp.ne.b32 p, %" SC ", 0;\n mov.b64 da, {%" A0 ", %" A1 "};\n"                   \
+    " mov.b64 db, {%" B0 ", %" B1 "};\n wgmma.mma_async.sync.aligned.m64n" NS "k16.f32." TYPE "." TYPE " " REGS                 \
+    ", da, db, p, 1, 1, %" TA_ ", %" TB_ ";\n}\n"
+#define LVG_WGMMA(NS, REGS, A0, A1, B0, B1, TA_, TB_, SC, ...)                                                                \
+    do {                                                                                                                       \
+        if constexpr (BF16)                                                                                                    \
+            asm volatile(LVG_WGMMA_ASM(NS, "bf16", REGS, A0, A1, B0, B1, TA_, TB_, SC)                                        \
+                         : __VA_ARGS__ : "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "n"(TA), "n"(TB), "r"(1));               \
+        else                                                                                                                   \
+            asm volatile(LVG_WGMMA_ASM(NS, "f16", REGS, A0, A1, B0, B1, TA_, TB_, SC)                                         \
+                         : __VA_ARGS__ : "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "n"(TA), "n"(TB), "r"(1));               \
+    } while (0)
+template <bool BF16, int N, int TA, int TB>
+__device__ __forceinline__ void wgmma_m64nNk16(float (&d)[N / 2], uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi)
 {
-#define LVG_WGMMA_N64(TYPE)                                                                                                        \
-    asm volatile(                                                                                                                  \
-        "{\n"                                                                                                                      \
-        " .reg .b64 da, db;\n"                                                                                                     \
-        " .reg .pred p;\n"                                                                                                         \
-        " setp.ne.b32 p, %38, 0;\n"                                                                                                \
-        " mov.b64 da, {%32, %33};\n"                                                                                               \
-        " mov.b64 db, {%34, %35};\n"                                                                                               \
-        " wgmma.mma_async.sync.aligned.m64n64k16.f32." TYPE "." TYPE " "                                                           \
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                                  \
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, da, db, p, 1, 1, %36, %37;\n"            \
-        "}\n"                                                                                                                      \
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), \
-          "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),    \
-          "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),    \
-          "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])                                                                       \
-        : "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "n"(TA), "n"(TB), "r"(1))
-    if constexpr (BF16) LVG_WGMMA_N64("bf16");
-    else LVG_WGMMA_N64("f16");
-#undef LVG_WGMMA_N64
+    static_assert(N % 16 == 0 && N >= 16 && N <= 256, "wgmma: N = 16, 32, ..., 256");
+    // ---- BEGIN GENERATED (tools/gen_wgmma.py)
+    if constexpr (N == 16) LVG_WGMMA("16", "{%0, %1, %2, %3, %4, %5, %6, %7}", "8", "9", "10", "11", "12", "13", "14", LVG_D8(0));
+    else if constexpr (N == 32) LVG_WGMMA("32", "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}", "16", "17", "18", "19", "20", "21", "22", LVG_D8(0), LVG_D8(8));
+    else if constexpr (N == 48) LVG_WGMMA("48", "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}", "24", "25", "26", "27", "28", "29", "30", LVG_D8(0), LVG_D8(8), LVG_D8(16));
+    else if constexpr (N == 64) LVG_WGMMA("64", "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}", "32", "33", "34", "35", "36", "37", "38", LVG_D8(0), LVG_D8(8), LVG_D8(16), LVG_D8(24));
+    else if constexpr (N == 80) LVG_WGMMA("80", "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}", "40", "41", "42", "43", "44", "45", "46", LVG_D8(0), LVG_D8(8), LVG_D8(16), LVG_D8(24), LVG_D8(32));
+    else if constexpr (N == 96) LVG_WGMMA("96", "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}", "48", "49", "50", "51", "52", "53", "54", LVG_D8(0), LVG_D8(8), LVG_D8(16), LVG_D8(24), LVG_D8(32), LVG_D8(40));
+    else if constexpr (N == 112) LVG_WGMMA("112", "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55}", "56", "57", "58", "59", "60", "61", "62", LVG_D8(0), LVG_D8(8), LVG_D8(16), LVG_D8(24), LVG_D8(32), LVG_D8(40), LVG_D8(48));
+    else if constexpr (N == 128) LVG_WGMMA("128", "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}", "64", "65", "66", "67", "68", "69", "70", LVG_D8(0), LVG_D8(8), LVG_D8(16), LVG_D8(24), LVG_D8(32), LVG_D8(40), LVG_D8(48), LVG_D8(56));
+    else if constexpr (N == 144) LVG_WGMMA("144", "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71}", "72", "73", "74", "75", "76", "77", "78", LVG_D8(0), LVG_D8(8), LVG_D8(16), LVG_D8(24), LVG_D8(32), LVG_D8(40), LVG_D8(48), LVG_D8(56), LVG_D8(64));
+    else if constexpr (N == 160) LVG_WGMMA("160", "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79}", "80", "81", "82", "83", "84", "85", "86", LVG_D8(0), LVG_D8(8), LVG_D8(16), LVG_D8(24), LVG_D8(32), LVG_D8(40), LVG_D8(48), LVG_D8(56), LVG_D8(64), LVG_D8(72));
+    else if constexpr (N == 176) LVG_WGMMA("176", "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87}", "88", "89", "90", "91", "92", "93", "94", LVG_D8(0), LVG_D8(8), LVG_D8(16), LVG_D8(24), LVG_D8(32), LVG_D8(40), LVG_D8(48), LVG_D8(56), LVG_D8(64), LVG_D8(72), LVG_D8(80));
+    else if constexpr (N == 192) LVG_WGMMA("192", "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}", "96", "97", "98", "99", "100", "101", "102", LVG_D8(0), LVG_D8(8), LVG_D8(16), LVG_D8(24), LVG_D8(32), LVG_D8(40), LVG_D8(48), LVG_D8(56), LVG_D8(64), LVG_D8(72), LVG_D8(80), LVG_D8(88));
+    else if constexpr (N == 208) LVG_WGMMA("208", "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103}", "104", "105", "106", "107", "108", "109", "110", LVG_D8(0), LVG_D8(8), LVG_D8(16), LVG_D8(24), LVG_D8(32), LVG_D8(40), LVG_D8(48), LVG_D8(56), LVG_D8(64), LVG_D8(72), LVG_D8(80), LVG_D8(88), LVG_D8(96));
+    else if constexpr (N == 224) LVG_WGMMA("224", "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111}", "112", "113", "114", "115", "116", "117", "118", LVG_D8(0), LVG_D8(8), LVG_D8(16), LVG_D8(24), LVG_D8(32), LVG_D8(40), LVG_D8(48), LVG_D8(56), LVG_D8(64), LVG_D8(72), LVG_D8(80), LVG_D8(88), LVG_D8(96), LVG_D8(104));
+    else if constexpr (N == 240) LVG_WGMMA("240", "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119}", "120", "121", "122", "123", "124", "125", "126", LVG_D8(0), LVG_D8(8), LVG_D8(16), LVG_D8(24), LVG_D8(32), LVG_D8(40), LVG_D8(48), LVG_D8(56), LVG_D8(64), LVG_D8(72), LVG_D8(80), LVG_D8(88), LVG_D8(96), LVG_D8(104), LVG_D8(112));
+    else if constexpr (N == 256) LVG_WGMMA("256", "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}", "128", "129", "130", "131", "132", "133", "134", LVG_D8(0), LVG_D8(8), LVG_D8(16), LVG_D8(24), LVG_D8(32), LVG_D8(40), LVG_D8(48), LVG_D8(56), LVG_D8(64), LVG_D8(72), LVG_D8(80), LVG_D8(88), LVG_D8(96), LVG_D8(104), LVG_D8(112), LVG_D8(120));
+    // ---- END GENERATED
 }
-
-// the same with N = 32 (d[4 j + r] as above, j < 4)
-template <bool BF16, int TA, int TB>
-__device__ __forceinline__ void wgmma_m64n32k16(float (&d)[16], uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi)
-{
-#define LVG_WGMMA_N32(TYPE)                                                                                                        \
-    asm volatile(                                                                                                                  \
-        "{\n"                                                                                                                      \
-        " .reg .b64 da, db;\n"                                                                                                     \
-        " .reg .pred p;\n"                                                                                                         \
-        " setp.ne.b32 p, %22, 0;\n"                                                                                                \
-        " mov.b64 da, {%16, %17};\n"                                                                                               \
-        " mov.b64 db, {%18, %19};\n"                                                                                               \
-        " wgmma.mma_async.sync.aligned.m64n32k16.f32." TYPE "." TYPE " "                                                           \
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, da, db, p, 1, 1, %20, %21;\n"                     \
-        "}\n"                                                                                                                      \
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), \
-          "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])                                             \
-        : "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "n"(TA), "n"(TB), "r"(1))
-    if constexpr (BF16) LVG_WGMMA_N32("bf16");
-    else LVG_WGMMA_N32("f16");
-#undef LVG_WGMMA_N32
-}
+#undef LVG_WGMMA
+#undef LVG_WGMMA_ASM
+#undef LVG_D8
 
 }  // namespace tc
 }  // namespace lvg
