@@ -615,44 +615,53 @@ int run_igemm(const void* x, const void* w, void* y, int dtype, int n, int group
     p.ks = (kt == 1) ? (taps2 == 1 ? 4 : (taps2 <= 3 ? 2 : 1)) : 1;
     if (p.ks > g.kc) p.ks = g.kc;
     p.a_stage = p.ks * taps2 * g.nimg * g.a_img;
-    // the column budget shrinks until two stages fit shared memory (split precision doubles both operands of a stage)
+    // the column budget shrinks until two stages fit shared memory (split precision doubles both operands of a stage); column
+    // tiles are at most max_wt pixels wide, a TMA box row (256 8-byte elements = 128 pixels) with its kw - 1 halo columns.
+    // When no budget fits at that width, narrower column tiles are tried: the row tiles of a strided convolution take at least
+    // `ostride` rows each, and tall kernels in split precision need large stages.
     int col_budget0 = cb_env ? atoi(cb_env) : 256;
     if (col_budget0 > 256) col_budget0 = 256;
-    for (int col_budget = col_budget0;; col_budget -= 64) {
-        LVG_REQUIRE(col_budget >= 64, "convnd: no tile fits shared memory");
-        const int max_wt = 128 - (kw - 1);                    // a TMA box row is at most 256 8-byte elements
-        p.tiles_x = (p.wo + max_wt - 1) / max_wt;
-        p.wt = (p.wo + p.tiles_x - 1) / p.tiles_x;
-        p.wtb = p.wt + kw - 1;
-        p.th = col_budget / p.wtb;
-        if (p.th > p.ho) p.th = p.ho;
-        if (p.th < 1) p.th = 1;
-        p.tiles_y = (p.ho + p.th - 1) / p.th;
-        p.th = (p.ho + p.tiles_y - 1) / p.tiles_y;           // balance the row tiles
-        if (ostride > 1) {                                     // tile origins on the output lattice
-            if (p.tiles_x > 1) { p.wt = round_up(p.wt, ostride); p.wtb = p.wt + kw - 1; p.tiles_x = (p.wo + p.wt - 1) / p.wt; if (p.th * p.wtb > col_budget) p.th = col_budget / p.wtb; }
-            if (p.th < p.ho) { p.th = p.th / ostride * ostride; if (p.th < ostride) p.th = ostride; }
+    bool fits = false;
+    for (int max_wt = 128 - (kw - 1); !fits; max_wt -= 8) {
+        LVG_REQUIRE(max_wt >= ostride, "convnd: no tile fits shared memory");
+        for (int col_budget = col_budget0; col_budget >= 64 && !fits; col_budget -= 64) {
+            p.tiles_x = (p.wo + max_wt - 1) / max_wt;
+            p.wt = (p.wo + p.tiles_x - 1) / p.tiles_x;
+            p.wtb = p.wt + kw - 1;
+            p.th = col_budget / p.wtb;
+            if (p.th > p.ho) p.th = p.ho;
+            if (p.th < 1) p.th = 1;
             p.tiles_y = (p.ho + p.th - 1) / p.th;
+            p.th = (p.ho + p.tiles_y - 1) / p.tiles_y;           // balance the row tiles
+            if (ostride > 1) {                                     // tile origins on the output lattice, column tiles within max_wt
+                if (p.tiles_x > 1) {
+                    p.wt = std::min(round_up(p.wt, ostride), max_wt / ostride * ostride);
+                    p.wtb = p.wt + kw - 1;
+                    p.tiles_x = (p.wo + p.wt - 1) / p.wt;
+                    if (p.th * p.wtb > col_budget) p.th = col_budget / p.wtb;
+                }
+                if (p.th < p.ho) { p.th = p.th / ostride * ostride; if (p.th < ostride) p.th = ostride; }
+                p.tiles_y = (p.ho + p.th - 1) / p.th;
+            }
+            p.thb = p.th + kh - 1;
+            p.frame_px = p.thb * p.wtb;
+            p.tt = 1;
+            if (p.tiles_y == 1 && p.tiles_x == 1) {                // whole frames: take as many as fit
+                while (p.tt < p.to && p.tt * p.frame_px + p.th * p.wtb <= col_budget && p.tt < 64) p.tt++;
+            }
+            p.tiles_t = (p.to + p.tt - 1) / p.tt;
+            p.tt = (p.to + p.tiles_t - 1) / p.tiles_t;
+            p.ncols = round_up((p.tt - 1) * p.frame_px + p.th * p.wtb, 16);
+            // TMA writes the two 8-channel blocks of a k-step densely: block 1 starts tt*thb*wtb*16 bytes after block 0 (= LBO);
+            // every pair of blocks starts at a 128-byte multiple (TMA destination alignment)
+            p.b_box = 2 * p.tt * p.frame_px * 16;                  // one pair of blocks as TMA writes it
+            p.b_bytes = round_up(p.b_box, 128);
+            p.b_step = g.nimg * p.b_bytes;
+            // + slack: the last taps and (64-row mode) the columns of the second warpgroup past ncols read up to 50 pixels past
+            // the tile
+            p.stage_bytes = round_up(p.a_stage + p.ks * p.b_step + kBSlack, 128);
+            fits = p.ncols <= 256 && 2 * p.stage_bytes <= smem_budget;
         }
-        p.thb = p.th + kh - 1;
-        p.frame_px = p.thb * p.wtb;
-        p.tt = 1;
-        if (p.tiles_y == 1 && p.tiles_x == 1) {                // whole frames: take as many as fit
-            while (p.tt < p.to && p.tt * p.frame_px + p.th * p.wtb <= col_budget && p.tt < 64) p.tt++;
-        }
-        p.tiles_t = (p.to + p.tt - 1) / p.tt;
-        p.tt = (p.to + p.tiles_t - 1) / p.tiles_t;
-        p.ncols = round_up((p.tt - 1) * p.frame_px + p.th * p.wtb, 16);
-        // TMA writes the two 8-channel blocks of a k-step densely: block 1 starts tt*thb*wtb*16 bytes after block 0 (= LBO);
-        // every pair of blocks starts at a 128-byte multiple (TMA destination alignment)
-        p.b_box = 2 * p.tt * p.frame_px * 16;                  // one pair of blocks as TMA writes it
-        p.b_bytes = round_up(p.b_box, 128);
-        p.b_step = g.nimg * p.b_bytes;
-        // + slack: the last taps and (64-row mode) the columns of the second warpgroup past ncols read up to 50 pixels past
-        // the tile
-        p.stage_bytes = round_up(p.a_stage + p.ks * p.b_step + kBSlack, 128);
-        if (p.ncols <= 256 && 2 * p.stage_bytes <= smem_budget) break;
-        if (p.th == 1 && p.tt == 1 && col_budget <= p.wtb) { LVG_REQUIRE(false, "convnd: a one-row tile does not fit shared memory"); }
     }
     LVG_REQUIRE(p.th >= 1 && p.ncols <= 256 && p.ncols >= 16, "convnd: tile geometry");
     p.ncw = p.m64 ? round_up(p.ncols / 2, 16) : p.ncols;
@@ -996,7 +1005,8 @@ struct WgradPlan {
 // follows in shared memory and are never stored -- rows of D depend on the same rows of A only). Otherwise whole m-tiles.
 inline int wgrad_cpad_a(int cout) { return (cout < kBM && env_flag("LVG_WGRAD_COMPACT", 1)) ? round_up(cout, 16) : round_up(cout, kBM); }
 
-WgradPlan wgrad_plan(int dtype, int n, int groups, int cin, int cout, int t, int h, int wd, int to, int ho, int wo, int kt, int kh, int kw)
+WgradPlan wgrad_plan(int dtype, int n, int groups, int cin, int cout, int t, int h, int wd, int to, int ho, int wo, int kt, int kh, int kw,
+                     bool fold = true)
 {
     WgradPlan q;
     q.split = dtype == LVG_F32;
@@ -1009,7 +1019,7 @@ WgradPlan wgrad_plan(int dtype, int n, int groups, int cin, int cout, int t, int
     // start-address shift of one tile row, like kx is a shift of one pixel -- so dy and x are fetched once per (kt, n-tile)
     // instead of once per (kt, ky), where the kh * kw accumulators of 32 columns each fit the 256 register columns of a
     // consumer warpgroup (kh * kw <= 8).
-    q.khc = (kh > 1 && kh * kw * 32 <= 256 && cin <= env_flag("LVG_WGRAD_FOLD_CIN", 32) && env_flag("LVG_WGRAD_FOLD", 1)) ? kh : 1;
+    q.khc = (fold && kh > 1 && kh * kw * 32 <= 256 && cin <= env_flag("LVG_WGRAD_FOLD_CIN", 32) && env_flag("LVG_WGRAD_FOLD", 1)) ? kh : 1;
     int nt_cap = (256 / (q.khc * kw)) / 32 * 32;
     if (q.split && nt_cap > 128) nt_cap = 128;
     // column segments (a TMA box row is at most 128 pixels incl. the kw - 1 halo) and the common tile pitch
@@ -1055,6 +1065,9 @@ WgradPlan wgrad_plan(int dtype, int n, int groups, int cin, int cout, int t, int
     q.stages = 2;
     while (q.stages < kMaxStages && (q.stages + 1) * q.stage_bytes + q.tail_bytes <= 220 * 1024) q.stages++;
     q.smem = (size_t)q.stages * q.stage_bytes + q.tail_bytes + 128;
+    // tall folded kernels (7 or 8 tap rows) over wide rows in split precision: even one-row stages of NT = 32 overflow shared
+    // memory with the x tile's kh - 1 halo rows -- one CTA per tap row instead
+    if (q.khc > 1 && q.smem > 227 * 1024) return wgrad_plan(dtype, n, groups, cin, cout, t, h, wd, to, ho, wo, kt, kh, kw, false);
     // Split the pixel range over `nsplit` CTAs per output tile. One CTA per SM is resident, so the kernel runs in waves of
     // num_sms CTAs: choose the split that minimises waves x (stages per CTA + a fixed per-CTA cost of ~4 stages: clearing
     // shared memory, the register -> global epilogue) -- e.g. with 132 SMs and 3 output tiles: 44 splits = 132 CTAs = one

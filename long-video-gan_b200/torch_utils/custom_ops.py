@@ -17,6 +17,7 @@ implementation behind these objects: a missing library or a non-CUDA tensor
 raises.
 """
 import ctypes
+import math
 import os
 
 import torch
@@ -578,36 +579,36 @@ class ConvNdPlugin:
         self._ws = {}
 
     @staticmethod
-    def _dims(x, w):
-        """-> (n, c, t, h, w), (kt, kh, kw), spatial rank"""
-        nd = x.ndim - 2
-        sp = list(x.shape[2:])
-        k = list(w.shape[2:])
-        while len(sp) < 3:
-            sp.insert(0, 1)
-            k.insert(0, 1)
-        return sp, k, nd
-
-    @staticmethod
     def _pad3(padding, nd):
         p = list(padding) if isinstance(padding, (list, tuple)) else [padding] * nd
         return [0] * (3 - nd) + [int(v) for v in p]
 
     def supported(self, x, w, stride, padding, dilation, groups):
-        if not (x.is_cuda and x.dtype in (torch.float16, torch.float32) and w.dtype == x.dtype and x.ndim == w.ndim and x.ndim in (3, 4, 5)):
+        return x.is_cuda and self._in_envelope(tuple(x.shape), tuple(w.shape), x.dtype if w.dtype == x.dtype else None, stride, padding,
+                                               dilation, groups)
+
+    @staticmethod
+    def _in_envelope(x_shape, w_shape, dtype, stride, padding, dilation, groups):
+        """The shapes the engine plans and runs in every direction (forward, input gradient, weight gradient): fp16 / fp32,
+        1-D / 2-D / 3-D, kh * kw <= 9 with kw <= 3, kt <= 7, 0 <= padding <= k - 1, dilation 1, the same stride 1-4 on H and W
+        (1 on T and on 1-D tensors), and a stride-1 output width the weight gradient's at most 4 column segments of
+        128 - (kw - 1) pixels cover (wgrad_in_envelope in csrc/conv_igemm.cu)."""
+        if not (dtype in (torch.float16, torch.float32) and len(x_shape) == len(w_shape) and len(x_shape) in (3, 4, 5)):
             return False
-        nd = x.ndim - 2
+        nd = len(x_shape) - 2
         as_t = lambda v: tuple(v) if isinstance(v, (list, tuple)) else (v,) * nd       # noqa: E731
         st = as_t(stride)
         if as_t(dilation) != (1,) * nd or len(set(st[-2:])) != 1 or not (1 <= st[-1] <= 4) or (nd == 3 and st[0] != 1) or (nd == 1 and st[0] != 1):
             return False
-        sp, k, _ = self._dims(x, w)
-        pad = self._pad3(padding, nd)
+        sp = [1] * (3 - nd) + list(x_shape[2:])
+        k = [1] * (3 - nd) + list(w_shape[2:])
+        pad = ConvNdPlugin._pad3(padding, nd)
         if k[1] * k[2] > 9 or k[0] > 7 or k[2] > 3 or min(pad) < 0 or any(p > kk - 1 for p, kk in zip(pad, k)):
             return False
-        if x.shape[1] != w.shape[1] * groups or w.shape[0] % groups != 0 or x.shape[0] * groups > 65535 or x.numel() == 0:
+        if x_shape[1] != w_shape[1] * groups or w_shape[0] % groups != 0 or x_shape[0] * groups > 65535 or math.prod(x_shape) == 0:
             return False
-        return all(s + 2 * p - kk + 1 >= 1 for s, p, kk in zip(sp, pad, k))
+        out = [s + 2 * p - kk + 1 for s, p, kk in zip(sp, pad, k)]
+        return min(out) >= 1 and out[2] <= 4 * (128 - k[2] + 1)
 
     def _workspace(self, device, need):
         if need < 0:

@@ -170,16 +170,17 @@ def conv3d(input, weight, bias=None, stride=1, padding=0, dilation=1, groups=1):
 def conv_transpose2d(input, weight, bias=None, stride=1, padding=0, output_padding=0, groups=1, dilation=1):
     """Transposed convolution = the input gradient of the convolution whose weight is `weight` ([Cin, Cout/groups, kh, kw]):
     output extent (H - 1) * stride - 2 * padding + k + output_padding."""
+    from .. import custom_ops
     nd = 2
     st, pd, op, dl = _tup(stride, nd), _tup(padding, nd), _tup(output_padding, nd), _tup(dilation, nd)
     kh, kw = weight.shape[2], weight.shape[3]
     out_h = (input.shape[2] - 1) * st[0] - 2 * pd[0] + kh + op[0]
     out_w = (input.shape[3] - 1) * st[1] - 2 * pd[1] + kw + op[1]
     x_shape = (input.shape[0], weight.shape[1] * groups, out_h, out_w)
-    native = (enabled_for(input) and weight.dtype == input.dtype and input.dtype in (torch.float16, torch.float32) and dl == (1, 1)
-              and st[0] == st[1] and 1 <= st[0] <= 4 and kh * kw <= 9 and kw <= 3 and 0 <= pd[0] <= kh - 1 and 0 <= pd[1] <= kw - 1
-              and max(op) < st[0] and input.shape[0] * groups <= 65535
-              # the forward convolution of that extent must reproduce the input's extent
+    # the forward convolution of that extent (whose gradients the backward pass takes) lies in the engine's envelope and
+    # reproduces the input's extent
+    native = (enabled_for(input) and weight.dtype == input.dtype and max(op) < st[0]
+              and custom_ops.ConvNdPlugin._in_envelope(x_shape, tuple(weight.shape), input.dtype, st, pd, dl, groups)
               and (out_h + 2 * pd[0] - kh) // st[0] + 1 == input.shape[2] and (out_w + 2 * pd[1] - kw) // st[1] + 1 == input.shape[3])
     if not native:
         return torch.nn.functional.conv_transpose2d(input, weight, bias, stride, padding, output_padding, groups, dilation)

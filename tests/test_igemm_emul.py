@@ -4,7 +4,7 @@ with the tiling the library itself plans (`lvg_convnd_plan`, host arithmetic of 
 What is replayed in numpy: the persistent tile loop and its decode order, the TMA boxes over the channel-block tensor X8
 with hardware zero fill (halo rows / columns / frames), the stage layout in shared memory, a filter tap as a shift of the
 linear pixel index (ky * tile_width + kx), the MMA over ALL accumulator columns including the halo columns that straddle
-rows and frames (in the kernel's 64-column chunks), the row order of the weight images (channels of a partial m-tile spread
+rows and frames (one instruction per tap and product at the tile's full width, ncols = 16 ... 256), the row order of the weight images (channels of a partial m-tile spread
 over the four 32-row quarters), and the epilogue's map from (accumulator row, column) to (channel, frame, row, column) with the stride lattice of strided
 convolutions -- against torch.nn.functional convolutions in float64. Checked besides the values: every read stays inside the
 stage buffer (+ its slack), every output element is written exactly once, the shared-memory budget, and the
@@ -60,7 +60,7 @@ def emulate(X, A, q, n, groups, ck, cm, garbage):
     assert fpx == thb * wtb and q['b_box'] == 2 * tt * fpx * 16 and q['b_bytes'] >= q['b_box'] and q['b_bytes'] % 128 == 0
     assert ncols % 16 == 0 and 16 <= ncols <= 256 and wtb <= 128 and thb <= 256 and tt <= 256
     assert q['stages'] >= 2 and q['stages'] * q['stage_bytes'] + 128 <= 227 * 1024
-    mma_cols = -(-ncols // 64) * 64                         # the MMAs run in chunks of 64 columns; columns >= ncols are dropped
+    mma_cols = ncols                                       # one MMA per tap over the tile's full width
     kchunks = -(-q['kc'] // q['ks'])
     if q['a_resident']:
         assert q['stages'] % (kt * kchunks) == 0 and groups == 1 and q['mt'] == 1
@@ -144,6 +144,9 @@ CASES = [
     (1, 1, 72, 40, (2, 5, 6), (1, 1, 1), (0, 0, 0), 1),        # 1x1x1: four k-steps per stage
     (2, 1, 64, 32, (1, 1, 16), (1, 1, 3), (0, 0, 1), 1),       # conv1d
     (1, 1, 16, 24, (7, 4, 6), (5, 3, 3), (2, 1, 1), 1),        # 5x3x3
+    (1, 1, 16, 16, (1, 7, 100), (1, 3, 3), (0, 1, 1), 3),      # stride 3, rows wider than 3 x 85: narrower column tiles on the lattice
+    (1, 1, 16, 16, (1, 9, 70), (1, 3, 3), (0, 1, 1), 4),       # stride 4, rows wider than 4 x 64
+    (1, 1, 16, 16, (1, 3, 252), (1, 2, 2), (0, 1, 1), 2),      # 2x2 stride 2: column tiles rounded to the lattice stay <= 128 pixels
 ]
 
 
