@@ -7,6 +7,8 @@ upsample2d :313, downsample2d :352, helpers :35-66). CUDA tensors run in
 kernel launch (the reference issues two, with the intermediate in HBM,
 upfirdn2d.py:244-245).
 """
+import math
+
 import numpy as np
 import torch
 
@@ -183,8 +185,17 @@ def _rank1_factors(f):
     i, j = divmod(int(a.abs().argmax()), a.shape[1])
     fac = None
     if float(a[i, j]) != 0.0:
-        fy, fx = a[:, j].clone(), a[i, :] / a[i, j]
-        if float((torch.outer(fy, fx) - a).abs().max()) <= 1e-6 * float(a.abs().max()):
+        # Balanced split first: both factors scaled by sqrt|a[i, j]|, the sign on fx. For the filters of setup_filter
+        # (outer(k, k) / sum^2, dyadic) it gives float32 factors whose products ARE the filter's taps, so the two 1-D
+        # passes compute the 2-D operator exactly. The unbalanced split a[:, j] x a[i, :] / a[i, j] does not always
+        # (setup_filter([1,3,3,1]): fx = [1/3, 1, 1, 1/3] misses the taps by 1e-9); it is the fallback.
+        s = abs(float(a[i, j])) ** 0.5
+        fy, fx = (a[:, j] / s).float(), (a[i, :] * (math.copysign(1.0, float(a[i, j])) / s)).float()
+        if not torch.equal(torch.outer(fy.double(), fx.double()), a):
+            fy, fx = a[:, j].clone(), a[i, :] / a[i, j]
+            if float((torch.outer(fy, fx) - a).abs().max()) > 1e-6 * float(a.abs().max()):
+                fy = fx = None
+        if fx is not None:
             fac = (fx.to(torch.float32).to(f.device).contiguous(), fy.to(torch.float32).to(f.device).contiguous())
     if len(_rank1_cache) >= 64:
         _rank1_cache.pop(next(iter(_rank1_cache)))
