@@ -1,6 +1,7 @@
 /*
  * lvg_ops.h -- C ABI of liblvg_ops.so, the sm_90a operator library behind the
- * torch_utils.ops drop-in (bias_act, upfirdn2d, filtered_lrelu, conv2d, fma).
+ * torch_utils.ops drop-in (bias_act, upfirdn2d, filtered_lrelu, fma, and the
+ * 1-D / 2-D / 3-D convolution engine behind conv2d_gradfix and conv_nd).
  *
  * Conventions
  *   - every pointer is a DEVICE pointer unless its name ends in _host;
@@ -28,7 +29,7 @@
 extern "C" {
 #endif
 
-#define LVG_ABI_VERSION 1
+#define LVG_ABI_VERSION 2
 
 #define LVG_OK            0
 #define LVG_UNSUPPORTED (-1)
@@ -179,44 +180,6 @@ int lvg_fma(const void* a, const void* b, const void* c, void* out, int dtype,
             const int64_t b_stride[6], const int64_t c_stride[6], void* stream);
 
 /*
- * Grouped 2-D convolution (cross-correlation, like torch.nn.functional.conv2d)
- * on the implicit-GEMM engine below (its T = kt = 1 case) -- the entry behind conv2d_gradfix.conv2d
- * (torch_utils/ops/conv2d_gradfix.py:37-40) for the per-sample-weight
- * "modulated" convolutions (model/generator_sres.py:63-65) and the
- * discriminator convolutions (conv2d_resample.py:29-41).
- *   x [N][G*Cin][H][W]  w [G*Cout][Cin][kh][kw]  y [N][G*Cout][Ho][Wo]
- * NCHW-contiguous fp16 operands, fp32 accumulation, stride 1, 3x3 or 1x1,
- * any batch n (samples share the weights of their group). `workspace` holds the
- * re-tiled operands (lvg_conv2d_fprop_workspace bytes, 16-byte aligned).
- * Returns LVG_UNSUPPORTED outside the covered envelope.
- */
-int lvg_conv2d_fprop(const void* x, const void* w, void* y, int dtype,
-                     int n, int groups, int cin, int cout, int h, int wd,
-                     int kh, int kw, int stride, int pad_h, int pad_w,
-                     void* workspace, int64_t workspace_bytes, void* stream);
-int64_t lvg_conv2d_fprop_workspace(int dtype, int n, int groups, int cin, int cout,
-                                   int h, int wd, int kh, int kw, int stride,
-                                   int pad_h, int pad_w);
-/*
- * Gradient of the convolution above with respect to its input (lvg_convnd_dgrad): dx [N][G*Cin][H][W] from
- * dy [N][G*Cout][Ho][Wo]. The argument list describes the FORWARD convolution. Same workspace.
- */
-int lvg_conv2d_dgrad(const void* dy, const void* w, void* dx, int dtype,
-                     int n, int groups, int cin, int cout, int h, int wd,
-                     int kh, int kw, int stride, int pad_h, int pad_w,
-                     void* workspace, int64_t workspace_bytes, void* stream);
-/*
- * Gradient of the same convolution with respect to its weights: dw [G*Cout][Cin][kh][kw] (fp16, summed
- * over the N samples) from x [N][G*Cin][H][W] and dy [N][G*Cout][Ho][Wo]. Replaces the weight-gradient
- * leg of conv2d_gradfix (conv2d_gradfix.py:119-141 -> aten::convolution_backward / cuDNN). The argument
- * list describes the FORWARD convolution. No workspace argument: lvg_convnd_wgrad runs on a stream-ordered
- * allocation (cudaMallocAsync). Returns -1 outside fp16 / stride 1 / 3x3, 1x1.
- */
-int lvg_conv2d_wgrad(const void* x, const void* dy, void* dw, int dtype,
-                     int n, int groups, int cin, int cout, int h, int wd,
-                     int kh, int kw, int stride, int pad_h, int pad_w, void* stream);
-
-/*
  * Grouped 1-D / 2-D / 3-D convolution (cross-correlation) on Hopper tensor cores (wgmma), TMA-fed (csrc/conv_igemm.cu): one
  * engine for conv2d_gradfix.conv2d / conv_transpose2d (conv2d_gradfix.py:37-45), the F.conv3d calls of the low-res
  * networks (generator_lres.py:119,578; discriminator_lres.py:172) and the F.conv1d calls of the low-res discriminator
@@ -259,7 +222,7 @@ int lvg_convnd_plan(int mode, int dtype, int n, int groups, int cin, int cout, i
                     int pad_t, int pad_h, int pad_w, int stride, int* out, int out_len);
 /*
  * Introspection: the tiling lvg_convnd_wgrad launches with, as 32 ints -- split, cpad_a, cpad_b, nt, ntiles, mt, nsplit,
- * ablk, khc, nseg, ps, rh, stages, a_stage, b_stage, stage_bytes, tail_bytes, smem, seg_w[4], seg_x0[4], pointwise, mrows, 0... --
+ * ablk, khc, nseg, ps, rh, stages, a_stage, b_stage, stage_bytes, tail_bytes, smem, seg_w[4], seg_x0[4], 0, mrows, 0... --
  * host arithmetic only (no device needed): tests/test_wgrad_emul.py replays the kernel's addressing with it on the CPU.
  */
 int lvg_convnd_wgrad_plan(int dtype, int n, int groups, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw,

@@ -39,10 +39,8 @@
 
 namespace lvg {
 // conv_pointwise.cu: streaming fp32 kernels for 1x1x1 convolutions with few channels (HBM-bound; the engine would re-tile and pad)
-bool pw_supported(int dtype, int groups, int cin, int cout, int kt, int kh, int kw, int pad_t, int pad_h, int pad_w, int stride, int64_t P, int wgrad);
+bool pw_supported(int dtype, int groups, int cin, int cout, int kt, int kh, int kw, int pad_t, int pad_h, int pad_w, int stride, int64_t P);
 int pw_conv(const float* x, const float* w, float* y, int n, int cin, int cout, int64_t P, int64_t w_sco, int64_t w_sci, cudaStream_t s);
-int64_t pw_wgrad_workspace(int cin, int cout);
-int pw_wgrad(const float* x, const float* dy, float* dw, int n, int cin, int cout, int64_t P, void* workspace, int64_t workspace_bytes, cudaStream_t s);
 }
 
 namespace lvg {
@@ -779,7 +777,7 @@ extern "C" int lvg_convnd_fprop(const void* x, const void* w, void* y, int dtype
 {
     LVG_REQUIRE(x && w && y, "convnd_fprop: x, w, y must not be NULL");
     if (!bias && act == 0 && gain == 1.f && clamp < 0.f &&
-        pw_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, (int64_t)t * h * wd, 0))
+        pw_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, (int64_t)t * h * wd))
         return pw_conv((const float*)x, (const float*)w, (float*)y, n, cin, cout, (int64_t)t * h * wd, cin, 1, (cudaStream_t)stream);
     if (!nd_supported(dtype, kt, kh, kw) || n < 1 || pad_t < 0 || pad_h < 0 || pad_w < 0 || stride < 1 || stride > 4) {
         set_error("convnd_fprop: outside the tensor-core kernel's envelope");
@@ -796,7 +794,7 @@ extern "C" int lvg_convnd_dgrad(const void* dy, const void* w, void* dx, int dty
                                 void* stream)
 {
     LVG_REQUIRE(dy && w && dx, "convnd_dgrad: dy, w, dx must not be NULL");
-    if (pw_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, (int64_t)t * h * wd, 0))   // dx = W^T dy
+    if (pw_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, (int64_t)t * h * wd))   // dx = W^T dy
         return pw_conv((const float*)dy, (const float*)w, (float*)dx, n, cout, cin, (int64_t)t * h * wd, 1, cin, (cudaStream_t)stream);
     if (!nd_supported(dtype, kt, kh, kw) || n < 1 || pad_t < 0 || pad_h < 0 || pad_w < 0 || pad_t > kt - 1 || pad_h > kh - 1 || pad_w > kw - 1 ||
         stride < 1 || stride > 4) {
@@ -1216,7 +1214,6 @@ extern "C" int64_t lvg_convnd_wgrad_workspace(int dtype, int n, int groups, int 
 {
     if (!wgrad_in_envelope(dtype, n, groups, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, 1)) return -1;
     const int to = t + 2 * pad_t - kt + 1, ho = h + 2 * pad_h - kh + 1, wo = wd + 2 * pad_w - kw + 1;
-    if (pw_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, 1, (int64_t)t * h * wd, 1)) return pw_wgrad_workspace(cin, cout);
     const WgradPlan q = wgrad_plan(dtype, n, groups, cin, cout, t, h, wd, to, ho, wo, kt, kh, kw);
     return q.a_bytes + q.b_bytes + q.part_bytes + 1024;
 }
@@ -1226,10 +1223,6 @@ extern "C" int lvg_convnd_wgrad(const void* x, const void* dy, void* dw, int dty
                                 void* stream)
 {
     LVG_REQUIRE(x && dy && dw, "convnd_wgrad: x, dy, dw must not be NULL");
-    if (pw_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, (int64_t)t * h * wd, 1)) {
-        LVG_REQUIRE(workspace, "convnd_wgrad: workspace must not be NULL");
-        return pw_wgrad((const float*)x, (const float*)dy, (float*)dw, n, cin, cout, (int64_t)t * h * wd, workspace, workspace_bytes, (cudaStream_t)stream);
-    }
     if (!wgrad_in_envelope(dtype, n, groups, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, stride)) {
         set_error("convnd_wgrad: outside the tensor-core kernel's envelope");
         return LVG_UNSUPPORTED;
@@ -1252,7 +1245,7 @@ extern "C" int lvg_convnd_plan(int mode, int dtype, int n, int groups, int cin, 
         return LVG_UNSUPPORTED;
     }
     for (int i = 0; i < out_len; i++) out[i] = 0;
-    if (pw_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, (int64_t)t * h * wd, 0)) { out[47] = 1; return LVG_OK; }
+    if (pw_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, (int64_t)t * h * wd)) { out[47] = 1; return LVG_OK; }
     IgemmParams p;
     memset(&p, 0, sizeof(p));
     void* dummy = reinterpret_cast<void*>(256);          // never dereferenced in plan-only mode
@@ -1292,7 +1285,7 @@ extern "C" int lvg_convnd_wgrad_plan(int dtype, int n, int groups, int cin, int 
     const WgradPlan q = wgrad_plan(dtype, n, groups, cin, cout, t, h, wd, to, ho, wo, kt, kh, kw);
     const int v[32] = {q.split, q.cpad_a, q.cpad_b, q.nt, q.ntiles, q.mt, q.nsplit, q.ablk, q.khc, q.nseg, q.ps, q.rh, q.stages, q.a_stage, q.b_stage,
                        q.stage_bytes, q.tail_bytes, (int)q.smem, q.seg_w[0], q.seg_w[1], q.seg_w[2], q.seg_w[3], q.seg_x0[0], q.seg_x0[1], q.seg_x0[2],
-                       q.seg_x0[3], pw_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, 1, (int64_t)t * h * wd, 1) ? 1 : 0, q.mrows, 0, 0, 0, 0};
+                       q.seg_x0[3], 0, q.mrows, 0, 0, 0, 0};
     for (int i = 0; i < 32; i++) out[i] = v[i];
     return LVG_OK;
 }
@@ -1308,9 +1301,7 @@ bool backward_shares_dy8(int dtype, int n, int groups, int cin, int cout, int t,
 {
     const int64_t P = (int64_t)t * h * wd;
     if (!env_flag("LVG_CONV_SHARED_DY8", 1)) return false;
-    if (pw_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, P, 0) ||
-        pw_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, P, 1))
-        return false;
+    if (pw_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, P)) return false;
     return wgrad_cpad_a(cout) == round_up(cout, 16);
 }
 }  // namespace

@@ -8,8 +8,8 @@
 // layer). These kernels read x once, write y once, and multiply in exact fp32:
 //   forward         y[n][co][p] = sum_ci W[co][ci] * x[n][ci][p]
 //   input gradient  the same kernel on dy with the transposed weight view
-//   weight gradient dW[co][ci]  = sum_{n,p} dy[n][co][p] * x[n][ci][p]   (per-CTA partials + the engine's fold kernel)
-// Envelope: 1x1x1, stride 1, no padding, groups 1, fp32, cin * cout <= 4096 (weight gradient: 512), pixels per sample a multiple of 4,
+// The weight gradient of these layers runs on the engine.
+// Envelope: 1x1x1, stride 1, no padding, groups 1, fp32, cin * cout <= 4096, pixels per sample a multiple of 4,
 // 16-byte aligned tensors; everything else stays on the engine (conv_igemm.cu calls pw_* first).
 #include "common.cuh"
 
@@ -82,112 +82,6 @@ __global__ void __launch_bounds__(kPwThreads, 2) pw_conv_kernel(const float* __r
     }
 }
 
-// Weight gradient. An item = 4 output channels x 4 input channels (16 sums, each kept as an (even pixel, odd pixel) pair);
-// IPT items per thread. With fewer than 256 items the threads form G groups that take the pixel quads of a tile round
-// robin; the groups' partial sums are folded through shared memory in a fixed order. A CTA walks over tiles of 64 pixels
-// (grid-stride) and writes ONE partial dW [COP4][CIP4] to `part`; conv_wgrad_reduce folds the CTAs.
-constexpr int kWgPx = 64;
-
-template <int IPT>
-__global__ void __launch_bounds__(kPwThreads, 2) pw_wgrad_kernel(const float* __restrict__ x, const float* __restrict__ dy, float* __restrict__ part,
-                                                                 int cin, int cout, int n, int64_t P, int tiles, int cop, int cip, int groups_g)
-{
-    extern __shared__ __align__(16) float smem[];
-    float* dys = smem;                                   // [cop][64]
-    float* xs = smem + (size_t)cop * kWgPx;              // [cip][64]
-    const int nci = cip / 4, nitems = (cop / 4) * nci;
-    const int g = IPT == 1 ? threadIdx.x / nitems : 0;   // pixel-quad group (only when every thread has one item)
-    const int G = IPT == 1 ? groups_g : 1;
-    const bool live0 = IPT == 1 ? (g < G) : true;
-    int item[IPT];
-#pragma unroll
-    for (int i = 0; i < IPT; i++) item[i] = IPT == 1 ? threadIdx.x - g * nitems : threadIdx.x + i * kPwThreads;
-    float2 acc[IPT][4][4];
-#pragma unroll
-    for (int i = 0; i < IPT; i++)
-#pragma unroll
-        for (int a = 0; a < 4; a++)
-#pragma unroll
-            for (int b = 0; b < 4; b++) acc[i][a][b] = make_float2(0.f, 0.f);
-
-    const int64_t total = (int64_t)n * tiles;
-    for (int64_t t = blockIdx.x; t < total; t += gridDim.x) {
-        const int s = (int)(t / tiles);
-        const int64_t p0 = (t - (int64_t)s * tiles) * kWgPx;
-        __syncthreads();
-        for (int i = threadIdx.x; i < (cop + cip) * (kWgPx / 4); i += kPwThreads) {
-            const int row = i / (kWgPx / 4), q = i - row * (kWgPx / 4);
-            const int64_t p = p0 + 4 * q;
-            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (p < P) {
-                if (row < cop) { if (row < cout) v = *reinterpret_cast<const float4*>(dy + ((int64_t)s * cout + row) * P + p); }
-                else if (row - cop < cin) v = *reinterpret_cast<const float4*>(x + ((int64_t)s * cin + (row - cop)) * P + p);
-            }
-            *reinterpret_cast<float4*>(smem + (size_t)row * kWgPx + 4 * q) = v;
-        }
-        __syncthreads();
-#pragma unroll
-        for (int i = 0; i < IPT; i++) {
-            if (!(IPT == 1 ? live0 : item[i] < nitems)) continue;
-            const int co4 = item[i] / nci, ci4 = item[i] - co4 * nci;
-            const float* dr = dys + (size_t)(4 * co4) * kWgPx;
-            const float* xr = xs + (size_t)(4 * ci4) * kWgPx;
-            for (int q = g; q < kWgPx / 4; q += G) {
-                float4 d[4], v[4];
-#pragma unroll
-                for (int a = 0; a < 4; a++) { d[a] = *reinterpret_cast<const float4*>(dr + a * kWgPx + 4 * q); v[a] = *reinterpret_cast<const float4*>(xr + a * kWgPx + 4 * q); }
-#pragma unroll
-                for (int a = 0; a < 4; a++)
-#pragma unroll
-                    for (int b = 0; b < 4; b++) {
-                        acc[i][a][b] = pw_fma2(make_float2(d[a].x, d[a].y), make_float2(v[b].x, v[b].y), acc[i][a][b]);
-                        acc[i][a][b] = pw_fma2(make_float2(d[a].z, d[a].w), make_float2(v[b].z, v[b].w), acc[i][a][b]);
-                    }
-            }
-        }
-    }
-    // fold (even, odd) pairs, then the pixel-quad groups in a fixed order, and write this CTA's partial
-    float* out = part + (size_t)blockIdx.x * cop * cip;
-    if (IPT == 1 && G > 1) {
-        __syncthreads();
-        float* red = smem;                               // [G][nitems][16]: at most 256 * 16 floats = 16 KB <= the tile buffers
-        if (live0) {
-#pragma unroll
-            for (int a = 0; a < 4; a++)
-#pragma unroll
-                for (int b = 0; b < 4; b++) red[((size_t)g * nitems + item[0]) * 16 + a * 4 + b] = acc[0][a][b].x + acc[0][a][b].y;
-        }
-        __syncthreads();
-        for (int i = threadIdx.x; i < nitems * 16; i += kPwThreads) {
-            float sum = 0.f;
-            for (int gg = 0; gg < G; gg++) sum += red[(size_t)gg * nitems * 16 + i];
-            const int it = i / 16, ab = i - it * 16, co4 = it / nci, ci4 = it - co4 * nci;
-            out[(size_t)(4 * co4 + ab / 4) * cip + 4 * ci4 + (ab & 3)] = sum;
-        }
-    } else {
-#pragma unroll
-        for (int i = 0; i < IPT; i++) {
-            if (item[i] >= nitems || !live0) continue;
-            const int co4 = item[i] / nci, ci4 = item[i] - co4 * nci;
-#pragma unroll
-            for (int a = 0; a < 4; a++)
-                *reinterpret_cast<float4*>(out + (size_t)(4 * co4 + a) * cip + 4 * ci4) =
-                    make_float4(acc[i][a][0].x + acc[i][a][0].y, acc[i][a][1].x + acc[i][a][1].y, acc[i][a][2].x + acc[i][a][2].y, acc[i][a][3].x + acc[i][a][3].y);
-        }
-    }
-}
-
-// dW[co][ci] = sum over CTAs of part[cta][co][ci] (padded pitch cip)
-__global__ void __launch_bounds__(256) pw_wgrad_fold_kernel(const float* __restrict__ part, float* __restrict__ dw, int ncta, int cin, int cout, int cop, int cip)
-{
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= cin * cout) return;
-    const int co = i / cin, ci = i - co * cin;
-    float s = 0.f;
-    for (int k = 0; k < ncta; k++) s += part[(size_t)k * cop * cip + (size_t)co * cip + ci];
-    dw[i] = s;
-}
-
 template <int CO_T, int CT>
 int pw_launch(const float* x, const float* w, float* y, int n, int cin, int cout, int64_t P, int64_t w_sco, int64_t w_sci, cudaStream_t s)
 {
@@ -212,19 +106,12 @@ bool pw_enabled()
 }
 
 // Channel limits: forward / input gradient take these kernels up to cin * cout = 4096, where the engine's re-tiling and
-// padding cost more than the layer's traffic. The weight-gradient kernel (shared-memory bound: 8 LDS.128 per 32 FMA pairs,
-// row pitches that collide in the banks) runs only on request (LVG_POINTWISE_WGRAD=1); the engine's weight gradient is
-// the default. These limits have not been re-measured on the H100 (tools/lres_conv_table.py compares both paths).
-bool pw_wgrad_enabled()
+// padding cost more than the layer's traffic. The limits have not been re-measured on the H100 (tools/lres_conv_table.py
+// compares both paths).
+bool pw_supported(int dtype, int groups, int cin, int cout, int kt, int kh, int kw, int pad_t, int pad_h, int pad_w, int stride, int64_t P)
 {
-    const char* e = getenv("LVG_POINTWISE_WGRAD");      // read per call: tests switch it
-    return e && e[0] == '1';
-}
-
-bool pw_supported(int dtype, int groups, int cin, int cout, int kt, int kh, int kw, int pad_t, int pad_h, int pad_w, int stride, int64_t P, int wgrad)
-{
-    return pw_enabled() && (!wgrad || pw_wgrad_enabled()) && dtype == LVG_F32 && groups == 1 && kt == 1 && kh == 1 && kw == 1 && pad_t == 0 && pad_h == 0 && pad_w == 0 && stride == 1 &&
-           cin >= 1 && cout >= 1 && cin <= 128 && cout <= 128 && cin * cout <= (wgrad ? 512 : 4096) && P % 4 == 0 && P >= 4;
+    return pw_enabled() && dtype == LVG_F32 && groups == 1 && kt == 1 && kh == 1 && kw == 1 && pad_t == 0 && pad_h == 0 && pad_w == 0 && stride == 1 &&
+           cin >= 1 && cout >= 1 && cin <= 128 && cout <= 128 && cin * cout <= 4096 && P % 4 == 0 && P >= 4;
 }
 
 // y[n][co][p] = sum_ci w[co * w_sco + ci * w_sci] * x[n][ci][p]   (forward: w_sco = cin, w_sci = 1; input gradient: swapped roles)
@@ -235,39 +122,6 @@ int pw_conv(const float* x, const float* w, float* y, int n, int cin, int cout, 
     if (cout <= 32) return pw_launch<8, 4>(x, w, y, n, cin, cout, P, w_sco, w_sci, s);
     if (cout <= 64) return pw_launch<16, 4>(x, w, y, n, cin, cout, P, w_sco, w_sci, s);
     return pw_launch<16, 8>(x, w, y, n, cin, cout, P, w_sco, w_sci, s);
-}
-
-int64_t pw_wgrad_workspace(int cin, int cout)
-{
-    const int cop = (cout + 3) / 4 * 4, cip = (cin + 3) / 4 * 4;
-    return (int64_t)2 * num_sms() * cop * cip * 4 + 256;
-}
-
-int pw_wgrad(const float* x, const float* dy, float* dw, int n, int cin, int cout, int64_t P, void* workspace, int64_t workspace_bytes, cudaStream_t s)
-{
-    LVG_REQUIRE(aligned16(x) && aligned16(dy) && aligned16(workspace), "pointwise wgrad: tensors must be 16-byte aligned");
-    const int cop = (cout + 3) / 4 * 4, cip = (cin + 3) / 4 * 4;
-    const int nitems = (cop / 4) * (cip / 4);
-    const int tiles = (int)((P + kWgPx - 1) / kWgPx);
-    int64_t ncta = 2 * (int64_t)num_sms();
-    if (ncta > (int64_t)n * tiles) ncta = (int64_t)n * tiles;
-    LVG_REQUIRE(workspace_bytes >= ncta * cop * cip * 4, "pointwise wgrad: workspace too small");
-    float* part = reinterpret_cast<float*>(workspace);
-    const size_t smem = (size_t)(cop + cip) * kWgPx * sizeof(float) < 16384 ? 16384 : (size_t)(cop + cip) * kWgPx * sizeof(float);
-    if (nitems <= kPwThreads) {
-        int G = kPwThreads / nitems;
-        if (G > kWgPx / 4) G = kWgPx / 4;
-        LVG_CUDA(cudaFuncSetAttribute(pw_wgrad_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        pw_wgrad_kernel<1><<<(unsigned)ncta, kPwThreads, smem, s>>>(x, dy, part, cin, cout, n, P, tiles, cop, cip, G);
-    } else {
-        LVG_REQUIRE(nitems <= 2 * kPwThreads, "pointwise wgrad: too many channel pairs");
-        LVG_CUDA(cudaFuncSetAttribute(pw_wgrad_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        pw_wgrad_kernel<2><<<(unsigned)ncta, kPwThreads, smem, s>>>(x, dy, part, cin, cout, n, P, tiles, cop, cip, 1);
-    }
-    LVG_LAUNCH_CHECK();
-    pw_wgrad_fold_kernel<<<(cin * cout + 255) / 256, 256, 0, s>>>(part, dw, (int)ncta, cin, cout, cop, cip);
-    LVG_LAUNCH_CHECK();
-    return LVG_OK;
 }
 
 }  // namespace lvg

@@ -59,10 +59,6 @@ _SIGNATURES = {
     'lvg_filtered_lrelu_supported': (_c_int, [_c_int] * 7),
     'lvg_filtered_lrelu_act': (_c_int, [_c_void_p] * 3 + [_c_int, _I64x4, _I64x4] + [_c_int] * 4 + [_c_float] * 3 + [_c_int, _c_void_p]),
     'lvg_fma': (_c_int, [_c_void_p] * 4 + [_c_int, _c_int, _I64x6, _I64x6, _I64x6, _I64x6, _c_void_p]),
-    'lvg_conv2d_fprop': (_c_int, [_c_void_p] * 3 + [_c_int] * 12 + [_c_void_p, _c_i64, _c_void_p]),
-    'lvg_conv2d_fprop_workspace': (_c_i64, [_c_int] * 12),
-    'lvg_conv2d_dgrad': (_c_int, [_c_void_p] * 3 + [_c_int] * 12 + [_c_void_p, _c_i64, _c_void_p]),
-    'lvg_conv2d_wgrad': (_c_int, [_c_void_p] * 3 + [_c_int] * 12 + [_c_void_p]),
     'lvg_fir1d_depthwise_workspace': (_c_i64, [_c_int]),
     'lvg_fir1d_depthwise': (_c_int, [_c_void_p] * 3 + [_c_int] * 4 + [_c_void_p, _c_i64, _c_void_p]),
     'lvg_convnd_workspace': (_c_i64, [_c_int] * 14),
@@ -101,7 +97,7 @@ def load_library():
             fn = getattr(lib, name)  # AttributeError here = header / library mismatch
             fn.restype = restype
             fn.argtypes = argtypes
-        if lib.lvg_abi_version() != 1:
+        if lib.lvg_abi_version() != 2:
             raise RuntimeError(f'{path}: unexpected ABI version {lib.lvg_abi_version()}')
         _lib = lib
     return _lib
@@ -492,83 +488,6 @@ class FmaPlugin:
         return out
 
 
-class Conv2dPlugin:
-    """Tensor-core convolution behind conv2d_gradfix.conv2d (no reference plugin: the reference calls cuDNN)."""
-
-    def __init__(self, lib):
-        self._lib = lib
-        self._ws = {}
-
-    def supported(self, x, w, stride, padding, dilation, groups):
-        if not (x.is_cuda and x.dtype == torch.float16 and w.dtype == torch.float16 and x.ndim == 4 and w.ndim == 4):
-            return False
-        if tuple(stride) != (1, 1) or tuple(dilation) != (1, 1):
-            return False
-        kh, kw = w.shape[2], w.shape[3]
-        # the C side's envelope, all three legs: 3x3 / 1x1, 0 <= pad <= k - 1 (lvg_conv2d_dgrad), at least one sample
-        if (kh, kw) not in ((3, 3), (1, 1)) or min(padding) < 0 or padding[0] > kh - 1 or padding[1] > kw - 1 or x.shape[0] < 1 or x.numel() == 0:
-            return False
-        if x.shape[1] != w.shape[1] * groups or w.shape[0] % groups != 0:
-            return False
-        return x.shape[0] * groups <= 65535 and x.shape[2] + 2 * padding[0] >= kh and x.shape[3] + 2 * padding[1] >= kw
-
-    def _workspace(self, x, n, groups, cin, cout, h, wd, kh, kw, ph, pw):
-        need = self._lib.lvg_conv2d_fprop_workspace(1, n, groups, cin, cout, h, wd, kh, kw, 1, ph, pw)
-        if need < 0:
-            raise RuntimeError('conv2d: configuration outside the tensor-core kernel envelope')
-        key = x.device
-        buf = self._ws.get(key)
-        if buf is None or buf.numel() < need:
-            buf = torch.empty(max(int(need), 1 << 20), dtype=torch.uint8, device=x.device)
-            self._ws[key] = buf     # stream-ordered reuse: every call repacks before it reads
-        return buf, need
-
-    def fprop(self, x, w, padding, groups):
-        x, w = x.contiguous(), w.contiguous()
-        n, ctot, h, wd = x.shape
-        cout_tot, cin, kh, kw = w.shape
-        ph, pw = padding
-        cout = cout_tot // groups
-        y = torch.empty([n, cout_tot, h + 2 * ph - kh + 1, wd + 2 * pw - kw + 1], dtype=x.dtype, device=x.device)
-        ws, need = self._workspace(x, n, groups, cin, cout, h, wd, kh, kw, ph, pw)
-        with _DeviceGuard(x):
-            rc = _check(self._lib.lvg_conv2d_fprop(_ptr(x), _ptr(w), _ptr(y), 1, n, groups, cin, cout, h, wd, kh, kw, 1, ph, pw,
-                                                   _ptr(ws), ws.numel(), _stream(x)), 'conv2d_fprop')
-        if rc == LVG_UNSUPPORTED:
-            raise RuntimeError('conv2d_fprop: ' + self._lib.lvg_last_error().decode())
-        return y
-
-    def dgrad(self, dy, w, x_shape, padding, groups):
-        dy, w = dy.contiguous(), w.contiguous()
-        n, ctot, h, wd = x_shape
-        cout_tot, cin, kh, kw = w.shape
-        ph, pw = padding
-        cout = cout_tot // groups
-        dx = torch.empty(list(x_shape), dtype=dy.dtype, device=dy.device)
-        ws, need = self._workspace(dy, n, groups, cin, cout, h, wd, kh, kw, ph, pw)
-        with _DeviceGuard(dy):
-            rc = _check(self._lib.lvg_conv2d_dgrad(_ptr(dy), _ptr(w), _ptr(dx), 1, n, groups, cin, cout, h, wd, kh, kw, 1, ph, pw,
-                                                   _ptr(ws), ws.numel(), _stream(dy)), 'conv2d_dgrad')
-        if rc == LVG_UNSUPPORTED:
-            raise RuntimeError('conv2d_dgrad: ' + self._lib.lvg_last_error().decode())
-        return dx
-
-    def wgrad(self, x, dy, w_shape, padding, groups):
-        """dw [G*Cout, Cin, kh, kw] (fp16, summed over the batch) from x and dy."""
-        x, dy = x.contiguous(), dy.contiguous()
-        n, ctot, h, wd = x.shape
-        cout_tot, cin, kh, kw = w_shape
-        ph, pw = padding
-        cout = cout_tot // groups
-        dw = torch.empty(list(w_shape), dtype=x.dtype, device=x.device)
-        with _DeviceGuard(x):
-            rc = _check(self._lib.lvg_conv2d_wgrad(_ptr(x), _ptr(dy), _ptr(dw), 1, n, groups, cin, cout, h, wd, kh, kw, 1, ph, pw,
-                                                   _stream(x)), 'conv2d_wgrad')
-        if rc == LVG_UNSUPPORTED:
-            raise RuntimeError('conv2d_wgrad: ' + self._lib.lvg_last_error().decode())
-        return dw
-
-
 class ConvNdPlugin:
     """TMA-fed wgmma implicit-GEMM convolution for 1-D / 2-D / 3-D NC(T)HW tensors, fp16 or fp32 (bf16 hi/lo split),
     stride 1: forward (optionally with the bias_act epilogue fused), input gradient, weight gradient. No reference
@@ -748,7 +667,6 @@ class ConvNdPlugin:
 
 _PLUGIN_CLASSES = {
     'convnd_plugin': ConvNdPlugin,
-    'conv2d_plugin': Conv2dPlugin,
     'bias_act_plugin': BiasActPlugin,
     'upfirdn2d_plugin': Upfirdn2dPlugin,
     'filtered_lrelu_plugin': FilteredLReluPlugin,

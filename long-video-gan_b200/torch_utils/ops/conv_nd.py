@@ -21,7 +21,6 @@ import os
 import torch
 
 _plugin = None
-weight_gradients_disabled = False       # mirrored from conv2d_gradfix.no_weight_gradients()
 
 
 def _get_plugin():
@@ -42,13 +41,13 @@ def enabled_for(x):
 
 def _weights_off():
     from . import conv2d_gradfix
-    return weight_gradients_disabled or conv2d_gradfix.weight_gradients_disabled
+    return conv2d_gradfix.weight_gradients_disabled
 
 
 def _fused_backward_ok(dy):
     """First-order backward pass asking for both gradients: one call that re-tiles dy once (lvg_convnd_backward). With
     create_graph=True (the R1 penalty's double backward) the two gradient Functions below are recorded instead."""
-    return not torch.is_grad_enabled() and os.environ.get('LVG_CONV_FUSED_BACKWARD', '1') != '0' and hasattr(_get_plugin(), 'backward')
+    return not torch.is_grad_enabled() and hasattr(_get_plugin(), 'backward')
 
 
 class _ConvNd(torch.autograd.Function):

@@ -27,9 +27,9 @@ def test_library_exports_every_declared_symbol():
     assert sorted(custom_ops.exported_symbols()) == decl, 'python binding table and header disagree'
 
 
-def test_version_and_error_string():
+def test_abi_version_and_error_string():
     lib = custom_ops.load_library()
-    assert lib.lvg_abi_version() == 1
+    assert lib.lvg_abi_version() == 2
     assert b'sm_90a' in lib.lvg_build_info()
     assert isinstance(lib.lvg_last_error(), bytes)
 
@@ -43,7 +43,7 @@ def test_argument_errors_are_reported_without_a_gpu():
     assert rc == 1
 
 
-def test_host_only_queries_answer_without_a_gpu():
+def test_host_size_queries_answer_without_a_gpu():
     lib = custom_ops.load_library()
     # size of the opaque relu / lrelu code buffer: one 4-byte (fp32) or 8-byte (fp16) word per thread and 1024-pack tile
     assert lib.lvg_bias_act_codes_bytes(0, 4 * 1024 * 7) == 7 * 256 * 4
@@ -52,10 +52,12 @@ def test_host_only_queries_answer_without_a_gpu():
     assert lib.lvg_bias_act_codes_bytes(2, 100) == -1                      # fp64 has no code path
     for n in (4, 1000, 1 << 20, (1 << 31) + 4096):
         assert lib.lvg_bias_act_codes_bytes(0, n) * 4 >= n                 # at least 2 bits per element
-    # envelope of the tensor-core convolution: fp16 (dtype code 1), stride 1, 3x3 / 1x1
-    assert lib.lvg_conv2d_fprop_workspace(1, 1, 4, 32, 64, 20, 20, 3, 3, 1, 1, 1) > 0
-    assert lib.lvg_conv2d_fprop_workspace(0, 1, 4, 32, 64, 20, 20, 3, 3, 1, 1, 1) == -1
-    assert lib.lvg_conv2d_fprop_workspace(1, 1, 4, 32, 64, 20, 20, 3, 3, 2, 1, 1) == -1
+    # envelope of the tensor-core convolution: fp16 (dtype code 1) and fp32 (code 0), not fp64 (code 2), kh * kw <= 9
+    # (dtype, n, groups, cin, cout, t, h, w, kt, kh, kw, pad_t, pad_h, pad_w)
+    assert lib.lvg_convnd_workspace(1, 1, 4, 32, 64, 1, 20, 20, 1, 3, 3, 0, 1, 1) > 0
+    assert lib.lvg_convnd_workspace(0, 1, 4, 32, 64, 1, 20, 20, 1, 3, 3, 0, 1, 1) > 0
+    assert lib.lvg_convnd_workspace(1, 1, 4, 32, 64, 1, 20, 20, 1, 5, 2, 0, 1, 1) == -1
+    assert lib.lvg_convnd_workspace(2, 1, 4, 32, 64, 1, 20, 20, 1, 3, 3, 0, 1, 1) == -1
 
 
 def test_plugins_reject_cpu_tensors():

@@ -20,7 +20,7 @@ FIELDS = ['wgroups', 'rows', 'mt', 'kc', 'nblk', 'nimg', 'lo_blk', 'to', 'ho', '
           'a_resident', 'a_stage', 'b_step', 'b_bytes', 'b_box', 'stage_bytes', 'ostride', 'hos', 'wos', 'm64', 'ncw']
 WFIELDS = ['split', 'cpad_a', 'cpad_b', 'nt', 'ntiles', 'mt', 'nsplit', 'ablk', 'khc', 'nseg', 'ps', 'rh', 'stages', 'a_stage', 'b_stage',
            'stage_bytes', 'tail_bytes', 'smem', 'seg_w0', 'seg_w1', 'seg_w2', 'seg_w3', 'seg_x00', 'seg_x01', 'seg_x02', 'seg_x03',
-           'pointwise', 'mrows']
+           'unused', 'mrows']
 SMEM = 227 * 1024                      # dynamic shared memory of one CTA on sm_90
 DTYPES = {0: torch.float32, 1: torch.float16}
 
@@ -81,8 +81,6 @@ def wgrad_kernel_exists(taps, nt, split):
 
 def wgrad_plan_problems(q, wo, kw):
     bad = []
-    if q['pointwise']:
-        return bad
     if not wgrad_kernel_exists(q['khc'] * kw, q['nt'], q['split']):
         bad.append(f"no kernel for {q['khc'] * kw} taps x {q['nt']} columns")
     if q['smem'] > SMEM or q['stages'] < 2:

@@ -1,4 +1,4 @@
-"""Bit-exact checks of the convolution kernels (csrc/conv_igemm.cu, conv2d_tc.cu, conv_pointwise.cu, fir1d.cu) over the
+"""Bit-exact checks of the convolution kernels (csrc/conv_igemm.cu, conv_pointwise.cu, fir1d.cu) over the
 envelope `ConvNdPlugin._in_envelope` declares.
 
 The operands are sparse small integers (x in {-1, 0, 1}, w in {-2, ..., 2}) or, for the fp32 split path, dyadic values
@@ -105,16 +105,14 @@ def split_exact(x, w, dy, stride, pad, groups, dtype):
 
 
 def plan_flags(plug, xs, ws, pad, groups, stride, dtype):
-    """(forward, input gradient, weight gradient) run by the streaming 1x1x1 kernels instead of the engine?"""
+    """(forward, input gradient) run by the streaming 1x1x1 kernels instead of the engine?"""
     args, _, _, _ = plug._args(tuple(xs), tuple(ws), pad, groups, dtype)
     out = (ctypes.c_int * 48)()
     flags = []
     for mode in (0, 1):
         assert plug._lib.lvg_convnd_plan(mode, *args, stride, out, 48) == 0, plug._lib.lvg_last_error().decode()
         flags.append(bool(out[47]))
-    w_out = (ctypes.c_int * 32)()
-    assert plug._lib.lvg_convnd_wgrad_plan(*args, w_out, 32) == 0, plug._lib.lvg_last_error().decode()
-    return flags + [bool(w_out[26])]
+    return flags
 
 
 # ---- shapes: (x shape, w shape, padding (t, h, w), stride, groups), pairwise over the envelope's axes
@@ -306,16 +304,18 @@ def test_functional_proxy_strided_wide_rows_exact(dtype, stride, W, k):
     assert_exact(wa.grad, dwe, adw, dtype, 1.0, 'F.conv2d weight gradient')
 
 
-# ---- the conv2d plugin's fp16 entry points (conv2d_tc.cu)
+# ---- conv2d_gradfix.conv2d (the reference's entry point) in fp16: forward, then both gradients through autograd
 @pytest.mark.parametrize('xs,ws,pad,groups', [((1, 4 * 24, 20, 26), (4 * 40, 24, 3, 3), (2, 2), 4), ((2, 40, 17, 130), (24, 40, 1, 1), (0, 0), 1),
                                               ((2, 16, 1, 9), (70, 16, 3, 3), (1, 1), 1)])
-def test_conv2d_plugin_exact(xs, ws, pad, groups):
-    p2 = custom_ops.get_plugin('conv2d_plugin')
+def test_conv2d_gradfix_exact(xs, ws, pad, groups):
+    from torch_utils.ops import conv2d_gradfix, conv_nd
     x, w = ints(xs, 41, 1, 0.5), ints(ws, 42, 2, 0.5)
-    y = p2.fprop(x.half(), w.half(), pad, groups)
+    xa, wa = x.half().requires_grad_(True), w.half().requires_grad_(True)
+    assert conv_nd._native_ok(xa, wa, 1, pad, 1, groups), 'expected the engine'
+    y = conv2d_gradfix.conv2d(xa, wa, padding=pad, groups=groups)
     dy = ints(tuple(y.shape), 43, 1, 0.5)
-    dx = p2.dgrad(dy.half(), w.half(), tuple(xs), pad, groups)
-    dw = p2.wgrad(x.half(), dy.half(), tuple(ws), pad, groups)
+    dx, dw = torch.autograd.grad(y, [xa, wa], dy.half())
+    y = y.detach()
     (ye, dxe, dwe), (ay, adx, adw) = split_exact(x, w, dy, 1, (0,) + pad, groups, torch.float16)
     assert_exact(y, ye, ay, torch.float16, 1.0, 'conv2d fprop')
     assert_exact(dx, dxe, adx, torch.float16, 1.0, 'conv2d dgrad')
@@ -358,10 +358,10 @@ def test_modconv_exact(plug, xs, ws, pad, dtype):
     assert_exact(dyy, exp[4], ab[4], torch.float32, 1.0 / 8, 'modconv sum dy*y')
 
 
-# ---- fp32 streaming kernels: pointwise 1x1x1 forward / input gradient / weight gradient, depthwise long FIR
+# ---- fp32 streaming kernels: pointwise 1x1x1 forward / input gradient (the weight gradient of these shapes: the engine),
+# depthwise long FIR
 @pytest.mark.parametrize('xs,ws', [((2, 3, 5, 16, 20), (32, 3, 1, 1, 1)), ((2, 64, 3, 36, 64), (3, 64, 1, 1, 1)), ((3, 16, 2, 6, 8), (24, 16, 1, 1, 1))])
-def test_pointwise_kernels_exact(plug, monkeypatch, xs, ws):
-    monkeypatch.setenv('LVG_POINTWISE_WGRAD', '1')
+def test_pointwise_kernels_and_engine_wgrad_exact(plug, xs, ws):
     assert all(plan_flags(plug, xs, ws, [0, 0, 0], 1, 1, torch.float32)), 'expected the streaming kernels'
     x, w = ints(xs, 61, 1, 0.5), ints(ws, 62, 2, 0.5)
     dy = ints((xs[0], ws[0]) + xs[2:], 63, 1, 0.5)
@@ -371,7 +371,7 @@ def test_pointwise_kernels_exact(plug, monkeypatch, xs, ws):
     (ye, dxe, dwe), (ay, adx, adw) = split_exact(x, w, dy, 1, (0, 0, 0), 1, torch.float16)       # full products
     assert_exact(y, ye, ay, torch.float32, 1.0, 'pw_conv forward')
     assert_exact(dx, dxe, adx, torch.float32, 1.0, 'pw_conv input gradient')
-    assert_exact(dw, dwe, adw, torch.float32, 1.0, 'pw_wgrad')
+    assert_exact(dw, dwe, adw, torch.float32, 1.0, 'engine weight gradient')
 
 
 @pytest.mark.parametrize('lead', range(6))

@@ -291,13 +291,13 @@ def test_convnd_resident_weight_slots_change_nothing(plug, monkeypatch, name, xs
 
 
 @pytest.mark.parametrize('xs,ws', [((2, 3, 5, 16, 20), (32, 3, 1, 1, 1)), ((2, 64, 3, 36, 64), (3, 64, 1, 1, 1)), ((3, 16, 2, 6, 8), (24, 16, 1, 1, 1))])
-def test_pointwise_weight_gradient_both_paths(plug, monkeypatch, xs, ws):
-    """1x1x1 fp32 weight gradients with <= 512 channel pairs: the engine (default) and the streaming kernel
-    (LVG_POINTWISE_WGRAD=1, csrc/conv_pointwise.cu) against float64."""
+def test_pointwise_weight_gradient_both_paths(plug, xs, ws):
+    """1x1x1 fp32 weight gradients of few-channel layers (the forward and input gradient take the streaming kernels, the
+    weight gradient the engine) against float64, through both entry points that produce one: lvg_convnd_wgrad and the
+    one-call lvg_convnd_backward."""
     x = rnd(xs, 51).float()
     dy = rnd((xs[0], ws[0]) + xs[2:], 52).float()
     gw = _wgrad_ref(x, dy, ws, (0, 0, 0))
-    for flag in ('0', '1'):
-        monkeypatch.setenv('LVG_POINTWISE_WGRAD', flag)
-        dw = plug.wgrad(x, dy, ws, (0, 0, 0), 1)
-        assert float((dw.double() - gw).abs().max()) <= 5e-5 * float(gw.abs().max()), flag
+    w = rnd(ws, 53).float()
+    for path, dw in (('wgrad', plug.wgrad(x, dy, ws, (0, 0, 0), 1)), ('backward', plug.backward(x, dy, w, (0, 0, 0), 1)[1])):
+        assert float((dw.double() - gw).abs().max()) <= 5e-5 * float(gw.abs().max()), path

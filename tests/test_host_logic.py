@@ -203,61 +203,6 @@ def test_conv2d_resample(name):
     assert_close(dw, _CV[f'{name}/dw'], 1e-5, 'dw')
 
 
-class _TorchConvNative:
-    """Stand-in for the convolution plugin: same methods, torch arithmetic (CPU). Counts the calls."""
-
-    def __init__(self):
-        self.calls = dict(fprop=0, dgrad=0, wgrad=0)
-
-    def supported(self, x, w, stride, padding, dilation, groups):
-        return True
-
-    def fprop(self, x, w, padding, groups):
-        self.calls['fprop'] += 1
-        return torch.nn.functional.conv2d(x, w, padding=padding, groups=groups)
-
-    def dgrad(self, dy, w, x_shape, padding, groups):
-        self.calls['dgrad'] += 1
-        return torch.nn.grad.conv2d_input(x_shape, w, dy, padding=padding, groups=groups)
-
-    def wgrad(self, x, dy, w_shape, padding, groups):
-        self.calls['wgrad'] += 1
-        return torch.nn.grad.conv2d_weight(x, w_shape, dy, padding=padding, groups=groups)
-
-
-@pytest.mark.parametrize('mode,cin,expect_native', [('auto', 8, True), ('auto', 80, False), ('1', 80, True), ('0', 8, False)])
-def test_conv2d_autograd_wiring_and_wgrad_policy(monkeypatch, mode, cin, expect_native):
-    # _Conv2d / _Conv2dDgrad / _Conv2dWgrad against torch's own convolution autograd (first and second order), and which
-    # weight-gradient implementation the LVG_NATIVE_WGRAD policy picks (native for <= 64 input channels per group)
-    native = _TorchConvNative()
-    monkeypatch.setattr(conv2d_gradfix, '_native', native)
-    if mode == 'auto':
-        monkeypatch.delenv('LVG_NATIVE_WGRAD', raising=False)
-    else:
-        monkeypatch.setenv('LVG_NATIVE_WGRAD', mode)
-    gen = torch.Generator().manual_seed(cin)
-    g = 2
-    x = torch.randn(2, g * cin, 7, 6, generator=gen, dtype=torch.float64, requires_grad=True)
-    w = (torch.randn(g * 4, cin, 3, 3, generator=gen, dtype=torch.float64) / 10).requires_grad_(True)
-    y = conv2d_gradfix._Conv2d.apply(x, w, (1, 1), g)
-    ref = torch.nn.functional.conv2d(x, w, padding=1, groups=g)
-    assert torch.allclose(y, ref)
-    dy = torch.randn(y.shape, generator=gen, dtype=torch.float64)
-    gx, gw = torch.autograd.grad(y, [x, w], dy, create_graph=True)
-    rx, rw = torch.autograd.grad(ref, [x, w], dy, create_graph=True)
-    assert torch.allclose(gx, rx) and torch.allclose(gw, rw)
-    assert (native.calls['wgrad'] == 1) == expect_native
-    # R1-style second order: d/dw and d/dx of |dy/dx|^2 + |dy/dw|^2
-    h = torch.autograd.grad(gx.square().sum() + gw.square().sum(), [x, w])
-    hr = torch.autograd.grad(rx.square().sum() + rw.square().sum(), [x, w])
-    for a, b in zip(h, hr):
-        assert torch.allclose(a, b, rtol=1e-9, atol=1e-12)
-    with conv2d_gradfix.no_weight_gradients():
-        y2 = conv2d_gradfix._Conv2d.apply(x, w, (1, 1), g)
-        gx2, gw2 = torch.autograd.grad(y2, [x, w], dy, allow_unused=True)
-        assert gw2 is None and torch.allclose(gx2, rx)
-
-
 def test_conv2d_gradfix_surface():
     assert conv2d_gradfix.enabled is False and conv2d_gradfix.weight_gradients_disabled is False
     with conv2d_gradfix.no_weight_gradients():

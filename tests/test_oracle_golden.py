@@ -73,7 +73,7 @@ def test_conv_and_fma():
 
 
 def test_conv2d_wgrad_restatement_matches_torch_autograd():
-    # the float64 restatement used to check lvg_conv2d_wgrad against the weight gradient torch derives for F.conv2d
+    # the oracle's float64 weight gradient (smoke() checks the engine's against it) equals the one torch derives for F.conv2d
     import torch
     gen = torch.Generator().manual_seed(1)
     for (n, g, cin, cout, h, w, k, pad) in ((2, 2, 3, 4, 5, 7, 3, 1), (1, 1, 5, 2, 6, 4, 3, 2), (3, 2, 4, 4, 5, 5, 1, 0)):

@@ -31,7 +31,6 @@ def plan(dtype_code, n, groups, cin, cout, t, h, w, kt, kh, kw, pt, ph, pw):
     q = {k: int(out[i]) for i, k in enumerate(FIELDS)}
     q['seg_w'] = [int(out[18 + j]) for j in range(4)]
     q['seg_x0'] = [int(out[22 + j]) for j in range(4)]
-    q['pointwise'] = int(out[26])
     q['mrows'] = int(out[27])
     return q
 
@@ -167,8 +166,6 @@ def test_wgrad_kernel_addressing_replayed_on_cpu(case, dtype_code, monkeypatch):
         monkeypatch.setenv('LVG_WGRAD_FOLD', str(fold))
         monkeypatch.setenv('LVG_WGRAD_COMPACT', str(compact))
         q = plan(dtype_code, n, groups, cin, cout, T, H, W, *k3, *pad3)
-        if q['pointwise']:
-            continue
         assert q['khc'] == (k3[1] if (fold and k3[1] > 1 and cin <= 64 and k3[1] * k3[2] * 32 <= 256) else 1)
         assert q['ablk'] == (-(-cout // 16) * 2 if (compact and cout < 128) else 16)
         assert q['mrows'] == (64 if (compact and cout <= 64) else 128)
@@ -197,8 +194,6 @@ def test_wgrad_plans_of_the_lowres_networks_fit_the_hardware(monkeypatch):
         xs, ws = c['x'], c['w']
         pad = c['padding'] if isinstance(c['padding'], (list, tuple)) else [c['padding']] * 3
         q = plan(0, 8, 1, ws[1], ws[0], xs[2], xs[3], xs[4], ws[2], ws[3], ws[4], *pad)
-        if q['pointwise']:
-            continue
         seen += 1
         assert q['smem'] <= 227 * 1024 and q['stages'] >= 2, (c, q)
         assert q['khc'] * ws[4] * q['nt'] <= 256 and q['nt'] % 32 == 0 and q['rh'] + q['khc'] - 1 <= 256 and q['ps'] <= 128, (c, q)

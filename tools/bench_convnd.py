@@ -57,7 +57,7 @@ def card():
 
 def executed_flops(lib, args, mode, split):
     """tensor-core multiply-adds x 2 that the planned launch issues for one pass (mode 0 forward, 1 input gradient,
-    2 weight gradient), or None on the streaming 1x1x1 kernels. args = the plugin's [dtype, n, groups, cin, cout, t, h, w,
+    2 weight gradient), or None when the forward or input gradient runs on the streaming 1x1x1 kernels. args = the plugin's [dtype, n, groups, cin, cout, t, h, w,
     kt, kh, kw, pad_t, pad_h, pad_w]."""
     dt, n, groups, cin, cout, t, h, wd, kt, kh, kw, pt, ph, pw = args
     prods = 3 if split else 1
@@ -71,8 +71,6 @@ def executed_flops(lib, args, mode, split):
         return 2.0 * total_tiles * (2 * 64 * ncw) * (kc * 16 * kt * kh * kw) * prods
     out = (ctypes.c_int * 32)()
     assert lib.lvg_convnd_wgrad_plan(*args, out, 32) == 0, lib.lvg_last_error().decode()
-    if out[26]:
-        return None
     nt, ntiles, mt, nseg, ps, rh, mrows = out[3], out[4], out[5], out[9], out[10], out[11], out[27]
     to, ho = t + 2 * pt - kt + 1, h + 2 * ph - kh + 1
     kpix = sum(-(-min(rh, ho - r0) * ps // 16) * 16 for r0 in range(0, ho, rh))
@@ -138,7 +136,6 @@ def main():
         return lres_table(a.filter)
     pat = a.filter
     plug = custom_ops.get_plugin('convnd_plugin')
-    old = custom_ops.get_plugin('conv2d_plugin')
     print(f'# {card()}; TFLOP/s = 2*N*Cout*Cin*taps*out_pixels / time; cuDNN fp32 runs with TF32 off (as the reference)')
     print(f'# {"shape":58s} {"fprop":>22s} {"dgrad":>22s} {"wgrad":>22s}   ms (TFLOP/s): ours | cudnn')
     cases = [
@@ -185,11 +182,7 @@ def main():
             a = timeit(ours)
             b = timeit(theirs, iters=3, warmup=1) if not slow_cudnn else float('nan')
             cells.append(f'{a:7.3f} ({flops / a / 1e9:5.0f}) |{b:7.3f}')
-        extra = ''
-        if nd == 2 and dt == torch.float16 and old.supported(x, w, (1, 1), pad, (1, 1), groups):
-            extra = f'  r1 kernels: {timeit(lambda: old.fprop(x, w, pad, groups)):.3f} / {timeit(lambda: old.dgrad(dy, w, xs, pad, groups)):.3f}' \
-                    f' / {timeit(lambda: old.wgrad(x, dy, ws, pad, groups)) if (groups > 1) else float("nan"):.3f}'
-        print(f'{name:60s} {cells[0]:>22s} {cells[1]:>22s} {cells[2]:>22s}  err {err:.1e}{extra}', flush=True)
+        print(f'{name:60s} {cells[0]:>22s} {cells[1]:>22s} {cells[2]:>22s}  err {err:.1e}', flush=True)
         del x, w, y, dy, ref
 
 

@@ -53,7 +53,6 @@ def main():
     pat = sys.argv[1] if len(sys.argv) > 1 else ''
     ref = ref_cuda.load()
     assert ref.bias_act._init() and ref.upfirdn2d._init() and ref.filtered_lrelu._init()
-    conv2d_gradfix.install_native(True)
     print(f'# {torch.cuda.get_device_name()}  torch {torch.__version__}; reference = its own plugins (oracle/_ref) + its own Python wrappers')
     print(f'# {"op / signature":64s} {"ours fwd":>9s} {"ref fwd":>9s} {"x":>6s} | {"ours f+b":>9s} {"ref f+b":>9s} {"x":>6s}   (ms)')
     worst = []

@@ -113,18 +113,18 @@ def main():
                                       ('L10 389->256 92x148', 16, 389, 256, 92, 148), ('L0 27->512 29x36', 64, 27, 512, 29, 36)):
         if pat not in 'conv2d cudnn':
             continue
+        from torch_utils import custom_ops
         from torch_utils.ops import conv2d_gradfix
         x = torch.randn(1, nt * cin, h, w, device=DEV, dtype=torch.float16)
         wt = torch.randn(nt * cout, cin, 3, 3, device=DEV, dtype=torch.float16) / 70
         flops = 2.0 * nt * cout * cin * 9 * (h + 2) * (w + 2)
-        conv2d_gradfix.install_native(True)
         ms = timeit(lambda: conv2d_gradfix.conv2d(x, wt, padding=2, groups=nt))
         print(f'conv2d engine grouped fp16 {name} NT={nt}: {ms:8.3f} ms {flops / ms / 1e9:8.1f} TFLOP/s', flush=True)
         if not (cin == 208 and nt > 4):     # cuDNN takes ~0.2 s on this shape: time it once at small NT only
             ms = timeit(lambda: torch.nn.functional.conv2d(x, wt, padding=2, groups=nt), iters=3, warmup=1)
             print(f'conv2d cudnn   grouped fp16 {name} NT={nt}: {ms:8.3f} ms {flops / ms / 1e9:8.1f} TFLOP/s', flush=True)
         # weight gradient: the engine vs aten::convolution_backward (cuDNN)
-        plug = conv2d_gradfix._native
+        plug = custom_ops.get_plugin('convnd_plugin')
         y = conv2d_gradfix.conv2d(x, wt, padding=2, groups=nt)
         dy = torch.randn_like(y)
         ms = timeit(lambda: plug.wgrad(x, dy, tuple(wt.shape), (2, 2), nt))

@@ -47,11 +47,12 @@ x = torch.randn(16, 128, 166, 278, device=DEV, dtype=torch.float16)
 bb = torch.randn(128, device=DEV, dtype=torch.float16)
 run('flrelu_u2d2', lambda: filtered_lrelu.filtered_lrelu(x, k12, k12, bb, up=2, down=2, padding=[9, 8, 9, 8], clamp=256))
 
+from torch_utils import custom_ops  # noqa: E402
 from torch_utils.ops import conv2d_gradfix  # noqa: E402
-conv2d_gradfix.install_native(True)
-xc = torch.randn(1, 16 * 539, 92, 148, device=DEV, dtype=torch.float16)
+convnd = custom_ops.get_plugin('convnd_plugin')
+xc =torch.randn(1, 16 * 539, 92, 148, device=DEV, dtype=torch.float16)
 wc = torch.randn(16 * 512, 539, 3, 3, device=DEV, dtype=torch.float16) / 70
 run('conv_l8', lambda: conv2d_gradfix.conv2d(xc, wc, padding=2, groups=16))
 yc = conv2d_gradfix.conv2d(xc, wc, padding=2, groups=16)
 dyc = torch.randn_like(yc)
-run('conv_wgrad_l8', lambda: conv2d_gradfix._native.wgrad(xc, dyc, tuple(wc.shape), (2, 2), 16))
+run('conv_wgrad_l8', lambda: convnd.wgrad(xc, dyc, tuple(wc.shape), (2, 2), 16))
