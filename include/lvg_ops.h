@@ -145,7 +145,10 @@ int lvg_upfirdn2d_sep(const void* x, const float* fx, const float* fy, void* y,
  *   write_signs != 0 : so written (forward with gradients)
  *   si != NULL       : signs read at offset (sx, sy) instead of evaluating lrelu/clamp (backward)
  *   neither          : plain forward
- * Returns LVG_UNSUPPORTED when no fused kernel covers (up, down, filter sizes).
+ * Returns LVG_UNSUPPORTED when no fused kernel covers (up, down, filter sizes),
+ * and for the resampling configurations (up or down > 1) when slope > 1.
+ * In read mode those configurations also need s_wbytes % 4 == 0 and si on a
+ * 4-byte boundary (LVG_ERR_ARG otherwise); 1x1 filters take any slope and rows.
  */
 int lvg_filtered_lrelu(const void* x, const float* fu, const float* fd, const void* b,
                        const uint8_t* si, void* y, uint8_t* so, int dtype,

@@ -1,7 +1,7 @@
 // Register-blocked separable polyphase FIR passes over shared-memory tiles.
 //
-// Building blocks of the fused filtered_lrelu kernel and of the single-launch
-// separable upfirdn2d kernel. Every pass reads a tile from shared memory,
+// Building blocks of the single-launch separable upfirdn2d kernel
+// (upfirdn2d_tiled.cu). Every pass reads a tile from shared memory,
 // keeps the (compile-time sized) filter in registers and lets each thread
 // produce a short run of outputs from one contiguous window of inputs, so a
 // shared-memory load feeds ~4-5 FMAs instead of 1 (LDS issue rate is 1/4 of the
@@ -54,94 +54,6 @@ template <class Begin, class Put> struct EmitCtx<ItemEmitter<Begin, Put>> {
     __device__ __forceinline__ EmitCtx(ItemEmitter<Begin, Put>& e, int pl, int col) : ctx(e.begin(pl, col)) {}
     __device__ __forceinline__ void put(ItemEmitter<Begin, Put>& e, int row, float v) const { e.put(ctx, row, v); }
 };
-
-// ---------------------------------------------------------------------------
-// up-sampling along x.  in: [rows][pin], out: [rows][pout] (phase-aligned axis)
-// groups = number of input-aligned groups to produce per row (each UP outputs).
-template <int UP, int F, int R, int NTHREADS>
-__device__ __forceinline__ void up_x(const float* __restrict__ in, int pin, float* __restrict__ out, int pout,
-                                     int rows, int groups, const float* __restrict__ s_taps)
-{
-    static_assert(F % UP == 0, "filter length must be a multiple of the up-sampling factor");
-    constexpr int K = F / UP;
-    constexpr int RW = R;                 // rows per warp (= per-thread input advance)
-    constexpr int GW = kWarp / RW;        // column groups per warp
-    float g[F];
-#pragma unroll
-    for (int i = 0; i < F; i++) g[i] = s_taps[i];
-    const int warp = threadIdx.x / kWarp, lane = threadIdx.x % kWarp;
-    const int gthreads = (groups + R - 1) / R;                 // thread-level groups per row
-    const int n_rt = (rows + RW - 1) / RW, n_gt = (gthreads + GW - 1) / GW;
-    const FastDiv by_gt(n_gt);
-    for (int wi = warp; wi < n_rt * n_gt; wi += NTHREADS / kWarp) {
-        const int rt = by_gt.div(wi), gt = wi - rt * n_gt;
-        const int r = rt * RW + lane % RW;
-        const int tg = gt * GW + lane / RW;
-        if (r < rows && tg < gthreads) {
-            const float* src = in + r * pin + tg * R;
-            float v[K + R];
-#pragma unroll
-            for (int i = 0; i < K + R; i++) v[i] = src[i];
-            float* dst = out + r * pout + tg * R * UP;
-#pragma unroll
-            for (int j = 0; j < R; j++) {
-#pragma unroll
-                for (int ph = 0; ph < UP; ph++) {
-                    float acc = 0.f;
-#pragma unroll
-                    for (int k = 0; k < K; k++)
-                        acc = fmaf(g[(UP - ph) % UP + k * UP], v[j + (ph > 0 ? 1 : 0) + k], acc);
-                    dst[j * UP + ph] = acc;
-                }
-            }
-        }
-    }
-}
-
-// ---------------------------------------------------------------------------
-// up-sampling along y.  in: [nplanes][plane_rows][pin]; for every plane produces rows a = UP*q + r
-// for q < groups and every column < cols, and hands (plane, row a, col, value) to `emit`.
-// Lanes run over the flattened (plane, column) index so narrow planes still fill a warp.
-
-template <int UP, int F, int R, int NTHREADS, class Emit>
-__device__ __forceinline__ void up_y(const float* __restrict__ in, int pin, int cols, int groups,
-                                     const float* __restrict__ s_taps, Emit emit, int nplanes = 1, int plane_rows = 0)
-{
-    static_assert(F % UP == 0, "filter length must be a multiple of the up-sampling factor");
-    constexpr int K = F / UP;
-    float g[F];
-#pragma unroll
-    for (int i = 0; i < F; i++) g[i] = s_taps[i];
-    const int warp = threadIdx.x / kWarp, lane = threadIdx.x % kWarp;
-    const int gthreads = (groups + R - 1) / R;
-    const int vcols = nplanes * cols;
-    const int n_cc = (vcols + kWarp - 1) / kWarp;
-    const FastDiv by_cols(cols), by_cc(n_cc);
-    for (int wi = warp; wi < gthreads * n_cc; wi += NTHREADS / kWarp) {
-        const int tg = by_cc.div(wi), cc = wi - tg * n_cc;
-        const int vc = cc * kWarp + lane;
-        if (vc < vcols) {
-            const int pl = nplanes > 1 ? by_cols.div(vc) : 0;
-            const int col = vc - pl * cols;
-            const float* src = in + (pl * plane_rows + tg * R) * pin + col;
-            float v[K + R];
-#pragma unroll
-            for (int i = 0; i < K + R; i++) v[i] = src[i * pin];
-            const EmitCtx<Emit> ec(emit, pl, col);
-#pragma unroll
-            for (int j = 0; j < R; j++) {
-#pragma unroll
-                for (int ph = 0; ph < UP; ph++) {
-                    float acc = 0.f;
-#pragma unroll
-                    for (int k = 0; k < K; k++)
-                        acc = fmaf(g[(UP - ph) % UP + k * UP], v[j + (ph > 0 ? 1 : 0) + k], acc);
-                    ec.put(emit, (tg * R + j) * UP + ph, acc);
-                }
-            }
-        }
-    }
-}
 
 // ---------------------------------------------------------------------------
 // down-sampling along x.  in: [rows][pin] read from column offset `xoff`;
@@ -222,10 +134,9 @@ __device__ __forceinline__ void down_y(const float* __restrict__ in, int pin, in
 // ===========================================================================================
 // Paired variants: every thread produces TWO outputs per coefficient load, as two scalar FMAs
 // (sm_90 has no packed f32x2 FMA), which halves the shared-memory reads of the inner loops.
-// The two outputs of a pair lie along the axis that is NOT being filtered:
-//   y passes: columns L and L + 32 of a 64-column span (lane L; all accesses stay stride-1 32-bit)
-//   x passes: rows r and r + RW of the same warp item (two conflict-free 32-bit loads)
-// Coefficients are held as (g, g) pairs.
+// The two outputs of a pair lie along the axis that is NOT being filtered: rows r and r + RW of
+// the same warp item (two conflict-free 32-bit loads). The paired y passes of upfirdn2d_tiled.cu
+// pair columns L and L + 32 of a 64-column span instead. Coefficients are held as (g, g) pairs.
 
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 
@@ -273,52 +184,6 @@ __device__ __forceinline__ void up_x2(const float* __restrict__ in, int pin, flo
     }
 }
 
-// Packed y pass: a warp item covers TWO 32-column chunks; lane L owns columns L and L + 32 of the
-// item's 64-column span, so every shared-memory access stays a stride-1 32-bit access (no pitch
-// or alignment constraints) while the FMAs are issued in pairs. Same interface as up_y.
-template <int UP, int F, int R, int NTHREADS, class Emit>
-__device__ __forceinline__ void up_y2(const float* __restrict__ in, int pin, int cols, int groups,
-                                      const float* __restrict__ s_taps, Emit emit, int nplanes = 1, int plane_rows = 0)
-{
-    static_assert(F % UP == 0, "filter length must be a multiple of the up-sampling factor");
-    constexpr int K = F / UP;
-    float2 g[F];
-#pragma unroll
-    for (int i = 0; i < F; i++) g[i] = make_float2(s_taps[i], s_taps[i]);
-    const int warp = threadIdx.x / kWarp, lane = threadIdx.x % kWarp;
-    const int gthreads = (groups + R - 1) / R;
-    const int vcols = nplanes * cols;
-    const int n_cc = (vcols + 2 * kWarp - 1) / (2 * kWarp);
-    const FastDiv by_cols(cols), by_cc(n_cc);
-    for (int wi = warp; wi < gthreads * n_cc; wi += NTHREADS / kWarp) {
-        const int tg = by_cc.div(wi), cc = wi - tg * n_cc;
-        const int va = cc * 2 * kWarp + lane, vb = va + kWarp;
-        if (va < vcols) {
-            const bool has_b = vb < vcols;
-            const int pla = nplanes > 1 ? by_cols.div(va) : 0, cola = va - pla * cols;
-            const int plb = has_b ? (nplanes > 1 ? by_cols.div(vb) : 0) : pla, colb = has_b ? vb - plb * cols : cola;
-            const float* sa = in + (pla * plane_rows + tg * R) * pin + cola;
-            const float* sb = in + (plb * plane_rows + tg * R) * pin + colb;
-            float2 v[K + R];
-#pragma unroll
-            for (int i = 0; i < K + R; i++) v[i] = make_float2(sa[i * pin], sb[i * pin]);
-            const EmitCtx<Emit> ea(emit, pla, cola), eb(emit, plb, colb);
-#pragma unroll
-            for (int j = 0; j < R; j++) {
-#pragma unroll
-                for (int ph = 0; ph < UP; ph++) {
-                    float2 acc = make_float2(0.f, 0.f);
-#pragma unroll
-                    for (int k = 0; k < K; k++)
-                        acc = ffma2(g[(UP - ph) % UP + k * UP], v[j + (ph > 0 ? 1 : 0) + k], acc);
-                    ea.put(emit, (tg * R + j) * UP + ph, acc.x);
-                    if (has_b) eb.put(emit, (tg * R + j) * UP + ph, acc.y);
-                }
-            }
-        }
-    }
-}
-
 template <int DOWN, int F, int R, int NTHREADS>
 __device__ __forceinline__ void down_x2(const float* __restrict__ in, int pin, int xoff, float* __restrict__ out, int pout,
                                         int rows, int outs, const float* __restrict__ s_taps)
@@ -359,53 +224,7 @@ __device__ __forceinline__ void down_x2(const float* __restrict__ in, int pin, i
     }
 }
 
-template <int DOWN, int F, int R, int NTHREADS, class Emit>
-__device__ __forceinline__ void down_y2(const float* __restrict__ in, int pin, int yoff, int cols, int outs,
-                                        const float* __restrict__ s_taps, Emit emit, int nplanes = 1, int plane_rows = 0)
-{
-    constexpr int NIN = (R - 1) * DOWN + F;
-    float2 g[F];
-#pragma unroll
-    for (int i = 0; i < F; i++) g[i] = make_float2(s_taps[i], s_taps[i]);
-    const int warp = threadIdx.x / kWarp, lane = threadIdx.x % kWarp;
-    const int gthreads = (outs + R - 1) / R;
-    const int vcols = nplanes * cols;
-    const int n_cc = (vcols + 2 * kWarp - 1) / (2 * kWarp);
-    const FastDiv by_cols(cols), by_cc(n_cc);
-    for (int wi = warp; wi < gthreads * n_cc; wi += NTHREADS / kWarp) {
-        const int tg = by_cc.div(wi), cc = wi - tg * n_cc;
-        const int va = cc * 2 * kWarp + lane, vb = va + kWarp;
-        if (va < vcols) {
-            const bool has_b = vb < vcols;
-            const int pla = nplanes > 1 ? by_cols.div(va) : 0, cola = va - pla * cols;
-            const int plb = has_b ? (nplanes > 1 ? by_cols.div(vb) : 0) : pla, colb = has_b ? vb - plb * cols : cola;
-            const float* sa = in + (pla * plane_rows + yoff + tg * R * DOWN) * pin + cola;
-            const float* sb = in + (plb * plane_rows + yoff + tg * R * DOWN) * pin + colb;
-            float2 v[NIN];
-#pragma unroll
-            for (int i = 0; i < NIN; i++) v[i] = make_float2(sa[i * pin], sb[i * pin]);
-            const EmitCtx<Emit> ea(emit, pla, cola), eb(emit, plb, colb);
-#pragma unroll
-            for (int j = 0; j < R; j++) {
-                float2 acc = make_float2(0.f, 0.f);
-#pragma unroll
-                for (int t = 0; t < F; t++) acc = ffma2(g[t], v[j * DOWN + t], acc);
-                if (tg * R + j < outs) {
-                    ea.put(emit, tg * R + j, acc.x);
-                    if (has_b) eb.put(emit, tg * R + j, acc.y);
-                }
-            }
-        }
-    }
-}
-
 __host__ __device__ constexpr int even_pitch(int w) { return (w + 1) & ~1; }
-
-// filter taps global -> shared, oriented for correlation: g[t] = flip ? f[t] : f[F-1-t]
-__device__ __forceinline__ void load_taps(float* s_taps, const float* __restrict__ f, int n, bool flip)
-{
-    for (int i = threadIdx.x; i < n; i += blockDim.x) s_taps[i] = flip ? f[i] : f[n - 1 - i];
-}
 
 __host__ __device__ constexpr int odd_pitch(int w) { return w | 1; }
 __host__ __device__ constexpr int round_up(int a, int b) { return (a + b - 1) / b * b; }

@@ -72,8 +72,8 @@ __host__ __device__ constexpr int mid_extent(int n)
 
 
 // ---- y passes that store straight to global memory.
-// Same item decomposition as fir::up_y2 / fir::down_y2 (lane L owns columns L and L + 32 of a 64-column span,
-// R groups / outputs along y per item), but the store addresses are formed ONCE per item as two 64-bit column
+// Paired like the x passes of fir_passes.cuh, but along columns: lane L owns columns L and L + 32 of a 64-column span,
+// R groups / outputs along y per item. The store addresses are formed ONCE per item as two 64-bit column
 // pointers; every result then costs one pointer bump and one store, and items that lie completely inside the
 // tile (all but the first / last along y) take a path without row checks. `ys*` are element strides of y; the
 // host guarantees that one CTA's outputs span < 2^31 elements.

@@ -421,6 +421,12 @@ class FilteredLReluPlugin:
             if not (s.is_contiguous() and s.dtype == torch.uint8 and s.device == x.device and s.ndim == 4
                     and s.shape[0] == x.shape[0] and s.shape[1] == x.shape[1]):
                 raise RuntimeError('signs must be a contiguous uint8 [N, C, H, W/4] tensor on the same device as x')
+        if read_signs and up * down > 1 and (s.shape[3] % 4 or s.data_ptr() % 4):
+            # the resampling kernel reads sign rows as aligned 32-bit words: copy into zero-filled rows of a multiple of
+            # 4 bytes. A zero byte is code 0 ("unchanged"), as for samples outside the tensor, so the operator is the same.
+            padded = torch.zeros([*s.shape[:3], (s.shape[3] + 3) & ~3], dtype=torch.uint8, device=x.device)
+            padded[..., :s.shape[3]] = s
+            s = padded
         s_h, s_wb = (s.shape[2], s.shape[3]) if s is not None else (0, 0)
         fu_c, fd_c, b_c = fu.contiguous(), fd.contiguous(), b.contiguous()
         with _DeviceGuard(x):

@@ -1,5 +1,5 @@
 """Bit-exact checks of the resampling and activation kernels: upfirdn2d (csrc/upfirdn2d.cu, upfirdn2d_stream.cu,
-upfirdn2d_tiled.cu + fir_passes.cuh), filtered_lrelu (filtered_lrelu_v3.cuh, filtered_lrelu_fused.cu,
+upfirdn2d_tiled.cu + fir_passes.cuh), filtered_lrelu (filtered_lrelu_v3.cuh, filtered_lrelu.cu,
 filtered_lrelu_act.cu) and bias_act (bias_act.cu).
 
 Operands are sparse small integers (about 40 % zeros) and filters have dyadic taps k / 2^m with small k of both signs,
@@ -14,12 +14,9 @@ oracle (oracle/oracle.py) element for element; a wrong tap, halo row, tile seam 
 element by at least one unit. Sign tensors are compared as whole uint8 tensors, padding columns included.
 
 The case lists are plain data so that tests/test_ops_exact_host.py can check the operands and preconditions without a
-GPU. `test_routes_reached` runs every case under torch.profiler and asserts that each kernel family and template
+GPU. `test_kernel_routes_reached` runs every case under torch.profiler and asserts that each kernel family and template
 instance named in the case comments was launched."""
-import os
 import re
-import subprocess
-import sys
 import zlib
 
 import numpy as np
@@ -457,8 +454,8 @@ def test_upfirdn2d_exact(case, dtn):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# filtered_lrelu cases. cfg: (up, down, fu taps, fd taps); configurations 1-3 have fused kernels (v3 tiles 56 x 24,
-# and 31 x 16 for configuration 3; the scalar-access kernels use 64 x 24 / 64 x 32, chosen by tile_rows(oh), and 32 x 16).
+# filtered_lrelu cases. cfg: (up, down, fu taps, fd taps); configurations 1-3 have a fused kernel (v3 tiles 56 x 24,
+# and 31 x 16 for configuration 3) for slope <= 1; slope > 1 takes the composed path.
 
 FU12, FD12 = taps(12, 21, m=2, density=0.5), taps(12, 22, m=2, density=0.5)
 FU24, FD24 = taps(24, 23, m=2, density=0.3), taps(24, 24, m=2, density=0.3)
@@ -503,9 +500,9 @@ def _fl_cases():
                 c.append(flcase(f'c{cfg}_{oh}x{o}_p{px0}', cfg, 1 + (k % 2) * 2, 1 + (k % 3), oh, o, px0, py0,
                                 flip=bool(k % 2), gain=(1, 4)[k % 2]))
                 k += 1
-        # slope 2: the scalar-access kernels in every mode; oh 24 and 32 pick the 24- and 32-row tiles
+        # slope 2: the fused kernel declines (rc = -1), the composed path runs in every mode
         for oh in ((24, 32) if cfg != 3 else (16,)):
-            c.append(flcase(f'c{cfg}_slope2_oh{oh}', cfg, 1, 3, oh, 40, 9, 8, slope=2, family='scalar'))
+            c.append(flcase(f'c{cfg}_slope2_rc_oh{oh}', cfg, 1, 3, oh, 40, 9, 8, slope=2, family='composed'))
         c.append(flcase(f'c{cfg}_noclamp', cfg, 2, 3, 9, 17, 9, 9, clamp=None))
         c.append(flcase(f'c{cfg}_slope_half', cfg, 1, 2, 13, 20, -6, 9, slope=0.5, flip=True))
         c.append(flcase(f'c{cfg}_slope0_1', cfg, 1, 2, 7, 9, 9, -6, slope=0, gain=4))
@@ -677,8 +674,9 @@ def test_fl_exact(case, dtn):
 
 
 # read mode with random sign tensors: codes 0..3, tensors smaller / larger than the consumed extent, offsets of every
-# sign and residue. Rows of s_wb % 4 == 0 bytes at a word-aligned address take the vectorised v3 kernel (entries 0, 6-9),
-# s_wb % 4 != 0 or a 1-3 byte storage offset the scalar-access kernels (entries 1-5); fl_read_route() tells which.
+# sign and residue. Rows of s_wb % 4 == 0 bytes at a word-aligned address go to the v3 kernel as they are (entries 0,
+# 6-9); for s_wb % 4 != 0 or a 1-3 byte storage offset the plugin passes a zero-padded, aligned copy (entries 1-5).
+# fl_read_route() tells which.
 FL_READ = []
 for _cfg in (1, 2, 3):
     for _k, (_sx, _sy, _dh, _dwb, _off) in enumerate(((0, 0, 0, 0, 0), (-5, 3, -3, 1, 0), (6, -2, 4, 3, 0),
@@ -695,12 +693,14 @@ FL_READ.append(dict(case=flcase('read_composed', None, 1, 2, 6, 9, 4, 3, fu=FU8,
 
 
 def fl_read_route(rc):
-    """'v3' or 'scalar': the dispatch of lvg_filtered_lrelu in read mode (filtered_lrelu_fused.cu dispatch())."""
+    """'v3' or 'padded' for configurations 1-3: whether FilteredLReluPlugin.filtered_lrelu passes the sign tensor to
+    the v3 kernel as it is or as a zero-padded, aligned copy (custom_ops.py)."""
     case = rc['case']
     x, b, pad = fl_inputs(case)
     swb = max(1, orc.sign_shape(x.shape, case['fu'], case['fd'], case['up'], case['down'], pad)[3] + rc['dwb'])
-    v3 = case['cfg'] in CFGS and case['slope'] <= 1 and swb % 4 == 0 and rc['off'] % 4 == 0
-    return 'v3' if v3 else 'scalar' if case['cfg'] in CFGS else case['family']
+    if case['cfg'] not in CFGS:
+        return case['family']
+    return 'v3' if swb % 4 == 0 and rc['off'] % 4 == 0 else 'padded'
 
 
 def fl_read_inputs(rc):
@@ -737,17 +737,27 @@ def test_fl_read_random_signs(rc, dtn):
     run_fl_read(rc, dtn)
 
 
-def test_fl_scalar_engine_subprocess():
-    """The filtered_lrelu tests once more with LVG_FL_ENGINE=r2 (read once per process): the only way to run the
-    scalar-access kernels' slope <= 1 write path."""
-    if os.environ.get('LVG_FL_ENGINE') == 'r2':
-        pytest.skip('already running with LVG_FL_ENGINE=r2')
-    env = dict(os.environ, LVG_FL_ENGINE='r2')
-    r = subprocess.run([sys.executable, '-m', 'pytest', '-q', '-x', '-p', 'no:cacheprovider', '-m', 'gpu',
-                        os.path.abspath(__file__), '-k', 'test_fl_exact or test_fl_read_random_signs'],
-                       env=env, cwd=os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
-                       stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=1200)
-    assert r.returncode == 0, r.stdout[-6000:]
+@pytest.mark.parametrize('cfg', sorted(CFGS))
+def test_fl_fused_kernel_limits(cfg):
+    """Configurations 1-3: with slope > 1 the plugin reports rc = -1, so the caller runs the composed path; and the
+    library itself (no padded copy in between) refuses read-mode signs that do not start on a 4-byte boundary."""
+    from torch_utils import custom_ops as co
+    case = flcase(f'limits_c{cfg}', cfg, 1, 2, 7, 9, 9, 8)
+    x_np, b_np, pad = fl_inputs(case)
+    x, b, fu, fd = _fl_tensors(case, torch.float32, x_np, b_np)
+    up, down = case['up'], case['down']
+    _, _, rc = fl_plugin().filtered_lrelu(x, fu, fd, b, None, up, down, *pad, 0, 0, 1.0, 2.0, float('inf'), False, True)
+    assert rc == -1, f'configuration {cfg}: slope 2 reached a fused kernel'
+    n, c, sh, swb = orc.sign_shape(x_np.shape, case['fu'], case['fd'], up, down, pad)
+    assert swb % 4 == 0
+    s = torch.zeros(n * c * sh * swb + 4, dtype=torch.uint8, device=DEV)[1:1 + n * c * sh * swb].view(n, c, sh, swb)
+    y = torch.empty(orc.filtered_lrelu_out_shape(x_np.shape, case['fu'], case['fd'], up, down, pad), device=DEV)
+    lib = co.load_library()
+    rc = lib.lvg_filtered_lrelu(x.data_ptr(), fu.data_ptr(), fd.data_ptr(), b.data_ptr(), s.data_ptr(), y.data_ptr(),
+                                None, co._DTYPE_CODE[torch.float32], co._i4(x.shape), co._i4(x.stride()),
+                                co._i4(y.shape), co._i4(y.stride()), len(case['fu']), 0, len(case['fd']), 0, up, down,
+                                pad[0], pad[2], sh, swb, 0, 0, 1.0, 0.25, float('inf'), 0, 0, co._stream(x))
+    assert rc > 0 and b'4-byte boundary' in lib.lvg_last_error(), (rc, lib.lvg_last_error())
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -879,9 +889,6 @@ def expected_kernels():
     for g in geoms:
         for mode in (0, 1, 2):
             k[f'v3<{g}>,{mode}'] = rf'filtered_lrelu_v3_kernel<{T},lvg::flv3::Geom<{g}>,{mode}>'
-    for g in ('2,12,2,12,64,24', '2,12,2,12,64,32', '4,24,2,12,64,24', '4,24,2,12,64,32', '2,12,4,24,32,16'):
-        for mode in (0, 1, 2):
-            k[f'scalar<{g}>,{mode}'] = rf'filtered_lrelu_kernel<{T},{g},{mode}>'
     for mode in (0, 1, 2):
         k[f'1x1,{mode}'] = rf'filtered_lrelu_1x1_kernel<{T},{mode}>'
         k[f'act,{mode}'] = rf'filtered_lrelu_act_kernel<{T},{mode}>'
@@ -905,7 +912,7 @@ def all_runs():
             yield run_ba, (c, d)
 
 
-def test_routes_reached(monkeypatch):
+def test_kernel_routes_reached(monkeypatch):
     from torch.profiler import ProfilerActivity, profile
     names = set()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:

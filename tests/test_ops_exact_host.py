@@ -49,9 +49,9 @@ def test_filtered_lrelu_case_preconditions(case):
 
 
 def test_filtered_lrelu_read_routes():
-    """Both the vectorised v3 kernel and the scalar-access kernels get random sign tensors with non-zero, odd and
-    negative offsets, and tensors smaller and larger than the consumed extent."""
-    for route in ('v3', 'scalar'):
+    """Sign tensors passed to the v3 kernel as they are and as zero-padded, aligned copies both come with random
+    codes, non-zero, odd and negative offsets, and sizes smaller and larger than the consumed extent."""
+    for route in ('v3', 'padded'):
         rcs = [r for r in gx.FL_READ if gx.fl_read_route(r) == route]
         assert {r['case']['cfg'] for r in rcs} == {1, 2, 3}, route
         assert any(r['sx'] > 0 and r['sx'] % 2 for r in rcs) and any(r['sx'] < 0 for r in rcs), route
