@@ -276,6 +276,22 @@ int lvg_fir1d_depthwise(const float* x, const float* w, float* y, int n, int gro
                         void* workspace, int64_t workspace_bytes, void* stream);
 
 /*
+ * Separable 4-tap FIR over the T, H, W axes of a contiguous NCTHW tensor (fp32 or fp16, fp32 accumulation), and its exact
+ * adjoint. The operator P maps x [n][c][t_in][h_in][w_in] to y [n][c][t_out][h_out][w_out]; per axis, filt = 0 copies
+ * (in == out) and filt = 1 computes  out[m] = sum_j f[3 - j] * in[step * m + off + j]  (step 1 or 2, zero outside the
+ * input) -- Downsample3d's [1,3,3,1]/8 filter (discriminator_lres.py:186-213) at full rate or with step 2. fold = 1 stores
+ * the T axis of the filtered side (t_out even) as two phase blocks of channels: [n][2c][t_out / 2], t = 2 t' + p -> channel
+ * p * c + ci. f: 4 fp32 taps on the device. lvg_fir3d_adjoint takes the same arguments describing P and computes
+ * x' = P^T y' (y' laid out as P's output, x' as P's input).
+ */
+int lvg_fir3d(const void* x, const float* f, void* y, int dtype, int n, int c, int t_in, int h_in, int w_in, int t_out,
+              int h_out, int w_out, int filt_t, int filt_h, int filt_w, int step_t, int step_h, int step_w, int off_t,
+              int off_h, int off_w, int fold, void* stream);
+int lvg_fir3d_adjoint(const void* x, const float* f, void* y, int dtype, int n, int c, int t_in, int h_in, int w_in,
+                      int t_out, int h_out, int w_out, int filt_t, int filt_h, int filt_w, int step_t, int step_h,
+                      int step_w, int off_t, int off_h, int off_w, int fold, void* stream);
+
+/*
  * Post-processing of an all-reduced flat gradient buffer, in place and in one pass:
  *   g = g * scale;  NaN -> 0, +inf -> +limit, -inf -> -limit  (finite values untouched)
  * -- the `/ world_size * gain` + `nan_to_num(nan=0, posinf=1e5, neginf=-1e5)` tail of

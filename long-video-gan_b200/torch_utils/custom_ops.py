@@ -73,6 +73,8 @@ _SIGNATURES = {
     'lvg_modconv_workspace': (_c_i64, [_c_int] * 13),
     'lvg_modconv_fprop': (_c_int, [_c_void_p] * 5 + [_c_int] * 13 + [_c_void_p, _c_i64, _c_void_p]),
     'lvg_modconv_backward': (_c_int, [_c_void_p] * 10 + [_c_int] * 13 + [_c_void_p, _c_i64, _c_void_p]),
+    'lvg_fir3d': (_c_int, [_c_void_p] * 3 + [_c_int] * 19 + [_c_void_p]),
+    'lvg_fir3d_adjoint': (_c_int, [_c_void_p] * 3 + [_c_int] * 19 + [_c_void_p]),
 }
 
 LVG_UNSUPPORTED = -1
@@ -671,8 +673,41 @@ class ConvNdPlugin:
         return dx, dw, da, dyy
 
 
+class Fir3dPlugin:
+    """Separable 4-tap FIR over T, H, W of NCTHW tensors and its adjoint (no reference plugin: Downsample3d runs upfirdn2d
+    twice, discriminator_lres.py:197-213). ``axes``: per T, H, W a tuple (filt, step, off, n_in, n_out) of the operator P
+    (see lvg_fir3d in include/lvg_ops.h)."""
+
+    def __init__(self, lib):
+        self._lib = lib
+
+    def fir3d(self, x, f, axes, fold, adjoint=False):
+        """y = P x (adjoint=False, x laid out as P's input) or P^T x (x laid out as P's output)."""
+        if not x.is_cuda or f.device != x.device:
+            raise RuntimeError('fir3d: x and f must reside on one CUDA device')
+        if f.dtype != torch.float32 or f.numel() != 4 or x.ndim != 5:
+            raise RuntimeError('fir3d: needs a 5-D x and 4 float32 taps')
+        code = _dtype_code(x, 'fir3d')
+        x, f = x.contiguous(), f.contiguous()
+        n, c = x.shape[0], x.shape[1] // (2 if (fold and adjoint) else 1)
+        ins = [a[3] for a in axes]
+        outs = [a[4] for a in axes]
+        src, dst = (outs, ins) if adjoint else (ins, outs)
+        fold_src, fold_dst = (fold and adjoint), (fold and not adjoint)
+        want = [n, c * (2 if fold_src else 1), src[0] // (2 if fold_src else 1), src[1], src[2]]
+        if list(x.shape) != want:
+            raise RuntimeError(f'fir3d: x has shape {list(x.shape)}, expected {want}')
+        y = torch.empty([n, c * (2 if fold_dst else 1), dst[0] // (2 if fold_dst else 1), dst[1], dst[2]], dtype=x.dtype, device=x.device)
+        fn = self._lib.lvg_fir3d_adjoint if adjoint else self._lib.lvg_fir3d
+        with _DeviceGuard(x):
+            _check(fn(_ptr(x), _ptr(f), _ptr(y), code, n, c, *ins, *outs, *[a[0] for a in axes], *[a[1] for a in axes],
+                      *[a[2] for a in axes], int(bool(fold)), _stream(x)), 'fir3d')
+        return y
+
+
 _PLUGIN_CLASSES = {
     'convnd_plugin': ConvNdPlugin,
+    'fir3d_plugin': Fir3dPlugin,
     'bias_act_plugin': BiasActPlugin,
     'upfirdn2d_plugin': Upfirdn2dPlugin,
     'filtered_lrelu_plugin': FilteredLReluPlugin,
