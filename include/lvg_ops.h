@@ -292,6 +292,28 @@ int lvg_fir3d_adjoint(const void* x, const float* f, void* y, int dtype, int n, 
                       int step_w, int off_t, int off_h, int off_w, int fold, void* stream);
 
 /*
+ * Input augmentation of the low-res discriminator, fp32: DiffAugment's color, translation and cutout steps and the
+ * temporal-scale augmentation of LowResVideoGAN.run_D (video_gan_lres.py:237-266, diff_augment.py) as one per-sample
+ * affine map x [n][c][t_in][h][w] -> y [n][c][t_out][h][w] (DESIGN.md 7d). params: fp32 [n][12] on the device, per sample
+ *   beta, sigma, kappa, dh, dw, r0, r1, c0, c1, r, L, off
+ * (brightness, saturation, contrast; integer translation; cutout rows [r0, r1] x columns [c0, c1] of the translated frame,
+ * empty when r1 < r0; output frame t reads frame u = t + off of the interpolated clip of length L, 2-tap
+ * align_corners=False interpolation with reciprocal scale r, zero outside [0, L)). The integers are stored exactly in
+ * fp32. flags: LVG_VIDEO_AUGMENT_LINEAR drops beta (the linear part of the map). lvg_video_augment_adjoint computes
+ * dx = A^T dy of the linear part, the same arguments describing the forward map. `workspace`:
+ * lvg_video_augment_workspace bytes (per-CTA partial sums of the per-sample means, folded in a fixed order: results are
+ * bitwise reproducible; no atomics). Two kernel launches per call. LVG_UNSUPPORTED for c > 4. L is read on the device,
+ * so the caller keeps L >= 1 (the draw of the scale does: LowResVideoGAN's F.interpolate fails for an empty clip);
+ * frames outside [0, L) are zero for any L.
+ */
+#define LVG_VIDEO_AUGMENT_LINEAR 1
+int64_t lvg_video_augment_workspace(int n, int c, int t_in, int h, int w, int t_out);
+int lvg_video_augment(const float* x, const float* params, float* y, void* workspace, int n, int c, int t_in, int h, int w,
+                      int t_out, int flags, void* stream);
+int lvg_video_augment_adjoint(const float* dy, const float* params, float* dx, void* workspace, int n, int c, int t_in,
+                              int h, int w, int t_out, void* stream);
+
+/*
  * Post-processing of an all-reduced flat gradient buffer, in place and in one pass:
  *   g = g * scale;  NaN -> 0, +inf -> +limit, -inf -> -limit  (finite values untouched)
  * -- the `/ world_size * gain` + `nan_to_num(nan=0, posinf=1e5, neginf=-1e5)` tail of

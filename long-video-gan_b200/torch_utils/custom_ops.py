@@ -75,6 +75,9 @@ _SIGNATURES = {
     'lvg_modconv_backward': (_c_int, [_c_void_p] * 10 + [_c_int] * 13 + [_c_void_p, _c_i64, _c_void_p]),
     'lvg_fir3d': (_c_int, [_c_void_p] * 3 + [_c_int] * 19 + [_c_void_p]),
     'lvg_fir3d_adjoint': (_c_int, [_c_void_p] * 3 + [_c_int] * 19 + [_c_void_p]),
+    'lvg_video_augment_workspace': (_c_i64, [_c_int] * 6),
+    'lvg_video_augment': (_c_int, [_c_void_p] * 4 + [_c_int] * 7 + [_c_void_p]),
+    'lvg_video_augment_adjoint': (_c_int, [_c_void_p] * 4 + [_c_int] * 6 + [_c_void_p]),
 }
 
 LVG_UNSUPPORTED = -1
@@ -705,7 +708,45 @@ class Fir3dPlugin:
         return y
 
 
+class VideoAugmentPlugin:
+    """The low-res discriminator's input augmentation as one affine map per sample and its adjoint (no reference plugin:
+    LowResVideoGAN.run_D composes DiffAugment and F.interpolate, video_gan_lres.py:237-266). ``params``: fp32 [N, 12] on the
+    device (see lvg_video_augment in include/lvg_ops.h)."""
+
+    def __init__(self, lib):
+        self._lib = lib
+
+    def workspace(self, n, c, t_in, h, w, t_out):
+        """Workspace bytes of one call, or -1 where the kernels do not take the shape (c > 4)."""
+        return int(self._lib.lvg_video_augment_workspace(n, c, t_in, h, w, t_out))
+
+    def run(self, x, params, t_other, linear=False, adjoint=False):
+        """y = A x (x [N, C, T, H, W], y with t_other frames) or, adjoint=True, dx = A^T x (x with the output's frames, dx with
+        t_other). linear drops the brightness offset. Returns None where the library has no kernel (LVG_UNSUPPORTED)."""
+        if not (x.is_cuda and params.device == x.device and x.dtype == torch.float32 and params.dtype == torch.float32):
+            raise RuntimeError('video_augment: x and params must be float32 tensors on one CUDA device')
+        n, c, t, h, w = x.shape
+        if tuple(params.shape) != (n, 12):
+            raise RuntimeError(f'video_augment: params must have shape [{n}, 12], got {list(params.shape)}')
+        t_in, t_out = (t_other, t) if adjoint else (t, t_other)
+        nbytes = self.workspace(n, c, t_in, h, w, t_out)
+        if nbytes < 0:
+            return None
+        x, params = x.contiguous(), params.contiguous()
+        y = torch.empty([n, c, t_other, h, w], dtype=x.dtype, device=x.device)
+        ws = torch.empty([nbytes // 4], dtype=torch.float32, device=x.device)
+        with _DeviceGuard(x):
+            if adjoint:
+                rc = self._lib.lvg_video_augment_adjoint(_ptr(x), _ptr(params), _ptr(y), _ptr(ws), n, c, t_in, h, w, t_out, _stream(x))
+            else:
+                rc = self._lib.lvg_video_augment(_ptr(x), _ptr(params), _ptr(y), _ptr(ws), n, c, t_in, h, w, t_out, int(bool(linear)),
+                                                 _stream(x))
+            _check(rc, 'video_augment')
+        return None if rc == LVG_UNSUPPORTED else y
+
+
 _PLUGIN_CLASSES = {
+    'video_augment_plugin': VideoAugmentPlugin,
     'convnd_plugin': ConvNdPlugin,
     'fir3d_plugin': Fir3dPlugin,
     'bias_act_plugin': BiasActPlugin,
