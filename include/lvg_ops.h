@@ -314,6 +314,30 @@ int lvg_video_augment_adjoint(const float* dy, const float* params, float* dx, v
                               int h, int w, int t_out, void* stream);
 
 /*
+ * ADA's AugmentPipe (ada_augment.py:115-439) of the super-res step without imgfilter and cutout, fp32, c = 3: one affine map
+ * per sample of x [n][c][t][h][w] (DESIGN.md 7e). With LVG_AUGMENT_PIPE_GEOM
+ *   y = C[:3,:3] . downsample2d(grid_sample(upsample2d(reflect_pad(x, margins), f), affine_grid(theta)), f) + C[:3,3] + sigma noise
+ * (upsample2d up = 2; grid of (2h + 12) x (2w + 12), bilinear, zeros, align_corners = False; downsample2d down = 2,
+ * padding -6, flip_filter), without it y = C[:3,:3] x + C[:3,3] + sigma noise, mixing the 3 channels of a frame per pixel.
+ * params: fp32 [n][LVG_AUGMENT_PIPE_NPAR] on the device, per sample
+ *   mx0, my0, mx1, my1, theta[2][3], C[3][4], sigma
+ * (the batch-wide reflect-pad margins, integers stored exactly, 0 <= margin <= size - 1; affine_grid's theta; the colour
+ * matrix; the noise scale). filter: the ntaps taps of Hz_geom on the device. noise: [n][c][t][h][w] or NULL (no noise
+ * term). LVG_AUGMENT_PIPE_LINEAR drops C[:3,3] and the noise (the linear part A). lvg_augment_pipe_adjoint computes
+ * dx = A^T dy, the same arguments describing the forward map; with GEOM it needs `workspace` of
+ * lvg_augment_pipe_workspace bytes (D^T C^T dy on the sampled grid). One kernel launch per call, two for the geometric
+ * adjoint; no atomics, results are bitwise reproducible. LVG_UNSUPPORTED for c != 3 or ntaps != 12.
+ */
+#define LVG_AUGMENT_PIPE_NPAR 23
+#define LVG_AUGMENT_PIPE_GEOM 1
+#define LVG_AUGMENT_PIPE_LINEAR 2
+int64_t lvg_augment_pipe_workspace(int n, int c, int t, int h, int w, int flags);
+int lvg_augment_pipe(const float* x, const float* params, const float* filter, int ntaps, const float* noise, float* y, int n,
+                     int c, int t, int h, int w, int flags, void* stream);
+int lvg_augment_pipe_adjoint(const float* dy, const float* params, const float* filter, int ntaps, float* dx, void* workspace,
+                             int n, int c, int t, int h, int w, int flags, void* stream);
+
+/*
  * Post-processing of an all-reduced flat gradient buffer, in place and in one pass:
  *   g = g * scale;  NaN -> 0, +inf -> +limit, -inf -> -limit  (finite values untouched)
  * -- the `/ world_size * gain` + `nan_to_num(nan=0, posinf=1e5, neginf=-1e5)` tail of

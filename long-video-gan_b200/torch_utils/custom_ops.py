@@ -78,6 +78,9 @@ _SIGNATURES = {
     'lvg_video_augment_workspace': (_c_i64, [_c_int] * 6),
     'lvg_video_augment': (_c_int, [_c_void_p] * 4 + [_c_int] * 7 + [_c_void_p]),
     'lvg_video_augment_adjoint': (_c_int, [_c_void_p] * 4 + [_c_int] * 6 + [_c_void_p]),
+    'lvg_augment_pipe_workspace': (_c_i64, [_c_int] * 6),
+    'lvg_augment_pipe': (_c_int, [_c_void_p] * 3 + [_c_int] + [_c_void_p] * 2 + [_c_int] * 6 + [_c_void_p]),
+    'lvg_augment_pipe_adjoint': (_c_int, [_c_void_p] * 3 + [_c_int] + [_c_void_p] * 2 + [_c_int] * 6 + [_c_void_p]),
 }
 
 LVG_UNSUPPORTED = -1
@@ -745,7 +748,49 @@ class VideoAugmentPlugin:
         return None if rc == LVG_UNSUPPORTED else y
 
 
+class AugmentPipePlugin:
+    """ADA's AugmentPipe without imgfilter and cutout as one affine map per sample and its adjoint (no reference plugin:
+    AugmentPipe.forward composes F.pad, upfirdn2d, affine_grid / grid_sample and a colour bmm, ada_augment.py:180-439).
+    ``params``: fp32 [N, 23] on the device, ``f``: the 12 taps of Hz_geom (see lvg_augment_pipe in include/lvg_ops.h)."""
+
+    def __init__(self, lib):
+        self._lib = lib
+
+    def workspace(self, n, c, t, h, w, flags):
+        """Workspace bytes of the adjoint, or -1 where the kernels do not take the shape (c != 3)."""
+        return int(self._lib.lvg_augment_pipe_workspace(n, c, t, h, w, flags))
+
+    def run(self, x, params, f, noise, flags, adjoint=False):
+        """y = A x (+ C[:3,3] + sigma noise unless flags has LINEAR) or, adjoint=True, dx = A^T x; x [N, C, T, H, W]. Returns
+        None where the library has no kernel (LVG_UNSUPPORTED)."""
+        if not (x.is_cuda and params.device == x.device and f.device == x.device and x.dtype == torch.float32
+                and params.dtype == torch.float32 and f.dtype == torch.float32):
+            raise RuntimeError('augment_pipe: x, params and the filter must be float32 tensors on one CUDA device')
+        n, c, t, h, w = x.shape
+        if tuple(params.shape) != (n, 23):
+            raise RuntimeError(f'augment_pipe: params must have shape [{n}, 23], got {list(params.shape)}')
+        if noise is not None and (tuple(noise.shape) != tuple(x.shape) or noise.dtype != torch.float32 or noise.device != x.device):
+            raise RuntimeError('augment_pipe: noise must be a float32 tensor of the shape of x on its device')
+        nbytes = self.workspace(n, c, t, h, w, flags)
+        if nbytes < 0 or f.numel() != 12:
+            return None
+        x, params, f = x.contiguous(), params.contiguous(), f.contiguous()
+        noise = None if noise is None else noise.contiguous()
+        y = torch.empty_like(x)
+        with _DeviceGuard(x):
+            if adjoint:
+                ws = torch.empty([max(nbytes // 4, 1)], dtype=torch.float32, device=x.device)
+                rc = self._lib.lvg_augment_pipe_adjoint(_ptr(x), _ptr(params), _ptr(f), f.numel(), _ptr(y), _ptr(ws), n, c, t, h, w,
+                                                        int(flags), _stream(x))
+            else:
+                rc = self._lib.lvg_augment_pipe(_ptr(x), _ptr(params), _ptr(f), f.numel(), _ptr(noise), _ptr(y), n, c, t, h, w,
+                                                int(flags), _stream(x))
+            _check(rc, 'augment_pipe')
+        return None if rc == LVG_UNSUPPORTED else y
+
+
 _PLUGIN_CLASSES = {
+    'augment_pipe_plugin': AugmentPipePlugin,
     'video_augment_plugin': VideoAugmentPlugin,
     'convnd_plugin': ConvNdPlugin,
     'fir3d_plugin': Fir3dPlugin,
