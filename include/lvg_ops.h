@@ -224,6 +224,15 @@ int lvg_convnd_wgrad(const void* x, const void* dy, void* dw, int dtype, int n, 
 int lvg_convnd_plan(int mode, int dtype, int n, int groups, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw,
                     int pad_t, int pad_h, int pad_w, int stride, int* out, int out_len);
 /*
+ * Introspection: the kernels a call takes -- mode 0 forward (`epilogue` != 0: with bias / act / gain / clamp), 1 input
+ * gradient, 2 weight gradient -> 0 the implicit-GEMM engine, 1 the streaming SIMT kernels for few-channel fp32 1x1x1
+ * layers, 2 the pointwise wgmma kernels for every other 1x1x1 forward / input gradient (stride 1, no padding, groups 1,
+ * T*H*W a multiple of 4 (fp32) / 8 (fp16)); LVG_UNSUPPORTED outside the envelope. Host arithmetic only; tensors are
+ * taken to be 16-byte aligned (route 2 runs on the engine for a misaligned one). LVG_CONV_PW_TC=0 turns route 2 off.
+ */
+int lvg_convnd_route(int mode, int dtype, int n, int groups, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw,
+                     int pad_t, int pad_h, int pad_w, int stride, int epilogue);
+/*
  * Introspection: the tiling lvg_convnd_wgrad launches with, as 32 ints -- split, cpad_a, cpad_b, nt, ntiles, mt, nsplit,
  * ablk, khc, nseg, ps, rh, stages, a_stage, b_stage, stage_bytes, tail_bytes, smem, seg_w[4], seg_x0[4], 0, mrows, 0... --
  * host arithmetic only (no device needed): tests/test_wgrad_emul.py replays the kernel's addressing with it on the CPU.

@@ -41,6 +41,10 @@ namespace lvg {
 // conv_pointwise.cu: streaming fp32 kernels for 1x1x1 convolutions with few channels (HBM-bound; the engine would re-tile and pad)
 bool pw_supported(int dtype, int groups, int cin, int cout, int kt, int kh, int kw, int pad_t, int pad_h, int pad_w, int stride, int64_t P);
 int pw_conv(const float* x, const float* w, float* y, int n, int cin, int cout, int64_t P, int64_t w_sco, int64_t w_sci, cudaStream_t s);
+// conv_pw_tc.cu: every other 1x1x1 forward / input gradient on wgmma, straight from the NC(T)HW tensors (no re-tiling)
+bool pw_tc_supported(int dtype, int groups, int cin, int cout, int kt, int kh, int kw, int pad_t, int pad_h, int pad_w, int stride, int64_t P);
+int pw_tc_conv(const void* x, const void* w, void* y, int dtype, int n, int ck, int cm, int64_t P, int64_t w_sm, int64_t w_sk, void* workspace,
+               int64_t workspace_bytes, cudaStream_t s);
 }
 
 namespace lvg {
@@ -776,9 +780,11 @@ extern "C" int lvg_convnd_fprop(const void* x, const void* w, void* y, int dtype
                                 float gain, float clamp, void* workspace, int64_t workspace_bytes, void* stream)
 {
     LVG_REQUIRE(x && w && y, "convnd_fprop: x, w, y must not be NULL");
-    if (!bias && act == 0 && gain == 1.f && clamp < 0.f &&
-        pw_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, (int64_t)t * h * wd))
-        return pw_conv((const float*)x, (const float*)w, (float*)y, n, cin, cout, (int64_t)t * h * wd, cin, 1, (cudaStream_t)stream);
+    const int route = lvg_convnd_route(0, dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, stride,
+                                       bias || act != 0 || gain != 1.f || clamp >= 0.f);
+    if (route == 1) return pw_conv((const float*)x, (const float*)w, (float*)y, n, cin, cout, (int64_t)t * h * wd, cin, 1, (cudaStream_t)stream);
+    if (route == 2 && aligned16(x) && aligned16(y))
+        return pw_tc_conv(x, w, y, dtype, n, cin, cout, (int64_t)t * h * wd, cin, 1, workspace, workspace_bytes, (cudaStream_t)stream);
     if (!nd_supported(dtype, kt, kh, kw) || n < 1 || pad_t < 0 || pad_h < 0 || pad_w < 0 || stride < 1 || stride > 4) {
         set_error("convnd_fprop: outside the tensor-core kernel's envelope");
         return LVG_UNSUPPORTED;
@@ -794,8 +800,10 @@ extern "C" int lvg_convnd_dgrad(const void* dy, const void* w, void* dx, int dty
                                 void* stream)
 {
     LVG_REQUIRE(dy && w && dx, "convnd_dgrad: dy, w, dx must not be NULL");
-    if (pw_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, (int64_t)t * h * wd))   // dx = W^T dy
-        return pw_conv((const float*)dy, (const float*)w, (float*)dx, n, cout, cin, (int64_t)t * h * wd, 1, cin, (cudaStream_t)stream);
+    const int route = lvg_convnd_route(1, dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, stride, 0);     // dx = W^T dy
+    if (route == 1) return pw_conv((const float*)dy, (const float*)w, (float*)dx, n, cout, cin, (int64_t)t * h * wd, 1, cin, (cudaStream_t)stream);
+    if (route == 2 && aligned16(dy) && aligned16(dx))
+        return pw_tc_conv(dy, w, dx, dtype, n, cout, cin, (int64_t)t * h * wd, 1, cin, workspace, workspace_bytes, (cudaStream_t)stream);
     if (!nd_supported(dtype, kt, kh, kw) || n < 1 || pad_t < 0 || pad_h < 0 || pad_w < 0 || pad_t > kt - 1 || pad_h > kh - 1 || pad_w > kw - 1 ||
         stride < 1 || stride > 4) {
         set_error("convnd_dgrad: outside the tensor-core kernel's envelope");
@@ -1231,6 +1239,26 @@ extern "C" int lvg_convnd_wgrad(const void* x, const void* dy, void* dw, int dty
                      (cudaStream_t)stream);
 }
 
+// which kernels a call takes (host arithmetic only): mode 0 forward (`epilogue` != 0: with a bias / activation / gain /
+// clamp epilogue), 1 input gradient, 2 weight gradient -> 0 the engine, 1 the streaming SIMT kernels (conv_pointwise.cu),
+// 2 the pointwise wgmma kernels (conv_pw_tc.cu); LVG_UNSUPPORTED outside the envelope. Tensors are taken to be 16-byte
+// aligned (the pointwise wgmma route falls back to the engine for a misaligned one).
+extern "C" int lvg_convnd_route(int mode, int dtype, int n, int groups, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw, int pad_t,
+                                int pad_h, int pad_w, int stride, int epilogue)
+{
+    if (mode < 0 || mode > 2 || n < 1 || groups < 1) return LVG_UNSUPPORTED;
+    if (mode == 2) return wgrad_in_envelope(dtype, n, groups, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, stride) ? 0 : LVG_UNSUPPORTED;
+    const int64_t P = (int64_t)t * h * wd;
+    if (mode == 1 || !epilogue) {
+        if (pw_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, P)) return 1;
+        if (pw_tc_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, P)) return 2;
+    }
+    if (!nd_supported(dtype, kt, kh, kw) || pad_t < 0 || pad_h < 0 || pad_w < 0 || stride < 1 || stride > 4 ||
+        (mode == 1 && (pad_t > kt - 1 || pad_h > kh - 1 || pad_w > kw - 1)))
+        return LVG_UNSUPPORTED;
+    return 0;
+}
+
 // the tiling lvg_convnd_fprop (mode 0) / lvg_convnd_dgrad (mode 1) would launch with, as ints (host arithmetic only;
 // tests/test_igemm_emul.py replays the forward kernel's addressing with it on the CPU)
 extern "C" int lvg_convnd_plan(int mode, int dtype, int n, int groups, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw, int pad_t,
@@ -1302,6 +1330,7 @@ bool backward_shares_dy8(int dtype, int n, int groups, int cin, int cout, int t,
     const int64_t P = (int64_t)t * h * wd;
     if (!env_flag("LVG_CONV_SHARED_DY8", 1)) return false;
     if (pw_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, P)) return false;
+    if (pw_tc_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, P)) return false;     // reads dy as it is
     return wgrad_cpad_a(cout) == round_up(cout, 16);
 }
 }  // namespace

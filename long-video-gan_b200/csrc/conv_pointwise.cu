@@ -10,7 +10,8 @@
 //   input gradient  the same kernel on dy with the transposed weight view
 // The weight gradient of these layers runs on the engine.
 // Envelope: 1x1x1, stride 1, no padding, groups 1, fp32, cin * cout <= 4096, pixels per sample a multiple of 4,
-// 16-byte aligned tensors; everything else stays on the engine (conv_igemm.cu calls pw_* first).
+// 16-byte aligned tensors; every other 1x1x1 forward / input gradient runs on the pointwise wgmma kernels (conv_pw_tc.cu),
+// everything else on the engine (lvg_convnd_route in conv_igemm.cu checks pw_supported first).
 #include "common.cuh"
 
 namespace lvg {

@@ -68,6 +68,7 @@ _SIGNATURES = {
     'lvg_convnd_wgrad': (_c_int, [_c_void_p] * 3 + [_c_int] * 15 + [_c_void_p, _c_i64, _c_void_p]),
     'lvg_convnd_plan': (_c_int, [_c_int] * 16 + [ctypes.POINTER(_c_int), _c_int]),
     'lvg_convnd_wgrad_plan': (_c_int, [_c_int] * 14 + [ctypes.POINTER(_c_int), _c_int]),
+    'lvg_convnd_route': (_c_int, [_c_int] * 17),
     'lvg_convnd_backward_workspace': (_c_i64, [_c_int] * 14),
     'lvg_convnd_backward': (_c_int, [_c_void_p] * 5 + [_c_int] * 15 + [_c_void_p, _c_i64, _c_void_p]),
     'lvg_modconv_workspace': (_c_i64, [_c_int] * 13),
@@ -559,6 +560,15 @@ class ConvNdPlugin:
         pad = self._pad3(padding, nd)
         code = 1 if dtype == torch.float16 else 0
         return [code, x_shape[0], groups, w_shape[1], w_shape[0] // groups] + sp + k + pad, sp, k, pad
+
+    ROUTES = ('engine', 'simt', 'pointwise_wgmma')
+
+    def route(self, mode, x_shape, w_shape, padding, groups, dtype, stride=1, epilogue=False):
+        """Which kernels a call takes: mode 'fprop' / 'dgrad' / 'wgrad' (shapes of the forward convolution) -> one of ROUTES,
+        or None outside the envelope (lvg_convnd_route)."""
+        a, _, _, _ = self._args(tuple(x_shape), tuple(w_shape), padding, groups, dtype)
+        r = self._lib.lvg_convnd_route(('fprop', 'dgrad', 'wgrad').index(mode), *a, int(stride), int(bool(epilogue)))
+        return None if r < 0 else self.ROUTES[r]
 
     def fprop(self, x, w, padding, groups, bias=None, act=0, alpha=0.2, gain=1.0, clamp=-1.0, stride=1):
         x, w = x.contiguous(), w.contiguous()
