@@ -347,6 +347,32 @@ int lvg_augment_pipe_adjoint(const float* dy, const float* params, const float* 
                              int n, int c, int t, int h, int w, int flags, void* stream);
 
 /*
+ * Tail of the low-res generator's residual block (Synthesis3dResBlock.forward, generator_lres.py:577-589), fp32 or fp16
+ * storage with fp32 arithmetic, as one op over s, h [n][c][t][h][w] -> z [n][c][t_out][h_out][w_out] (DESIGN.md 7f):
+ *   m = (s + h) sqrt(1/2);  u = crop_T(U_T m);  v = crop_HW(U_HW u);  z = bias_act(v, b, act, alpha, gain, clamp)
+ * U_T (flag LVG_GBLOCK_TAIL_TUP) / U_HW (LVG_GBLOCK_TAIL_SUP): 2x upsampling with [1,3,3,1]/8 at gain 2 per axis and
+ * padding (2, 1), as upfirdn2d.upsample2d; without the flag the axis is copied. The crops are center_crop's: offset
+ * (size - out) / 2, 1 <= out <= size on every axis. b: fp32 [c] or NULL. act: LVG_ACT_LRELU or LVG_ACT_LINEAR
+ * (LVG_UNSUPPORTED otherwise); clamp < 0 = none. codes (NULL = none): the 2-bit codes of z in lvg_bias_act_fwd_codes'
+ * layout, lvg_bias_act_codes_bytes(dtype, numel(z)) bytes. s, h and z are dense and 16-byte (fp32) / 8-byte (fp16)
+ * aligned. One kernel launch.
+ * lvg_gblock_tail_adjoint: from dz and the codes, dv = the bias_act gradient, db[c] = sum of dv over n, t, h, w (fp32, a
+ * fixed summation order: bitwise reproducible, no atomics) and dm = sqrt(1/2) * the transposed upsamplings and crops
+ * applied to dv -- the gradient of both s and h. alpha and gain as in the forward call. `workspace`:
+ * lvg_gblock_tail_workspace bytes (per-CTA partial sums of db). Two kernel launches. The size query returns -1 for shapes
+ * outside the envelope (crops larger than the axis, a w_out row of dv that does not fit the adjoint's shared-memory tile).
+ */
+#define LVG_GBLOCK_TAIL_TUP 1
+#define LVG_GBLOCK_TAIL_SUP 2
+int64_t lvg_gblock_tail_workspace(int n, int c, int t, int h, int w, int t_out, int h_out, int w_out, int flags);
+int lvg_gblock_tail(const void* s, const void* h, const float* b, void* z, uint8_t* codes, int dtype, int n, int c, int t,
+                    int hh, int ww, int t_out, int h_out, int w_out, int flags, int act, float alpha, float gain, float clamp,
+                    void* stream);
+int lvg_gblock_tail_adjoint(const void* dz, const uint8_t* codes, void* dm, float* db, void* workspace, int64_t workspace_bytes,
+                            int dtype, int n, int c, int t, int hh, int ww, int t_out, int h_out, int w_out, int flags, int act,
+                            float alpha, float gain, void* stream);
+
+/*
  * Post-processing of an all-reduced flat gradient buffer, in place and in one pass:
  *   g = g * scale;  NaN -> 0, +inf -> +limit, -inf -> -limit  (finite values untouched)
  * -- the `/ world_size * gain` + `nan_to_num(nan=0, posinf=1e5, neginf=-1e5)` tail of

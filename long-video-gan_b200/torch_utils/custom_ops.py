@@ -82,6 +82,9 @@ _SIGNATURES = {
     'lvg_augment_pipe_workspace': (_c_i64, [_c_int] * 6),
     'lvg_augment_pipe': (_c_int, [_c_void_p] * 3 + [_c_int] + [_c_void_p] * 2 + [_c_int] * 6 + [_c_void_p]),
     'lvg_augment_pipe_adjoint': (_c_int, [_c_void_p] * 3 + [_c_int] + [_c_void_p] * 2 + [_c_int] * 6 + [_c_void_p]),
+    'lvg_gblock_tail_workspace': (_c_i64, [_c_int] * 9),
+    'lvg_gblock_tail': (_c_int, [_c_void_p] * 5 + [_c_int] * 11 + [_c_float] * 3 + [_c_void_p]),
+    'lvg_gblock_tail_adjoint': (_c_int, [_c_void_p] * 5 + [_c_i64] + [_c_int] * 11 + [_c_float] * 2 + [_c_void_p]),
 }
 
 LVG_UNSUPPORTED = -1
@@ -799,7 +802,76 @@ class AugmentPipePlugin:
         return None if rc == LVG_UNSUPPORTED else y
 
 
+class GblockTailPlugin:
+    """Tail of the low-res generator's residual block, z = bias_act(crop(U_HW crop(U_T (s + h) sqrt(1/2))), b), and its
+    adjoint (no reference plugin: Synthesis3dResBlock.forward composes ATen add / mul, two upfirdn2d calls, slices and
+    bias_act, generator_lres.py:577-589). ``flags``: LVG_GBLOCK_TAIL_TUP | LVG_GBLOCK_TAIL_SUP (see lvg_gblock_tail in
+    include/lvg_ops.h)."""
+
+    TUP, SUP = 1, 2
+
+    def __init__(self, lib):
+        self._lib = lib
+
+    def workspace(self, n, c, t, h, w, t_out, h_out, w_out, flags):
+        """Workspace bytes of the adjoint, or -1 where the kernels do not take the shape."""
+        return int(self._lib.lvg_gblock_tail_workspace(n, c, t, h, w, t_out, h_out, w_out, flags))
+
+    @staticmethod
+    def _check(x, what):
+        if not x.is_cuda or x.dtype not in (torch.float16, torch.float32) or x.ndim != 5:
+            raise RuntimeError(f'gblock_tail: {what} must be a 5-D float16 / float32 CUDA tensor')
+
+    def forward(self, s, h, b, out_size, flags, act, alpha, gain, clamp, want_codes):
+        """(z [N, C, *out_size], codes or None) from s and h [N, C, T, H, W] (one dtype and shape) and b (fp32 [C] or None)."""
+        self._check(s, 's')
+        if h.dtype != s.dtype or h.shape != s.shape or h.device != s.device:
+            raise RuntimeError('gblock_tail: s and h must have one shape, dtype and device')
+        n, c, t, hh, ww = s.shape
+        if b is not None and (b.dtype != torch.float32 or tuple(b.shape) != (c,) or b.device != s.device):
+            raise RuntimeError(f'gblock_tail: b must be a float32 [{c}] tensor on the device of s')
+        to, ho, wo = (int(v) for v in out_size)
+        if self.workspace(n, c, t, hh, ww, to, ho, wo, flags) < 0:
+            raise RuntimeError(f'gblock_tail: no kernel for {list(s.shape)} -> {[to, ho, wo]} (flags {flags})')
+        s, h = s.contiguous(), h.contiguous()
+        b = None if b is None else b.contiguous()
+        z = torch.empty([n, c, to, ho, wo], dtype=s.dtype, device=s.device)
+        codes = None
+        if want_codes:
+            codes = torch.empty([int(self._lib.lvg_bias_act_codes_bytes(_dtype_code(s, 'gblock_tail'), z.numel()))], dtype=torch.uint8,
+                                device=s.device)
+        with _DeviceGuard(s):
+            if _check(self._lib.lvg_gblock_tail(_ptr(s), _ptr(h), _ptr(b), _ptr(z), _ptr(codes), _dtype_code(s, 'gblock_tail'), n, c, t,
+                                             hh, ww, to, ho, wo, int(flags), int(act), float(alpha), float(gain), float(clamp),
+                                             _stream(s)), 'gblock_tail') == LVG_UNSUPPORTED:
+                raise RuntimeError('gblock_tail: ' + self._lib.lvg_last_error().decode())
+        return z, codes
+
+    def adjoint(self, dz, codes, in_size, flags, act, alpha, gain):
+        """(dm [N, C, *in_size], db fp32 [C]) from dz [N, C, T_out, H_out, W_out] and the forward's codes."""
+        self._check(dz, 'dz')
+        n, c, to, ho, wo = dz.shape
+        t, hh, ww = (int(v) for v in in_size)
+        nbytes = self.workspace(n, c, t, hh, ww, to, ho, wo, flags)
+        if nbytes < 0:
+            raise RuntimeError(f'gblock_tail_adjoint: no kernel for {[t, hh, ww]} -> {list(dz.shape)} (flags {flags})')
+        need = int(self._lib.lvg_bias_act_codes_bytes(_dtype_code(dz, 'gblock_tail'), dz.numel()))
+        if codes.dtype != torch.uint8 or codes.device != dz.device or codes.numel() < need or not codes.is_contiguous():
+            raise RuntimeError(f'gblock_tail_adjoint: codes must be a contiguous uint8 buffer of {need} bytes on the device of dz')
+        dz = dz.contiguous()
+        dm = torch.empty([n, c, t, hh, ww], dtype=dz.dtype, device=dz.device)
+        db = torch.empty([c], dtype=torch.float32, device=dz.device)
+        ws = torch.empty([nbytes // 4], dtype=torch.float32, device=dz.device)
+        with _DeviceGuard(dz):
+            if _check(self._lib.lvg_gblock_tail_adjoint(_ptr(dz), _ptr(codes), _ptr(dm), _ptr(db), _ptr(ws), nbytes,
+                                                     _dtype_code(dz, 'gblock_tail'), n, c, t, hh, ww, to, ho, wo, int(flags), int(act),
+                                                     float(alpha), float(gain), _stream(dz)), 'gblock_tail_adjoint') == LVG_UNSUPPORTED:
+                raise RuntimeError('gblock_tail_adjoint: ' + self._lib.lvg_last_error().decode())
+        return dm, db
+
+
 _PLUGIN_CLASSES = {
+    'gblock_tail_plugin': GblockTailPlugin,
     'augment_pipe_plugin': AugmentPipePlugin,
     'video_augment_plugin': VideoAugmentPlugin,
     'convnd_plugin': ConvNdPlugin,
