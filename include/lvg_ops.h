@@ -373,6 +373,47 @@ int lvg_gblock_tail_adjoint(const void* dz, const uint8_t* codes, void* dm, floa
                             float alpha, float gain, void* stream);
 
 /*
+ * Tail of the low-res discriminator's residual block (DiscriminatorBlock.forward after conv_1's convolution,
+ * discriminator_lres.py:321-333, 169-179, 197-213), fp32 or fp16 storage with fp32 arithmetic, as one op over
+ * y [n][c][t][h][w] -> z [n][c][t_out][h_out][w_out] (DESIGN.md 7g):
+ *   z = scale * (bias_act(P y, b, act, alpha, gain, clamp) + s)
+ * P: per axis a copy or Downsample3d's filter out[m] = sum_j f[3 - j] * in[2 m - 1 + j] (zero outside; the extent must be
+ * even, the output extent is half of it) -- lvg_fir3d's operator with (filt, step, off) = (1, 2, -1) -- on T with
+ * LVG_DBLOCK_TAIL_TDOWN and on H and W with LVG_DBLOCK_TAIL_SDOWN. With LVG_DBLOCK_TAIL_MERGE scale = sqrt(1/2) and
+ * s [n][c][t_out][h_out][w_out] (NULL = zero) is the skip tensor; without it scale = 1 and s must be NULL. bias_act's
+ * output is rounded to the storage type before s is added (as the composition stores it); read mode rounds only its
+ * result. f: 4 fp32 taps on the device, NULL allowed where no axis is filtered. b: fp32 [c] or NULL. act: LVG_ACT_LRELU or LVG_ACT_LINEAR (LVG_UNSUPPORTED otherwise); clamp < 0 = none.
+ * mode:
+ *   LVG_DBLOCK_TAIL_NONE   z only; codes must be NULL.
+ *   LVG_DBLOCK_TAIL_WRITE  z and the 2-bit codes of every output (bit 0: bias_act's stored value is not positive, bit 1: it
+ *                          is clamped, both evaluated as bias_act evaluates them): lvg_dblock_tail_codes_bytes bytes, one
+ *                          byte per 4 consecutive outputs along W (output k of the group in bits 2k, 2k + 1), rows padded
+ *                          to ceil(w_out / 4) bytes, rows in z's order.
+ *   LVG_DBLOCK_TAIL_READ   codes are an input: z = scale * (G (P y + b) + s) with G = gain, gain * alpha or 0 (clamped) per
+ *                          output, for arbitrary y, b, s: the linear map that is the adjoint's backward.
+ * One kernel launch.
+ * lvg_dblock_tail_adjoint: from dz [n][c][t_out][h_out][w_out] and the codes, dv = scale * G dz, dy = P^T dv
+ * [n][c][t][h][w], ds = scale * dz (NULL = not wanted) and db[c] = sum of dv over n, t, h, w (fp32). db is summed from one
+ * partial per CTA in `workspace` (lvg_dblock_tail_workspace bytes), folded by a second kernel in a fixed order; the
+ * partition depends on the shape only and there are no atomics, so every result is bitwise reproducible. alpha and gain
+ * as in the forward call. Two kernel launches. Both size queries return -1 for shapes outside the envelope (an odd extent
+ * on a filtered axis, more than 65535 tiles of 8 x 32 per plane, n * c >= 2^31); such calls return LVG_UNSUPPORTED.
+ */
+#define LVG_DBLOCK_TAIL_TDOWN 1
+#define LVG_DBLOCK_TAIL_SDOWN 2
+#define LVG_DBLOCK_TAIL_MERGE 4
+#define LVG_DBLOCK_TAIL_NONE 0
+#define LVG_DBLOCK_TAIL_WRITE 1
+#define LVG_DBLOCK_TAIL_READ 2
+int64_t lvg_dblock_tail_workspace(int n, int c, int t, int h, int w, int flags);
+int64_t lvg_dblock_tail_codes_bytes(int n, int c, int t, int h, int w, int flags);
+int lvg_dblock_tail(const void* y, const void* s, const float* b, const float* f, void* z, uint8_t* codes, int mode, int dtype,
+                    int n, int c, int t, int h, int w, int flags, int act, float alpha, float gain, float clamp, void* stream);
+int lvg_dblock_tail_adjoint(const void* dz, const uint8_t* codes, const float* f, void* dy, void* ds, float* db, void* workspace,
+                            int64_t workspace_bytes, int dtype, int n, int c, int t, int h, int w, int flags, int act,
+                            float alpha, float gain, void* stream);
+
+/*
  * Post-processing of an all-reduced flat gradient buffer, in place and in one pass:
  *   g = g * scale;  NaN -> 0, +inf -> +limit, -inf -> -limit  (finite values untouched)
  * -- the `/ world_size * gain` + `nan_to_num(nan=0, posinf=1e5, neginf=-1e5)` tail of

@@ -85,6 +85,10 @@ _SIGNATURES = {
     'lvg_gblock_tail_workspace': (_c_i64, [_c_int] * 9),
     'lvg_gblock_tail': (_c_int, [_c_void_p] * 5 + [_c_int] * 11 + [_c_float] * 3 + [_c_void_p]),
     'lvg_gblock_tail_adjoint': (_c_int, [_c_void_p] * 5 + [_c_i64] + [_c_int] * 11 + [_c_float] * 2 + [_c_void_p]),
+    'lvg_dblock_tail_workspace': (_c_i64, [_c_int] * 6),
+    'lvg_dblock_tail_codes_bytes': (_c_i64, [_c_int] * 6),
+    'lvg_dblock_tail': (_c_int, [_c_void_p] * 6 + [_c_int] * 9 + [_c_float] * 3 + [_c_void_p]),
+    'lvg_dblock_tail_adjoint': (_c_int, [_c_void_p] * 7 + [_c_i64] + [_c_int] * 8 + [_c_float] * 2 + [_c_void_p]),
 }
 
 LVG_UNSUPPORTED = -1
@@ -870,7 +874,100 @@ class GblockTailPlugin:
         return dm, db
 
 
+class DblockTailPlugin:
+    """Tail of the low-res discriminator's residual block, z = scale (bias_act(P y, b) + s) with P Downsample3d's filter, its
+    read-mode linear map and its adjoint (no reference plugin: DiscriminatorBlock.forward composes two upfirdn2d calls,
+    bias_act and ATen add / mul, discriminator_lres.py:321-333). ``flags``: TDOWN | SDOWN | MERGE, ``mode``: NONE / WRITE /
+    READ (see lvg_dblock_tail in include/lvg_ops.h)."""
+
+    TDOWN, SDOWN, MERGE = 1, 2, 4
+    NONE, WRITE, READ = 0, 1, 2
+
+    def __init__(self, lib):
+        self._lib = lib
+
+    def workspace(self, n, c, t, h, w, flags):
+        """Workspace bytes of the adjoint for y [n, c, t, h, w], or -1 where the kernels do not take the shape."""
+        return int(self._lib.lvg_dblock_tail_workspace(n, c, t, h, w, flags))
+
+    def codes_bytes(self, n, c, t, h, w, flags):
+        """Bytes of the codes of one forward call, or -1 where the kernels do not take the shape."""
+        return int(self._lib.lvg_dblock_tail_codes_bytes(n, c, t, h, w, flags))
+
+    @staticmethod
+    def out_size(in_size, flags):
+        t, h, w = in_size
+        return (t // 2 if flags & 1 else t, h // 2 if flags & 2 else h, w // 2 if flags & 2 else w)
+
+    @staticmethod
+    def _check(x, what):
+        if not x.is_cuda or x.dtype not in (torch.float16, torch.float32) or x.ndim != 5:
+            raise RuntimeError(f'dblock_tail: {what} must be a 5-D float16 / float32 CUDA tensor')
+
+    def _check_codes(self, codes, ref, need):
+        if codes.dtype != torch.uint8 or codes.device != ref.device or codes.numel() != need or not codes.is_contiguous():
+            raise RuntimeError(f'dblock_tail: codes must be a contiguous uint8 buffer of {need} bytes on the device of the data')
+
+    def forward(self, y, s, b, f, flags, act, alpha, gain, clamp, mode, codes=None):
+        """(z, codes) from y [N, C, T, H, W], s [N, C, T', H', W'] or None, b ([C], passed as fp32, or None) and the 4 fp32 taps f. WRITE
+        returns new codes, READ takes ``codes``, NONE returns None for them."""
+        self._check(y, 'y')
+        n, c, t, h, w = y.shape
+        nbytes = self.codes_bytes(n, c, t, h, w, flags)
+        if nbytes < 0:
+            raise RuntimeError(f'dblock_tail: no kernel for {list(y.shape)} (flags {flags})')
+        out = [n, c, *self.out_size((t, h, w), flags)]
+        if s is not None and (list(s.shape) != out or s.dtype != y.dtype or s.device != y.device or not flags & self.MERGE):
+            raise RuntimeError(f'dblock_tail: s must be a {y.dtype} tensor of shape {out} on the device of y, with MERGE')
+        if b is not None and (tuple(b.shape) != (c,) or b.device != y.device):
+            raise RuntimeError(f'dblock_tail: b must be a [{c}] tensor on the device of y')
+        if f is None and flags & (self.TDOWN | self.SDOWN) or f is not None and (f.dtype != torch.float32 or f.numel() != 4
+                                                                                  or f.device != y.device):
+            raise RuntimeError('dblock_tail: f must hold 4 float32 taps on the device of y (None where no axis is filtered)')
+        y, f = y.contiguous(), (None if f is None else f.contiguous())
+        s = None if s is None else s.contiguous()
+        b = None if b is None else b.float().contiguous()
+        if mode == self.WRITE:
+            codes = torch.empty([nbytes], dtype=torch.uint8, device=y.device)
+        elif mode == self.READ:
+            self._check_codes(codes, y, nbytes)
+        else:
+            codes = None
+        z = torch.empty(out, dtype=y.dtype, device=y.device)
+        with _DeviceGuard(y):
+            if _check(self._lib.lvg_dblock_tail(_ptr(y), _ptr(s), _ptr(b), _ptr(f), _ptr(z), _ptr(codes), int(mode),
+                                             _dtype_code(y, 'dblock_tail'), n, c, t, h, w, int(flags), int(act), float(alpha),
+                                             float(gain), float(clamp), _stream(y)), 'dblock_tail') == LVG_UNSUPPORTED:
+                raise RuntimeError('dblock_tail: ' + self._lib.lvg_last_error().decode())
+        return z, codes
+
+    def adjoint(self, dz, codes, f, in_size, flags, act, alpha, gain, want_ds):
+        """(dy [N, C, *in_size], ds like dz or None, db fp32 [C]) from dz [N, C, T', H', W'] and the forward's codes."""
+        self._check(dz, 'dz')
+        n, c = dz.shape[:2]
+        t, h, w = (int(v) for v in in_size)
+        nbytes = self.workspace(n, c, t, h, w, flags)
+        if nbytes < 0 or list(dz.shape[2:]) != list(self.out_size((t, h, w), flags)):
+            raise RuntimeError(f'dblock_tail_adjoint: no kernel for {[t, h, w]} -> {list(dz.shape)} (flags {flags})')
+        self._check_codes(codes, dz, self.codes_bytes(n, c, t, h, w, flags))
+        if f is None and flags & (self.TDOWN | self.SDOWN) or f is not None and (f.dtype != torch.float32 or f.numel() != 4
+                                                                                  or f.device != dz.device):
+            raise RuntimeError('dblock_tail_adjoint: f must hold 4 float32 taps on the device of dz (None where no axis is filtered)')
+        dz, f = dz.contiguous(), (None if f is None else f.contiguous())
+        dy = torch.empty([n, c, t, h, w], dtype=dz.dtype, device=dz.device)
+        ds = torch.empty_like(dz) if want_ds else None
+        db = torch.empty([c], dtype=torch.float32, device=dz.device)
+        ws = torch.empty([nbytes // 4], dtype=torch.float32, device=dz.device)
+        with _DeviceGuard(dz):
+            if _check(self._lib.lvg_dblock_tail_adjoint(_ptr(dz), _ptr(codes), _ptr(f), _ptr(dy), _ptr(ds), _ptr(db), _ptr(ws), nbytes,
+                                                     _dtype_code(dz, 'dblock_tail'), n, c, t, h, w, int(flags), int(act),
+                                                     float(alpha), float(gain), _stream(dz)), 'dblock_tail_adjoint') == LVG_UNSUPPORTED:
+                raise RuntimeError('dblock_tail_adjoint: ' + self._lib.lvg_last_error().decode())
+        return dy, ds, db
+
+
 _PLUGIN_CLASSES = {
+    'dblock_tail_plugin': DblockTailPlugin,
     'gblock_tail_plugin': GblockTailPlugin,
     'augment_pipe_plugin': AugmentPipePlugin,
     'video_augment_plugin': VideoAugmentPlugin,

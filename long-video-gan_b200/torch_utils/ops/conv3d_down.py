@@ -279,8 +279,22 @@ def _conv3d_layer_forward(orig):
     return forward
 
 
+_WRAPPERS = ('lvg_conv3d_down', 'lvg_conv_bias_act')      # attributes under which an install keeps the method it replaced
+
+
+def wrapped_by(forward, attr):
+    """``forward`` or a method below it in the chain of installed wrappers carries ``attr``. conv3d_down.install (layers with
+    downsampling) and dblock_tail.install (layers without) both replace Conv3dLayer.forward, each calling the method it
+    replaced for the other's layers, in either order."""
+    while forward is not None:
+        if hasattr(forward, attr):
+            return True
+        forward = next((getattr(forward, a) for a in _WRAPPERS if hasattr(forward, a)), None)
+    return False
+
+
 def _patch(cls):
-    if getattr(cls.forward, 'lvg_conv3d_down', None) is None:
+    if not wrapped_by(cls.forward, 'lvg_conv3d_down'):
         cls.forward = _conv3d_layer_forward(cls.forward)
 
 

@@ -189,10 +189,31 @@ def conv_transpose2d(input, weight, bias=None, stride=1, padding=0, output_paddi
     return y
 
 
+class _BiasActGrad(torch.autograd.Function):
+    """dz = G(y) * dy, G the slope of linear / lrelu with gain and clamp decided from the saved output y (bias_act's grad-1
+    kernel; the sign of y is the sign of the pre-activation). Linear in dy with a piecewise constant G, so it is its own
+    backward."""
+
+    @staticmethod
+    def forward(ctx, dy, y, cfg):
+        from . import bias_act as ba
+        act, alpha, gain, clamp = cfg
+        ctx.save_for_backward(y)
+        ctx.cfg = cfg
+        return ba._plugin.bias_act(dy.contiguous(), None, None, y, None, 1, 1, ba.activation_funcs[act].cuda_idx, alpha, gain,
+                                   -1.0 if clamp is None else clamp)
+
+    @staticmethod
+    def backward(ctx, g):
+        y, = ctx.saved_tensors
+        return (_BiasActGrad.apply(g, y, ctx.cfg) if ctx.needs_input_grad[0] else None), None, None
+
+
 class _ConvBiasAct(torch.autograd.Function):
     """conv -> bias_act in ONE kernel: the convolution's epilogue adds the bias, applies linear / lrelu, gain and clamp while
     the accumulators leave the registers (no write + re-read of the pre-activation tensor). Backward: the activation
-    gradient from the saved output (bias_act semantics, bias_act.py:91-120), then the convolution gradients."""
+    gradient from the saved output (``_BiasActGrad``), then the convolution gradients; with create_graph=True every step is
+    a recorded Function, so gradients of any order work."""
 
     @staticmethod
     def forward(ctx, x, w, b, padding, groups, stride, act, alpha, gain, clamp):
@@ -204,12 +225,9 @@ class _ConvBiasAct(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dy):
-        from . import bias_act as ba
         x, w, y = ctx.saved_tensors
         padding, groups, stride, act, alpha, gain, clamp, has_b = ctx.cfg
-        # d(pre-activation): the bias_act backward kernel from the saved output (sign of y = sign of the pre-activation)
-        spec = ba.activation_funcs[act]
-        dz = ba._plugin.bias_act(dy.contiguous(), None, None, y, None, 1, 1, spec.cuda_idx, alpha, gain, -1.0 if clamp is None else clamp)
+        dz = _BiasActGrad.apply(dy, y, (act, alpha, gain, clamp))        # d(pre-activation)
         dx = dw = db = None
         want_dw = ctx.needs_input_grad[1] and not _weights_off()
         if ctx.needs_input_grad[0] and want_dw and _fused_backward_ok(dz):
@@ -220,15 +238,15 @@ class _ConvBiasAct(torch.autograd.Function):
             if want_dw:
                 dw = _ConvNdWgrad.apply(dz, x, w.shape, padding, groups, stride)
         if has_b and ctx.needs_input_grad[2]:
-            db = dz.float().sum([0] + list(range(2, dz.ndim))).to(dz.dtype)
+            db = (dz.float() if dz.dtype == torch.float16 else dz).sum([0] + list(range(2, dz.ndim))).to(dz.dtype)
         return dx, dw, db, None, None, None, None, None, None, None
 
 
 def conv_bias_act(x, w, b=None, stride=1, padding=0, groups=1, act='linear', alpha=None, gain=None, clamp=None):
     """``bias_act(conv(x, w), b, act=act, alpha=alpha, gain=gain, clamp=clamp)`` for act in ('linear', 'lrelu') -- what
     Conv3dLayer / Conv2dLayer compute (discriminator_lres.py:135-213, discriminator_sres.py:192-204, generator_lres.py:578-589)
-    -- with the bias / activation / gain / clamp fused into the convolution's epilogue on CUDA. First order only (the
-    separate ops support double backward). Falls back to the two separate ops outside the engine's envelope."""
+    -- with the bias / activation / gain / clamp fused into the convolution's epilogue on CUDA. Gradients of any order.
+    Falls back to the two separate ops outside the engine's envelope."""
     from . import bias_act as ba
     assert act in ('linear', 'lrelu')
     spec = ba.activation_funcs[act]
