@@ -414,6 +414,32 @@ int lvg_dblock_tail_adjoint(const void* dz, const uint8_t* codes, const float* f
                             float alpha, float gain, void* stream);
 
 /*
+ * Input of a super-res generator layer (generator_sres.py: Generator.prep_cond, the concatenation in
+ * SynthesisNetwork.forward and the cast in SynthesisLayer.forward) as one op, written in the layer's dtype (DESIGN.md 7h):
+ *   z[n t + t', :c]               = z_dtype(x[n t + t'])                     (c = 0: no x)
+ *   z[n t + t', c + k window + s] = z_dtype(A_H lr[n][k][t' + s] A_W^T)       k < c_lr, s < window
+ * x: dense [n t][c][h_out][w_out] (x_dtype); lr: fp32 [n][c_lr][t_lr][h_lr][w_lr] with element strides lr_strides[5];
+ * z: dense [n t][c + c_lr window][h_out][w_out], 16-byte aligned. A_H / A_W: the per-axis plan, LVG_SRES_COND_NPLAN ints
+ * {out, px0, mhi, x0, up, down, pad0, zlen, shift, ntaps} (host memory): output index i reads the resampler output
+ * m = x0 + clamp(i - px0, 0, mhi); that is gain * sum_k f[ntaps - 1 - k] * u[m down + k - pad0] with u the frame
+ * upsampled by `up` (zeros inserted) and zero outside [0, zlen); sample v of the frame is low-res row / column
+ * clamp(v - shift, 0, len - 1). ntaps = 0: an identity axis (up = down = 1, pad0 = 0, f NULL). f_h / f_w: the 1-D fp32
+ * filters on the device, at most 64 taps. Values are accumulated in fp32 and rounded once.
+ * mean_sq (NULL = not wanted): one fp32 on the device, the mean of the squares of the fp32 concatenation (x before any
+ * cast, the conditioning before rounding), summed from one partial per CTA in `workspace` (lvg_sres_cond_workspace bytes)
+ * by a second kernel in a fixed order: bitwise reproducible, no atomics. One kernel launch, two with mean_sq. The size
+ * query returns -1 for shapes and plans it does not take (more than 64 taps, tap tables beyond shared memory, t +
+ * window - 1 > t_lr, a z_dtype other than fp32 / fp16); such calls return LVG_UNSUPPORTED.
+ */
+#define LVG_SRES_COND_NPLAN 10
+int64_t lvg_sres_cond_workspace(int n, int t, int c, int c_lr, int window, int t_lr, int h_lr, int w_lr, int z_dtype,
+                                const int* plan_h, const int* plan_w);
+int lvg_sres_cond(const void* x, const float* lr, const float* f_h, const float* f_w, void* z, float* mean_sq, void* workspace,
+                  int64_t workspace_bytes, int x_dtype, int z_dtype, int n, int t, int c, int c_lr, int window, int t_lr,
+                  int h_lr, int w_lr, const int64_t* lr_strides, const int* plan_h, const int* plan_w, float gain_h,
+                  float gain_w, void* stream);
+
+/*
  * Post-processing of an all-reduced flat gradient buffer, in place and in one pass:
  *   g = g * scale;  NaN -> 0, +inf -> +limit, -inf -> -limit  (finite values untouched)
  * -- the `/ world_size * gain` + `nan_to_num(nan=0, posinf=1e5, neginf=-1e5)` tail of

@@ -89,6 +89,8 @@ _SIGNATURES = {
     'lvg_dblock_tail_codes_bytes': (_c_i64, [_c_int] * 6),
     'lvg_dblock_tail': (_c_int, [_c_void_p] * 6 + [_c_int] * 9 + [_c_float] * 3 + [_c_void_p]),
     'lvg_dblock_tail_adjoint': (_c_int, [_c_void_p] * 7 + [_c_i64] + [_c_int] * 8 + [_c_float] * 2 + [_c_void_p]),
+    'lvg_sres_cond_workspace': (_c_i64, [_c_int] * 9 + [_c_void_p] * 2),
+    'lvg_sres_cond': (_c_int, [_c_void_p] * 7 + [_c_i64] + [_c_int] * 10 + [_c_void_p] * 3 + [_c_float] * 2 + [_c_void_p]),
 }
 
 LVG_UNSUPPORTED = -1
@@ -966,7 +968,73 @@ class DblockTailPlugin:
         return dy, ds, db
 
 
+class SresCondPlugin:
+    """Input of a super-res generator layer: x_prev cast to the layer's dtype, concatenated with the layer's conditioning
+    built from the low-res video, and optionally the mean square of the fp32 concatenation (no reference plugin:
+    Generator.prep_cond, torch.cat and Tensor.to, generator_sres.py:581-610, 462-464, 307-325). ``plan_h`` / ``plan_w``:
+    LVG_SRES_COND_NPLAN ints per axis (see lvg_sres_cond in include/lvg_ops.h and torch_utils/ops/sres_cond.py)."""
+
+    NPLAN = 10
+
+    def __init__(self, lib):
+        self._lib = lib
+
+    @classmethod
+    def _plan(cls, q):
+        if len(q) != cls.NPLAN:
+            raise RuntimeError(f'sres_cond: a plan holds {cls.NPLAN} ints per axis')
+        return (_c_int * cls.NPLAN)(*[int(v) for v in q])
+
+    def workspace(self, n, t, c, c_lr, window, t_lr, h_lr, w_lr, dtype, plan_h, plan_w):
+        """Workspace bytes of a call with the mean square, or -1 where the kernel does not take the shape and plan."""
+        return int(self._lib.lvg_sres_cond_workspace(n, t, c, c_lr, window, t_lr, h_lr, w_lr, _DTYPE_CODE.get(dtype, -1),
+                                                     self._plan(plan_h), self._plan(plan_w)))
+
+    def forward(self, x, lr, f_h, f_w, plan_h, plan_w, gain_h, gain_w, window, dtype, want_sumsq):
+        """(z [N T, C + C_lr window, H, W] in ``dtype``, mean square (fp32 0-dim) or None) from x [N T, C, H, W] (fp16 /
+        fp32, or None) and lr [N, C_lr, T_lr, h, w] (fp32, any strides), T = T_lr - window + 1."""
+        if not lr.is_cuda or lr.dtype != torch.float32 or lr.ndim != 5:
+            raise RuntimeError('sres_cond: lr must be a 5-D float32 CUDA tensor')
+        if dtype not in (torch.float16, torch.float32):
+            raise RuntimeError(f'sres_cond: unsupported layer dtype {dtype}')
+        n, c_lr, t_lr, h_lr, w_lr = lr.shape
+        t = t_lr - window + 1
+        c = 0
+        if x is not None:
+            if not x.is_cuda or x.dtype not in (torch.float16, torch.float32) or x.ndim != 4 or x.device != lr.device:
+                raise RuntimeError('sres_cond: x must be a 4-D float16 / float32 tensor on the device of lr')
+            if x.shape[0] != n * t or list(x.shape[2:]) != [int(plan_h[0]), int(plan_w[0])]:
+                raise RuntimeError(f'sres_cond: x of shape {list(x.shape)} does not match the plan ({n * t} samples, '
+                                   f'{int(plan_h[0])} x {int(plan_w[0])})')
+            x = x.contiguous()
+            c = x.shape[1]
+        for f, q in ((f_h, plan_h), (f_w, plan_w)):
+            k = int(q[9])
+            if (k == 0) != (f is None) or f is not None and (f.dtype != torch.float32 or f.numel() != k or f.device != lr.device):
+                raise RuntimeError(f'sres_cond: a filter of {k} float32 taps on the device of lr (None for an identity axis)')
+        f_h = None if f_h is None else f_h.contiguous()
+        f_w = None if f_w is None else f_w.contiguous()
+        ph, pw = self._plan(plan_h), self._plan(plan_w)
+        nbytes = int(self._lib.lvg_sres_cond_workspace(n, t, c, c_lr, window, t_lr, h_lr, w_lr, _DTYPE_CODE[dtype], ph, pw))
+        if nbytes < 0:
+            raise RuntimeError(f'sres_cond: no kernel for {list(lr.shape)}, window {window}, plan {list(plan_h)} / {list(plan_w)}')
+        z = torch.empty([n * t, c + c_lr * window, int(plan_h[0]), int(plan_w[0])], dtype=dtype, device=lr.device)
+        ms = ws = None
+        if want_sumsq:
+            ms = torch.empty([], dtype=torch.float32, device=lr.device)
+            ws = torch.empty([nbytes // 8], dtype=torch.float64, device=lr.device)
+        strides = (_c_i64 * 5)(*lr.stride())
+        with _DeviceGuard(lr):
+            if _check(self._lib.lvg_sres_cond(_ptr(x), _ptr(lr), _ptr(f_h), _ptr(f_w), _ptr(z), _ptr(ms), _ptr(ws), nbytes,
+                                              _DTYPE_CODE[x.dtype] if x is not None else _DTYPE_CODE[dtype], _DTYPE_CODE[dtype],
+                                              n, t, c, c_lr, window, t_lr, h_lr, w_lr, strides, ph, pw, float(gain_h),
+                                              float(gain_w), _stream(lr)), 'sres_cond') == LVG_UNSUPPORTED:
+                raise RuntimeError('sres_cond: ' + self._lib.lvg_last_error().decode())
+        return z, ms
+
+
 _PLUGIN_CLASSES = {
+    'sres_cond_plugin': SresCondPlugin,
     'dblock_tail_plugin': DblockTailPlugin,
     'gblock_tail_plugin': GblockTailPlugin,
     'augment_pipe_plugin': AugmentPipePlugin,
