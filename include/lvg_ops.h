@@ -440,6 +440,50 @@ int lvg_sres_cond(const void* x, const float* lr, const float* f_h, const float*
                   float gain_w, void* stream);
 
 /*
+ * Layers of a super-res discriminator block (discriminator_sres.py DiscriminatorBlock, architecture 'resnet'; DESIGN.md 7i).
+ *
+ * lvg_sres_dblock_conv1: conv1, y = bias_act(conv2d(upfirdn2d(x, f, padding 2), w, stride 2), bias, act, alpha, gain,
+ * clamp) with f = outer(fy, fx) 4 x 4 (fx, fy: 4 fp32 taps each on the device; flip as upfirdn2d's flip_filter). The FIR
+ * runs inside the convolution's re-tiling pass (fp32 accumulation, rounded once to fp16 or split once into bf16 halves); the
+ * filtered image is never stored. x: dense fp16 / fp32 [n][cin][h][wd]; w: [cout][cin][3][3] in x's dtype; bias: fp32
+ * [cout] or NULL; y: [n][cout][h / 2][wd / 2] rounded down plus one where odd ((h + 1 - 3) / 2 + 1). act: 0 none,
+ * 1 linear, 2 lrelu, as lvg_convnd_fprop; clamp < 0: none. Two launches (re-tiling, convolution) plus the weight re-tiling.
+ *
+ * lvg_sres_dblock_skip: the skip with the residual merge, y = (W x + r) * rscale: a 1x1 convolution of the down-sampled
+ * input x [n][cin][P] (w: [cout][cin]) on the pointwise wgmma kernels, the residual r [n][cout][P] (conv1's output, x's
+ * dtype and layout) added to the fp32 accumulator and the sum scaled by rscale in the epilogue, one rounding to x's dtype.
+ * x, r, y 16-byte aligned; P % 4 == 0 (fp32) or P % 8 == 0 (fp16).
+ *
+ * lvg_sres_dblock_conv1_backward: conv1's first-order backward from dy (the gradient of conv1's pre-activation, [n][cout]
+ * [h / 2][wd / 2]): dhf = the gradient of the filtered image [n][cin][h + 1][wd + 1] (NULL = not wanted) as
+ * lvg_convnd_dgrad computes it, and dw [cout][cin][3][3] (NULL = not wanted) from the weight-gradient kernel with its x
+ * operand re-tiled straight from x by the FIR re-tiling pass: bit for bit lvg_convnd_wgrad of the filtered image that
+ * pass computes, which is never stored in NCHW.
+ *
+ * lvg_sres_dblock_fir_adjoint_act: dz = G(h0) (.) FIR^T(dhf) for h0 [n][c][h][w] (conv0's output) and dhf [n][c][h + 1]
+ * [w + 1]: the adjoint of upfirdn2d(., f, padding 2) (fp32, rounded once) times bias_act's first-order slope decided from h0
+ * (act 1 linear / 2 lrelu, alpha, gain, clamp < 0: none); db (fp32 [c], NULL = not wanted) = the sum of the stored dz per
+ * channel, per-CTA partials folded in a fixed order (no atomics, bitwise reproducible). Two launches.
+ *
+ * The size queries return -1 outside the envelope; the ops then return LVG_UNSUPPORTED.
+ */
+int64_t lvg_sres_dblock_conv1_workspace(int dtype, int n, int cin, int cout, int h, int wd);
+int lvg_sres_dblock_conv1(const void* x, const float* fx, const float* fy, int flip, const void* w, const float* bias, void* y,
+                          int dtype, int n, int cin, int cout, int h, int wd, int act, float alpha, float gain, float clamp,
+                          void* workspace, int64_t workspace_bytes, void* stream);
+int64_t lvg_sres_dblock_conv1_backward_workspace(int dtype, int n, int cin, int cout, int h, int wd);
+int lvg_sres_dblock_conv1_backward(const void* x, const float* fx, const float* fy, int flip, const void* dy, const void* w,
+                                   void* dhf, void* dw, int dtype, int n, int cin, int cout, int h, int wd, void* workspace,
+                                   int64_t workspace_bytes, void* stream);
+int64_t lvg_sres_dblock_fir_adjoint_act_workspace(int dtype, int n, int c, int h, int w);
+int lvg_sres_dblock_fir_adjoint_act(const void* dhf, const void* h0, const float* fx, const float* fy, int flip, void* dz,
+                                    float* db, void* workspace, int64_t workspace_bytes, int dtype, int n, int c, int h, int w,
+                                    int act, float alpha, float gain, float clamp, void* stream);
+int64_t lvg_sres_dblock_skip_workspace(int dtype, int n, int cin, int cout, int64_t P);
+int lvg_sres_dblock_skip(const void* x, const void* w, const void* r, void* y, int dtype, int n, int cin, int cout, int64_t P,
+                         float rscale, void* workspace, int64_t workspace_bytes, void* stream);
+
+/*
  * Post-processing of an all-reduced flat gradient buffer, in place and in one pass:
  *   g = g * scale;  NaN -> 0, +inf -> +limit, -inf -> -limit  (finite values untouched)
  * -- the `/ world_size * gain` + `nan_to_num(nan=0, posinf=1e5, neginf=-1e5)` tail of

@@ -44,7 +44,7 @@ int pw_conv(const float* x, const float* w, float* y, int n, int cin, int cout, 
 // conv_pw_tc.cu: every other 1x1x1 forward / input gradient on wgmma, straight from the NC(T)HW tensors (no re-tiling)
 bool pw_tc_supported(int dtype, int groups, int cin, int cout, int kt, int kh, int kw, int pad_t, int pad_h, int pad_w, int stride, int64_t P);
 int pw_tc_conv(const void* x, const void* w, void* y, int dtype, int n, int ck, int cm, int64_t P, int64_t w_sm, int64_t w_sk, void* workspace,
-               int64_t workspace_bytes, cudaStream_t s);
+               int64_t workspace_bytes, cudaStream_t s, const void* res = nullptr, float rscale = 1.f);
 }
 
 namespace lvg {
@@ -177,6 +177,81 @@ int pack_act(const void* x, void* x8, int split, int64_t inst, int c, int cblk, 
     else conv_pack_act_kernel<__half, false, false><<<(unsigned)blocks, 256, 0, s>>>((const __half*)x, (uint4*)x8, inst, c, cblk, gm);
     LVG_LAUNCH_CHECK();
     return LVG_OK;
+}
+
+// upfirdn2d(x, f, padding = [2, 2, 2, 2]) (up 1, down 1) with a rank-1 4 x 4 filter f = outer(fy, fx), written straight
+// into X8 of the filtered (h + 1) x (w + 1) image: the FIR of conv2d_resample's down-sampling 3x3 path fused into the
+// re-tiling, so the filtered image never exists in NCHW. One CTA = one 8-channel block of one sample and a 32 x 8 tile of
+// filtered pixels: the (8 + 3) x (32 + 3) input window of the 8 channels goes to shared memory once (zeros outside the
+// image and past the last channel), a pass along y and one along x (fp32, taps in order) leave 8 values per thread, and
+// the thread writes its pixel of the block as one 16-byte store (SPLIT: the bf16 hi and lo halves, one store each).
+// gx / gy: the taps oriented for correlation (mirrored unless flip, as upfirdn2d orients them).
+constexpr int kFirTX = 32, kFirTY = 8, kFirPitch = kFirTX + 4;
+
+template <class TIn, bool SPLIT>
+__global__ void __launch_bounds__(256) conv_pack_fir4_kernel(const TIn* __restrict__ x, uint4* __restrict__ y, int c, int cblk, int h, int w,
+                                                              const float* __restrict__ fx, const float* __restrict__ fy, int flip)
+{
+    __shared__ float s_in[8][kFirTY + 3][kFirPitch];
+    __shared__ float s_mid[8][kFirTY][kFirPitch];
+    const int ho = h + 1, wo = w + 1;
+    const int ox0 = blockIdx.x * kFirTX, oy0 = blockIdx.y * kFirTY;
+    const int blk = (int)(blockIdx.z % cblk);
+    const int64_t in = blockIdx.z / cblk;
+    const int c0 = blk * 8;
+    float gx[4], gy[4];
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        gx[k] = __ldg(fx + (flip ? k : 3 - k));
+        gy[k] = __ldg(fy + (flip ? k : 3 - k));
+    }
+    const TIn* xs = x + ((int64_t)in * c + c0) * h * w;
+    for (int i = threadIdx.x; i < 8 * (kFirTY + 3) * (kFirTX + 3); i += 256) {
+        const int col = i % (kFirTX + 3), r = (i / (kFirTX + 3)) % (kFirTY + 3), ch = i / ((kFirTX + 3) * (kFirTY + 3));
+        const int iy = oy0 + r - 2, ix = ox0 + col - 2;
+        float v = 0.f;
+        if (c0 + ch < c && iy >= 0 && iy < h && ix >= 0 && ix < w) {
+            if constexpr (SPLIT) v = __ldg(reinterpret_cast<const float*>(xs) + ((int64_t)ch * h + iy) * w + ix);
+            else v = __half2float(__ldg(reinterpret_cast<const __half*>(xs) + ((int64_t)ch * h + iy) * w + ix));
+        }
+        s_in[ch][r][col] = v;
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < 8 * kFirTY * (kFirTX + 3); i += 256) {
+        const int col = i % (kFirTX + 3), r = (i / (kFirTX + 3)) % kFirTY, ch = i / ((kFirTX + 3) * kFirTY);
+        float v = 0.f;
+#pragma unroll
+        for (int k = 0; k < 4; k++) v = fmaf(gy[k], s_in[ch][r + k][col], v);
+        s_mid[ch][r][col] = v;
+    }
+    __syncthreads();
+    const int tx = threadIdx.x % kFirTX, ty = threadIdx.x / kFirTX;
+    const int oy = oy0 + ty, ox = ox0 + tx;
+    if (oy >= ho || ox >= wo) return;
+    float v[8];
+#pragma unroll
+    for (int ch = 0; ch < 8; ch++) {
+        float a = 0.f;
+#pragma unroll
+        for (int k = 0; k < 4; k++) a = fmaf(gx[k], s_mid[ch][ty][tx + k], a);
+        v[ch] = a;
+    }
+    const int64_t plane = (int64_t)ho * wo, off = (int64_t)oy * wo + ox;
+    if constexpr (!SPLIT) {
+        alignas(16) __half o[8];
+#pragma unroll
+        for (int ch = 0; ch < 8; ch++) o[ch] = __float2half_rn(v[ch]);
+        y[(in * cblk + blk) * plane + off] = *reinterpret_cast<const uint4*>(o);
+    } else {
+        alignas(16) unsigned short hi[8], lo[8];
+#pragma unroll
+        for (int ch = 0; ch < 8; ch++) {
+            hi[ch] = bf16_bits(v[ch]);
+            lo[ch] = bf16_bits(v[ch] - bf16_val(hi[ch]));
+        }
+        y[(in * 2 * cblk + blk) * plane + off] = *reinterpret_cast<const uint4*>(hi);
+        y[(in * 2 * cblk + cblk + blk) * plane + off] = *reinterpret_cast<const uint4*>(lo);
+    }
 }
 
 // weights -> tile images.  Element (m, k, tap) of the logical A matrix of group g sits at
@@ -1139,8 +1214,10 @@ WgradKernel wgrad_kernel(int split, int taps, int nt) { return split ? wgrad_ker
 // the weight-gradient launch; `dy8_pre` != nullptr: dy is already re-tiled (the tensor the input gradient of the same call read)
 int run_wgrad(const void* x, const void* dy, void* dw, int dtype, int n, int groups, int cin, int cout, int t, int h, int wd, int kt, int kh,
               int kw, int pad_t, int pad_h, int pad_w, int stride, const unsigned char* dy8_pre, void* workspace, int64_t workspace_bytes,
-              cudaStream_t s, const float* x_scale = nullptr, const float* dy_scale = nullptr)
+              cudaStream_t s, const float* x_scale = nullptr, const float* dy_scale = nullptr, const unsigned char* x8_pre = nullptr)
 {
+    // `x8_pre` != nullptr: x is already re-tiled there, with cpad_b / 8 blocks (conv_pack_fir4_kernel: the filtered image of
+    // a super-res discriminator block); x is not read
     const int to = t + 2 * pad_t - kt + 1, ho = h + 2 * pad_h - kh + 1, wo = wd + 2 * pad_w - kw + 1;
     const WgradPlan q = wgrad_plan(dtype, n, groups, cin, cout, t, h, wd, to, ho, wo, kt, kh, kw);
     const int64_t a_room = dy8_pre ? 0 : ((q.a_bytes + 255) / 256) * 256;
@@ -1148,16 +1225,16 @@ int run_wgrad(const void* x, const void* dy, void* dw, int dtype, int n, int gro
     LVG_REQUIRE(aligned16(workspace), "convnd_wgrad: workspace must be 16-byte aligned");
     LVG_REQUIRE(groups <= 65535 && q.mt <= 65535, "convnd_wgrad: too many groups / channel tiles");
     const int64_t inst = (int64_t)n * groups;
-    unsigned char* x8 = reinterpret_cast<unsigned char*>(workspace) + a_room;
+    unsigned char* x8 = x8_pre ? const_cast<unsigned char*>(x8_pre) : reinterpret_cast<unsigned char*>(workspace) + a_room;
     unsigned char* dy8 = dy8_pre ? const_cast<unsigned char*>(dy8_pre) : reinterpret_cast<unsigned char*>(workspace);
-    float* part = reinterpret_cast<float*>(x8 + ((q.b_bytes + 255) / 256) * 256);
+    float* part = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(workspace) + a_room + ((q.b_bytes + 255) / 256) * 256);
     const int64_t thw_a = (int64_t)to * ho * wo, thw_b = (int64_t)t * h * wd;
     {
         // dy of a strided convolution is spread over every stride-th pixel of the stride-1 output grid (zeros between)
         int rc = dy8_pre ? LVG_OK : pack_act(dy, dy8, q.split, inst, cout, q.cpad_a / 8, to, (ho - 1) / stride + 1, (wo - 1) / stride + 1, ho, wo, stride, s,
                                              dy_scale);
         if (rc) return rc;
-        rc = pack_act(x, x8, q.split, inst, cin, q.cpad_b / 8, t, h, wd, h, wd, 1, s, x_scale);   // x_scale [n][cin][t]: x is modulated
+        rc = x8_pre ? LVG_OK : pack_act(x, x8, q.split, inst, cin, q.cpad_b / 8, t, h, wd, h, wd, 1, s, x_scale);   // x_scale [n][cin][t]: x is modulated
         if (rc) return rc;
     }
     WgradV2Params p;
@@ -1381,6 +1458,103 @@ extern "C" int lvg_convnd_backward(const void* x, const void* dy, const void* w,
     // (stream order: the weight gradient's re-tiling of x overwrites the packed weights only after the input gradient read them)
     return run_wgrad(x, dy, dw, dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, stride, dy8, rest,
                      workspace_bytes - dy8_room, s);
+}
+
+// ---- conv1 of a super-res discriminator block (conv2d_resample with down = 2, a 3x3 kernel and padding 1): the 4-tap FIR
+// with padding 2 runs inside the re-tiling pass (conv_pack_fir4_kernel), the stride-2 convolution and its bias_act epilogue
+// on the engine as lvg_convnd_fprop runs them. Workspace: [packed weights][X8 of the filtered image].
+extern "C" int64_t lvg_sres_dblock_conv1_workspace(int dtype, int n, int cin, int cout, int h, int wd)
+{
+    if ((dtype != LVG_F16 && dtype != LVG_F32) || n < 1 || cin < 1 || cout < 1 || h < 2 || wd < 2) return -1;
+    const int hf = h + 1, wf = wd + 1;
+    const Geometry g = geometry(dtype == LVG_F32, n, 1, cin, cout, (int64_t)hf * wf, 9);
+    if ((int64_t)n * g.cblk > 65535 || (int64_t)n * g.nblk >= (1ll << 31) || wf - 2 > 4 * (128 - 2)) return -1;
+    return ((g.w_bytes + 256 + 255) / 256) * 256 + g.act_bytes + 256;
+}
+
+extern "C" int lvg_sres_dblock_conv1(const void* x, const float* fx, const float* fy, int flip, const void* w, const float* bias, void* y, int dtype,
+                                     int n, int cin, int cout, int h, int wd, int act, float alpha, float gain, float clamp, void* workspace,
+                                     int64_t workspace_bytes, void* stream)
+{
+    LVG_REQUIRE(x && fx && fy && w && y, "sres_dblock_conv1: x, fx, fy, w, y must not be NULL");
+    const int64_t need = lvg_sres_dblock_conv1_workspace(dtype, n, cin, cout, h, wd);
+    if (need < 0) {
+        set_error("sres_dblock_conv1: outside the kernels' envelope");
+        return LVG_UNSUPPORTED;
+    }
+    LVG_REQUIRE(workspace && aligned16(workspace) && workspace_bytes >= need, "sres_dblock_conv1: workspace too small or misaligned");
+    cudaStream_t s = (cudaStream_t)stream;
+    const int split = dtype == LVG_F32;
+    const int hf = h + 1, wf = wd + 1;
+    const Geometry g = geometry(split, n, 1, cin, cout, (int64_t)hf * wf, 9);
+    const int64_t wp_room = ((g.w_bytes + 256 + 255) / 256) * 256;
+    unsigned char* x8 = reinterpret_cast<unsigned char*>(workspace) + wp_room;
+    {
+        const dim3 grid((unsigned)((wf + kFirTX - 1) / kFirTX), (unsigned)((hf + kFirTY - 1) / kFirTY), (unsigned)(n * g.cblk));
+        if (split) conv_pack_fir4_kernel<float, true><<<grid, 256, 0, s>>>((const float*)x, (uint4*)x8, cin, g.cblk, h, wd, fx, fy, flip);
+        else conv_pack_fir4_kernel<__half, false><<<grid, 256, 0, s>>>((const __half*)x, (uint4*)x8, cin, g.cblk, h, wd, fx, fy, flip);
+        LVG_LAUNCH_CHECK();
+    }
+    return run_igemm(x8, w, y, dtype, n, 1, cin, cout, 1, hf, wf, 1, 3, 3, 0, 0, 0, (int64_t)cout * cin * 9, (int64_t)cin * 9, 9, 0, bias, act, alpha,
+                     gain, clamp, hf, wf, 1, 2, x8, workspace, wp_room, s);
+}
+
+// ---- conv1's backward: dhf = the input gradient of the strided convolution (the filtered image's gradient, (h + 1) x (wd + 1),
+// lvg_convnd_dgrad), and dw from the weight-gradient kernel with its B operand re-tiled straight from x by
+// conv_pack_fir4_kernel (the filtered image is recomputed into X8, never into NCHW). Workspace: [X8 of the filtered image]
+// [the larger of the two kernels' workspaces].
+namespace lvg {
+namespace {
+int64_t conv1_bwd_x8_bytes(int dtype, int n, int cin, int cout, int h, int wd)
+{
+    const WgradPlan q = wgrad_plan(dtype, n, 1, cin, cout, 1, h + 1, wd + 1, 1, h - 1, wd - 1, 1, 3, 3);
+    return ((q.b_bytes + 255) / 256) * 256;
+}
+}  // namespace
+}  // namespace lvg
+
+extern "C" int64_t lvg_sres_dblock_conv1_backward_workspace(int dtype, int n, int cin, int cout, int h, int wd)
+{
+    if (lvg_sres_dblock_conv1_workspace(dtype, n, cin, cout, h, wd) < 0) return -1;
+    if (!wgrad_in_envelope(dtype, n, 1, 1, h + 1, wd + 1, 1, 3, 3, 0, 0, 0, 2)) return -1;
+    const int64_t a = lvg_convnd_workspace(dtype, n, 1, cin, cout, 1, h + 1, wd + 1, 1, 3, 3, 0, 0, 0);
+    const int64_t b = lvg_convnd_wgrad_workspace(dtype, n, 1, cin, cout, 1, h + 1, wd + 1, 1, 3, 3, 0, 0, 0);
+    if (a < 0 || b < 0) return -1;
+    return conv1_bwd_x8_bytes(dtype, n, cin, cout, h, wd) + (a > b ? a : b) + 1024;
+}
+
+extern "C" int lvg_sres_dblock_conv1_backward(const void* x, const float* fx, const float* fy, int flip, const void* dy, const void* w, void* dhf,
+                                              void* dw, int dtype, int n, int cin, int cout, int h, int wd, void* workspace, int64_t workspace_bytes,
+                                              void* stream)
+{
+    LVG_REQUIRE(x && fx && fy && dy && w && (dhf || dw), "sres_dblock_conv1_backward: x, fx, fy, dy, w and dhf or dw must not be NULL");
+    const int64_t need = lvg_sres_dblock_conv1_backward_workspace(dtype, n, cin, cout, h, wd);
+    if (need < 0) {
+        set_error("sres_dblock_conv1_backward: outside the kernels' envelope");
+        return LVG_UNSUPPORTED;
+    }
+    LVG_REQUIRE(workspace && aligned16(workspace) && workspace_bytes >= need, "sres_dblock_conv1_backward: workspace too small or misaligned");
+    cudaStream_t s = (cudaStream_t)stream;
+    const int hf = h + 1, wf = wd + 1;
+    const int64_t x8_room = conv1_bwd_x8_bytes(dtype, n, cin, cout, h, wd);
+    unsigned char* x8 = reinterpret_cast<unsigned char*>(workspace);
+    unsigned char* rest = x8 + x8_room;
+    const int64_t rest_bytes = workspace_bytes - x8_room;
+    if (dhf) {
+        const int rc = lvg_convnd_dgrad(dy, w, dhf, dtype, n, 1, cin, cout, 1, hf, wf, 1, 3, 3, 0, 0, 0, 2, rest, rest_bytes, stream);
+        if (rc) return rc;
+    }
+    if (!dw) return LVG_OK;
+    const WgradPlan q = wgrad_plan(dtype, n, 1, cin, cout, 1, hf, wf, 1, hf - 2, wf - 2, 1, 3, 3);
+    const int cblk = q.cpad_b / 8;
+    LVG_REQUIRE((int64_t)n * cblk <= 65535, "sres_dblock_conv1_backward: too many channel blocks");
+    {
+        const dim3 grid((unsigned)((wf + kFirTX - 1) / kFirTX), (unsigned)((hf + kFirTY - 1) / kFirTY), (unsigned)(n * cblk));
+        if (q.split) conv_pack_fir4_kernel<float, true><<<grid, 256, 0, s>>>((const float*)x, (uint4*)x8, cin, cblk, h, wd, fx, fy, flip);
+        else conv_pack_fir4_kernel<__half, false><<<grid, 256, 0, s>>>((const __half*)x, (uint4*)x8, cin, cblk, h, wd, fx, fy, flip);
+        LVG_LAUNCH_CHECK();
+    }
+    return run_wgrad(nullptr, dy, dw, dtype, n, 1, cin, cout, 1, hf, wf, 1, 3, 3, 0, 0, 0, 2, nullptr, rest, rest_bytes, s, nullptr, nullptr, x8);
 }
 
 // =================================================================================================

@@ -57,6 +57,8 @@ struct PwTcParams {
     int raw_bytes;               // TMA payload of a stage: 32 channels x 128 pixels
     int w_step;                  // bytes of the weight images of one k step: nimg * a_img
     int w_off, b_off, stage_bytes;
+    const void* res;             // RES: residual operand [n][cout][P] in y's dtype, y = (acc + res) * rscale
+    float rscale;
 };
 
 __device__ __forceinline__ unsigned short pt_bf16_bits(float v) { return __bfloat16_as_ushort(__float2bfloat16_rn(v)); }
@@ -110,9 +112,10 @@ __global__ void __launch_bounds__(256) conv_pw_tc_pack_w_kernel(const TW* __rest
 // Stage layout: [raw: 32 channels x 128 pixels as TMA wrote them][weight images of the k steps][converted B images:
 // per k step nimg images of kPtBImg bytes]. B image (MN-major, no swizzle): byte offset(k, px) = (px / 8) * kPtSBO +
 // (k / 8) * 128 + (k % 8) * 16 + (px % 8) * 2 -- 8 x 8 core matrices, LBO = 128 (next 8 channels), SBO = kPtSBO.
-// NW: MMA width of a consumer (128; 64 in 64-row mode).
-template <bool BF16, int NW>
-__global__ void __launch_bounds__(kPtThreads, 1) conv_pw_tc_kernel(const __grid_constant__ CUtensorMap tmx, const PwTcParams p)
+// NW: MMA width of a consumer (128; 64 in 64-row mode). RES: the epilogue adds p.res and scales by p.rscale (fp32, in that
+// order, one rounding to y's dtype); without it the epilogue is the plain store. Two kernels below instantiate it.
+template <bool BF16, int NW, bool RES>
+__device__ __forceinline__ void conv_pw_tc_body(const CUtensorMap& tmx, const PwTcParams& p)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     __shared__ uint64_t full_bar[kPtStages], empty_bar[kPtStages];
@@ -236,13 +239,33 @@ __global__ void __launch_bounds__(kPtThreads, 1) conv_pw_tc_kernel(const __grid_
                 for (int j = 0; j < NW / 8; j++) {
                     const int col = col0 + j * 8 + 2 * (lane % 4);
                     if (p0 + col >= p.P) continue;                 // P is even: the pair is whole
-                    const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                    float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                    if constexpr (RES) {
+                        float2 r;
+                        if constexpr (BF16) r = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(p.res) + base + col);
+                        else r = __half22float2(*reinterpret_cast<const __half2*>(reinterpret_cast<const __half*>(p.res) + base + col));
+                        v0 = __fmul_rn(__fadd_rn(v0, r.x), p.rscale);
+                        v1 = __fmul_rn(__fadd_rn(v1, r.y), p.rscale);
+                    }
                     if constexpr (BF16) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.y) + base + col) = make_float2(v0, v1);
                     else *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.y) + base + col) = __floats2half2_rn(v0, v1);
                 }
             }
         }
     }
+}
+
+template <bool BF16, int NW>
+__global__ void __launch_bounds__(kPtThreads, 1) conv_pw_tc_kernel(const __grid_constant__ CUtensorMap tmx, const PwTcParams p)
+{
+    conv_pw_tc_body<BF16, NW, false>(tmx, p);
+}
+
+// the skip of a super-res discriminator block: y = (W x + res) * rscale
+template <bool BF16, int NW>
+__global__ void __launch_bounds__(kPtThreads, 1) conv_pw_tc_res_kernel(const __grid_constant__ CUtensorMap tmx, const PwTcParams p)
+{
+    conv_pw_tc_body<BF16, NW, true>(tmx, p);
 }
 
 typedef CUresult (*PtEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
@@ -276,13 +299,20 @@ PwTcGeom pw_tc_geometry(int split, int ck, int cm)
 }  // namespace
 
 // the route: LVG_CONV_PW_TC=0 keeps these calls on the engine (read on every call, so one process can compare both)
+namespace {
+bool pw_tc_in_envelope(int dtype, int groups, int cin, int cout, int kt, int kh, int kw, int pad_t, int pad_h, int pad_w, int stride, int64_t P)
+{
+    const int64_t align = dtype == LVG_F32 ? 4 : 8;
+    return (dtype == LVG_F32 || dtype == LVG_F16) && groups == 1 && kt == 1 && kh == 1 && kw == 1 && pad_t == 0 && pad_h == 0 && pad_w == 0 &&
+           stride == 1 && cin >= 1 && cout >= 1 && P >= align && P % align == 0 && P / kPtNP < (1ll << 30);
+}
+}  // namespace
+
 bool pw_tc_supported(int dtype, int groups, int cin, int cout, int kt, int kh, int kw, int pad_t, int pad_h, int pad_w, int stride, int64_t P)
 {
     const char* e = getenv("LVG_CONV_PW_TC");
     if (e && e[0] == '0') return false;
-    const int64_t align = dtype == LVG_F32 ? 4 : 8;
-    return (dtype == LVG_F32 || dtype == LVG_F16) && groups == 1 && kt == 1 && kh == 1 && kw == 1 && pad_t == 0 && pad_h == 0 && pad_w == 0 &&
-           stride == 1 && cin >= 1 && cout >= 1 && P >= align && P % align == 0 && P / kPtNP < (1ll << 30);
+    return pw_tc_in_envelope(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, P);
 }
 
 // bytes of workspace the call needs (the packed weights): never more than the engine's packed weights of the same GEMM
@@ -290,13 +320,14 @@ int64_t pw_tc_workspace(int dtype, int ck, int cm) { return pw_tc_geometry(dtype
 
 // y[n][m][p] = sum_k w[m * w_sm + k * w_sk] * x[n][k][p]: x has ck channels, y cm (forward: ck = cin, cm = cout, w_sm = cin,
 // w_sk = 1; input gradient: x = dy, ck = cout, cm = cin, w_sm = 1, w_sk = cin)
+// `res` != nullptr: y = (W x + res) * rscale, res laid out as y (the residual merge of a super-res discriminator block)
 int pw_tc_conv(const void* x, const void* w, void* y, int dtype, int n, int ck, int cm, int64_t P, int64_t w_sm, int64_t w_sk, void* workspace,
-               int64_t workspace_bytes, cudaStream_t s)
+               int64_t workspace_bytes, cudaStream_t s, const void* res, float rscale)
 {
     const int split = dtype == LVG_F32 ? 1 : 0;
     const int es = split ? 4 : 2;
     const PwTcGeom g = pw_tc_geometry(split, ck, cm);
-    LVG_REQUIRE(aligned16(x) && aligned16(y), "pointwise conv: tensors must be 16-byte aligned");
+    LVG_REQUIRE(aligned16(x) && aligned16(y) && aligned16(res), "pointwise conv: tensors must be 16-byte aligned");
     LVG_REQUIRE(workspace && aligned16(workspace) && workspace_bytes >= g.w_bytes, "pointwise conv: workspace too small");
     PtEncodeFn enc = pt_encode_fn();
     LVG_REQUIRE(enc != nullptr, "pointwise conv: cuTensorMapEncodeTiled is not available from this driver");
@@ -336,10 +367,14 @@ int pw_tc_conv(const void* x, const void* w, void* y, int dtype, int n, int ck, 
     p.w_off = p.raw_bytes;
     p.b_off = p.w_off + kPtKS * p.w_step;
     p.stage_bytes = p.b_off + kPtKS * g.nimg * kPtBImg;
+    p.res = res; p.rscale = rscale;
     const size_t smem = (size_t)kPtStages * p.stage_bytes + 128;
 
     void (*kern)(const CUtensorMap, const PwTcParams) =
-        split ? (g.m64 ? conv_pw_tc_kernel<true, 64> : conv_pw_tc_kernel<true, 128>) : (g.m64 ? conv_pw_tc_kernel<false, 64> : conv_pw_tc_kernel<false, 128>);
+        res ? (split ? (g.m64 ? conv_pw_tc_res_kernel<true, 64> : conv_pw_tc_res_kernel<true, 128>)
+                     : (g.m64 ? conv_pw_tc_res_kernel<false, 64> : conv_pw_tc_res_kernel<false, 128>))
+            : (split ? (g.m64 ? conv_pw_tc_kernel<true, 64> : conv_pw_tc_kernel<true, 128>)
+                     : (g.m64 ? conv_pw_tc_kernel<false, 64> : conv_pw_tc_kernel<false, 128>));
     LVG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int64_t ctas = p.total_tiles < num_sms() ? p.total_tiles : num_sms();
     kern<<<(unsigned)ctas, kPtThreads, smem, s>>>(tm, p);
@@ -348,3 +383,22 @@ int pw_tc_conv(const void* x, const void* w, void* y, int dtype, int n, int ck, 
 }
 
 }  // namespace lvg
+
+// ---- skip of a super-res discriminator block with the block's residual merge: y = (W x + r) * rscale, x the
+// down-sampled block input [n][cin][P], r conv1's output [n][cout][P] in x's dtype
+extern "C" int64_t lvg_sres_dblock_skip_workspace(int dtype, int n, int cin, int cout, int64_t P)
+{
+    if (n < 1 || !lvg::pw_tc_in_envelope(dtype, 1, cin, cout, 1, 1, 1, 0, 0, 0, 1, P)) return -1;
+    return lvg::pw_tc_workspace(dtype, cin, cout);
+}
+
+extern "C" int lvg_sres_dblock_skip(const void* x, const void* w, const void* r, void* y, int dtype, int n, int cin, int cout, int64_t P, float rscale,
+                                    void* workspace, int64_t workspace_bytes, void* stream)
+{
+    LVG_REQUIRE(x && w && r && y, "sres_dblock_skip: x, w, r, y must not be NULL");
+    if (lvg_sres_dblock_skip_workspace(dtype, n, cin, cout, P) < 0) {
+        lvg::set_error("sres_dblock_skip: outside the kernel's envelope");
+        return LVG_UNSUPPORTED;
+    }
+    return lvg::pw_tc_conv(x, w, y, dtype, n, cin, cout, P, cin, 1, workspace, workspace_bytes, (cudaStream_t)stream, r, rscale);
+}

@@ -91,6 +91,14 @@ _SIGNATURES = {
     'lvg_dblock_tail_adjoint': (_c_int, [_c_void_p] * 7 + [_c_i64] + [_c_int] * 8 + [_c_float] * 2 + [_c_void_p]),
     'lvg_sres_cond_workspace': (_c_i64, [_c_int] * 9 + [_c_void_p] * 2),
     'lvg_sres_cond': (_c_int, [_c_void_p] * 7 + [_c_i64] + [_c_int] * 10 + [_c_void_p] * 3 + [_c_float] * 2 + [_c_void_p]),
+    'lvg_sres_dblock_conv1_workspace': (_c_i64, [_c_int] * 6),
+    'lvg_sres_dblock_conv1': (_c_int, [_c_void_p] * 3 + [_c_int] + [_c_void_p] * 3 + [_c_int] * 7 + [_c_float] * 3 + [_c_void_p, _c_i64, _c_void_p]),
+    'lvg_sres_dblock_conv1_backward_workspace': (_c_i64, [_c_int] * 6),
+    'lvg_sres_dblock_conv1_backward': (_c_int, [_c_void_p] * 3 + [_c_int] + [_c_void_p] * 4 + [_c_int] * 6 + [_c_void_p, _c_i64, _c_void_p]),
+    'lvg_sres_dblock_fir_adjoint_act_workspace': (_c_i64, [_c_int] * 5),
+    'lvg_sres_dblock_fir_adjoint_act': (_c_int, [_c_void_p] * 4 + [_c_int] + [_c_void_p] * 3 + [_c_i64] + [_c_int] * 6 + [_c_float] * 3 + [_c_void_p]),
+    'lvg_sres_dblock_skip_workspace': (_c_i64, [_c_int] * 4 + [_c_i64]),
+    'lvg_sres_dblock_skip': (_c_int, [_c_void_p] * 4 + [_c_int] * 4 + [_c_i64, _c_float, _c_void_p, _c_i64, _c_void_p]),
 }
 
 LVG_UNSUPPORTED = -1
@@ -1032,8 +1040,109 @@ class SresCondPlugin:
                 raise RuntimeError('sres_cond: ' + self._lib.lvg_last_error().decode())
         return z, ms
 
+class SresDblockPlugin:
+    """The two native layers of a super-res discriminator block (DESIGN.md 7i): ``conv1`` (the 4-tap FIR in the
+    convolution's re-tiling pass, the stride-2 3x3 convolution with its bias_act epilogue) and ``skip`` (the 1x1 convolution
+    of the down-sampled input with the residual merge in its epilogue)."""
+
+    def __init__(self, lib):
+        self._lib = lib
+        self._ws = {}
+
+    def _workspace(self, device, need):
+        buf = self._ws.get(device)
+        if buf is None or buf.numel() < need:
+            buf = torch.empty(max(int(need), 1 << 22), dtype=torch.uint8, device=device)
+            self._ws[device] = buf      # stream-ordered reuse: every call re-tiles its operands before it reads them
+        return buf
+
+    def conv1_workspace(self, dtype, n, cin, cout, h, w):
+        return int(self._lib.lvg_sres_dblock_conv1_workspace(_DTYPE_CODE.get(dtype, -1), n, cin, cout, h, w))
+
+    def skip_workspace(self, dtype, n, cin, cout, p):
+        return int(self._lib.lvg_sres_dblock_skip_workspace(_DTYPE_CODE.get(dtype, -1), n, cin, cout, p))
+
+    def conv1(self, x, fx, fy, flip, w, b, act, alpha, gain, clamp):
+        """bias_act(conv2d(upfirdn2d(x, outer(fy, fx), padding=2, flip_filter=flip), w, stride=2), b, ...): act 1 linear, 2 lrelu."""
+        x, w = x.contiguous(), w.contiguous()
+        n, cin, h, wd = x.shape
+        cout = w.shape[0]
+        need = self.conv1_workspace(x.dtype, n, cin, cout, h, wd)
+        if need < 0:
+            raise RuntimeError('sres_dblock_conv1: outside the kernels\' envelope')
+        y = torch.empty([n, cout, (h - 2) // 2 + 1, (wd - 2) // 2 + 1], dtype=x.dtype, device=x.device)
+        ws = self._workspace(x.device, need)
+        if b is not None:
+            b = b.to(torch.float32).contiguous()
+        with _DeviceGuard(x):
+            rc = _check(self._lib.lvg_sres_dblock_conv1(_ptr(x), _ptr(fx), _ptr(fy), int(bool(flip)), _ptr(w), _ptr(b), _ptr(y), _DTYPE_CODE[x.dtype],
+                                                   n, cin, cout, h, wd, int(act), float(alpha), float(gain), float(clamp), _ptr(ws), ws.numel(),
+                                                   _stream(x)), 'sres_dblock_conv1')
+        if rc == LVG_UNSUPPORTED:
+            raise RuntimeError('sres_dblock_conv1: ' + self._lib.lvg_last_error().decode())
+        return y
+
+    def conv1_backward(self, x, fx, fy, flip, dy, w, want_dx=True, want_dw=True):
+        """(d filtered image, dw) of conv1 from dy, the gradient of its pre-activation; dw's x operand is re-tiled from x
+        through the FIR (the filtered image is not stored)."""
+        x, dy, w = x.contiguous(), dy.contiguous(), w.contiguous()
+        n, cin, h, wd = x.shape
+        cout = w.shape[0]
+        need = int(self._lib.lvg_sres_dblock_conv1_backward_workspace(_DTYPE_CODE.get(x.dtype, -1), n, cin, cout, h, wd))
+        if need < 0:
+            raise RuntimeError('sres_dblock_conv1_backward: outside the kernels\' envelope')
+        dhf = torch.empty([n, cin, h + 1, wd + 1], dtype=x.dtype, device=x.device) if want_dx else None
+        dw = torch.empty_like(w) if want_dw else None
+        ws = self._workspace(x.device, need)
+        with _DeviceGuard(x):
+            rc = _check(self._lib.lvg_sres_dblock_conv1_backward(_ptr(x), _ptr(fx), _ptr(fy), int(bool(flip)), _ptr(dy), _ptr(w), _ptr(dhf), _ptr(dw),
+                                                            _DTYPE_CODE[x.dtype], n, cin, cout, h, wd, _ptr(ws), ws.numel(), _stream(x)),
+                        'sres_dblock_conv1_backward')
+        if rc == LVG_UNSUPPORTED:
+            raise RuntimeError('sres_dblock_conv1_backward: ' + self._lib.lvg_last_error().decode())
+        return dhf, dw
+
+    def fir_adjoint_act_workspace(self, dtype, n, c, h, w):
+        return int(self._lib.lvg_sres_dblock_fir_adjoint_act_workspace(_DTYPE_CODE.get(dtype, -1), n, c, h, w))
+
+    def fir_adjoint_act(self, dhf, h0, fx, fy, flip, act, alpha, gain, clamp, want_db=True):
+        """(G(h0) * FIR^T(dhf), fp32 db or None): act 1 linear, 2 lrelu; db from per-CTA partials folded in a fixed order."""
+        dhf, h0 = dhf.contiguous(), h0.contiguous()
+        n, c, h, w = h0.shape
+        need = self.fir_adjoint_act_workspace(h0.dtype, n, c, h, w)
+        if need < 0:
+            raise RuntimeError('sres_dblock_fir_adjoint_act: outside the kernel\'s envelope')
+        dz = torch.empty_like(h0)
+        db = torch.empty([c], dtype=torch.float32, device=h0.device) if want_db else None
+        ws = torch.empty([need], dtype=torch.uint8, device=h0.device)
+        with _DeviceGuard(h0):
+            rc = _check(self._lib.lvg_sres_dblock_fir_adjoint_act(_ptr(dhf), _ptr(h0), _ptr(fx), _ptr(fy), int(bool(flip)), _ptr(dz), _ptr(db),
+                                                             _ptr(ws), ws.numel(), _DTYPE_CODE[h0.dtype], n, c, h, w, int(act), float(alpha),
+                                                             float(gain), float(clamp), _stream(h0)), 'sres_dblock_fir_adjoint_act')
+        if rc == LVG_UNSUPPORTED:
+            raise RuntimeError('sres_dblock_fir_adjoint_act: ' + self._lib.lvg_last_error().decode())
+        return dz, db
+
+    def skip(self, x, w, r, rscale):
+        """(conv2d(x, w) + r) * rscale for a 1x1 weight w [cout, cin, 1, 1]; r has the output's shape and x's dtype."""
+        x, w, r = x.contiguous(), w.contiguous(), r.contiguous()
+        n, cin, h, wd = x.shape
+        cout = w.shape[0]
+        need = self.skip_workspace(x.dtype, n, cin, cout, h * wd)
+        if need < 0:
+            raise RuntimeError('sres_dblock_skip: outside the kernel\'s envelope')
+        y = torch.empty([n, cout, h, wd], dtype=x.dtype, device=x.device)
+        ws = self._workspace(x.device, need)
+        with _DeviceGuard(x):
+            rc = _check(self._lib.lvg_sres_dblock_skip(_ptr(x), _ptr(w), _ptr(r), _ptr(y), _DTYPE_CODE[x.dtype], n, cin, cout, h * wd, float(rscale),
+                                                  _ptr(ws), ws.numel(), _stream(x)), 'sres_dblock_skip')
+        if rc == LVG_UNSUPPORTED:
+            raise RuntimeError('sres_dblock_skip: ' + self._lib.lvg_last_error().decode())
+        return y
+
 
 _PLUGIN_CLASSES = {
+    'sres_dblock_plugin': SresDblockPlugin,
     'sres_cond_plugin': SresCondPlugin,
     'dblock_tail_plugin': DblockTailPlugin,
     'gblock_tail_plugin': GblockTailPlugin,
