@@ -22,6 +22,8 @@ import os
 
 import torch
 
+from .ops._util import is_absent, is_dense
+
 verbosity = 'brief'  # kept for API compatibility ('none' | 'brief' | 'full')
 
 _LIB_NAME = 'liblvg_ops.so'
@@ -138,12 +140,6 @@ def launch_count():
     return int(load_library().lvg_launch_count())
 
 
-def _check(rc, what):
-    if rc > 0:
-        raise RuntimeError(f'{what}: {_lib.lvg_last_error().decode()}')
-    return rc
-
-
 def _ptr(t):
     """Device pointer of a tensor, or NULL for None / empty ("absent" in the reference API)."""
     if t is None or t.numel() == 0:
@@ -172,24 +168,8 @@ def _dtype_code(t, what):
         raise RuntimeError(f'{what}: unsupported dtype {t.dtype}') from None
 
 
-def _absent(t):
-    return t is None or t.numel() == 0
-
-
 def _same_layout(a, b):
     return a.shape == b.shape and a.stride() == b.stride()
-
-
-def _is_dense(x):
-    if x.is_contiguous():
-        return True
-    dims = sorted((d for d in range(x.ndim) if x.shape[d] != 1), key=lambda d: x.stride(d))
-    expect = 1
-    for d in dims:
-        if x.stride(d) != expect:
-            return False
-        expect *= x.shape[d]
-    return True
 
 
 class _DeviceGuard:
@@ -210,6 +190,34 @@ class _DeviceGuard:
             torch.cuda.set_device(self.prev)
 
 
+def _launch(what, fn, anchor, *args, optional=False):
+    """fn(*args, stream) on anchor's device and current stream. Returns True once launched. LVG_UNSUPPORTED (no kernel for
+    the configuration) returns False when ``optional``, so the caller can compose other ops; it raises otherwise, as every
+    error code does."""
+    with _DeviceGuard(anchor):
+        rc = fn(*args, _stream(anchor))
+    if rc == LVG_UNSUPPORTED and optional:
+        return False
+    if rc != 0:
+        raise RuntimeError(f'{what}: {_lib.lvg_last_error().decode()}')
+    return True
+
+
+_ws = {}
+
+
+def _workspace(device, need):
+    """The convolution engine's workspace on ``device``: one buffer of at least ``need`` bytes (and 4 MiB), grown on
+    demand and shared by every ConvNdPlugin and SresDblockPlugin call."""
+    if need < 0:
+        raise RuntimeError('convnd: configuration outside the tensor-core kernel envelope')
+    buf = _ws.get(device)
+    if buf is None or buf.numel() < need:
+        buf = torch.empty(max(int(need), 1 << 22), dtype=torch.uint8, device=device)
+        _ws[device] = buf      # stream-ordered reuse: every call re-tiles its operands before it reads them
+    return buf
+
+
 # ----------------------------------------------------------------------------
 
 class BiasActPlugin:
@@ -223,12 +231,12 @@ class BiasActPlugin:
             raise RuntimeError('x must reside on CUDA device')
         code = _dtype_code(x, 'bias_act')
         for name, t in (('xref', xref), ('yref', yref), ('dy', dy)):
-            if not _absent(t) and not (t.dtype == x.dtype and t.device == x.device and _same_layout(t, x)):
+            if not is_absent(t) and not (t.dtype == x.dtype and t.device == x.device and _same_layout(t, x)):
                 raise RuntimeError(f'{name} must have the same shape, dtype, device and layout as x')
         if grad < 0:
             raise RuntimeError('grad must be non-negative')
         size_b, step_b = 1, 1
-        if not _absent(b):
+        if not is_absent(b):
             if b.dtype != x.dtype or b.device != x.device:
                 raise RuntimeError('b must have the same dtype and device as x')
             if b.ndim != 1:
@@ -240,15 +248,13 @@ class BiasActPlugin:
             if not b.is_contiguous():
                 raise RuntimeError('b must be contiguous')
             size_b, step_b = b.numel(), x.stride(dim)
-        if not _is_dense(x):
+        if not is_dense(x):
             raise RuntimeError('x must be non-overlapping and dense')
         y = torch.empty_like(x)
         if not _same_layout(y, x):
             raise RuntimeError('y must have the same layout as x')
-        with _DeviceGuard(x):
-            _check(self._lib.lvg_bias_act(_ptr(x), _ptr(b), _ptr(xref), _ptr(yref), _ptr(dy), _ptr(y), code,
-                                          x.numel(), size_b, max(step_b, 1), int(grad), int(act),
-                                          float(alpha), float(gain), float(clamp), _stream(x)), 'bias_act')
+        _launch('bias_act', self._lib.lvg_bias_act, x, _ptr(x), _ptr(b), _ptr(xref), _ptr(yref), _ptr(dy), _ptr(y), code,
+                x.numel(), size_b, max(step_b, 1), int(grad), int(act), float(alpha), float(gain), float(clamp))
         return y
 
     def bias_act_grad_db(self, dy, b, xref, yref, dim, act, alpha, gain, clamp):
@@ -257,19 +263,16 @@ class BiasActPlugin:
         if not dy.is_cuda:
             raise RuntimeError('dy must reside on CUDA device')
         code = _dtype_code(dy, 'bias_act_grad_db')
-        if not _is_dense(dy):
+        if not is_dense(dy):
             raise RuntimeError('dy must be non-overlapping and dense')
         for name, t in (('xref', xref), ('yref', yref)):
-            if not _absent(t) and not (t.dtype == dy.dtype and _same_layout(t, dy)):
+            if not is_absent(t) and not (t.dtype == dy.dtype and _same_layout(t, dy)):
                 raise RuntimeError(f'{name} must have the same shape, dtype and layout as dy')
         size_b, step_b = dy.shape[dim], max(dy.stride(dim), 1)
         dx = torch.empty_like(dy)
         db = torch.zeros([size_b], dtype=torch.float32, device=dy.device)
-        with _DeviceGuard(dy):
-            rc = _check(self._lib.lvg_bias_act_grad_db(_ptr(dy), _ptr(b), _ptr(xref), _ptr(yref), _ptr(dx), _ptr(db), code,
-                                                       dy.numel(), size_b, step_b, int(act), float(alpha), float(gain),
-                                                       float(clamp), _stream(dy)), 'bias_act_grad_db')
-        if rc == LVG_UNSUPPORTED:
+        if not _launch('bias_act_grad_db', self._lib.lvg_bias_act_grad_db, dy, _ptr(dy), _ptr(b), _ptr(xref), _ptr(yref), _ptr(dx),
+                       _ptr(db), code, dy.numel(), size_b, step_b, int(act), float(alpha), float(gain), float(clamp), optional=True):
             return None     # layout not covered by the fused kernel: caller runs bias_act(grad=1) + sum
         return dx, db.to(dy.dtype)
 
@@ -277,10 +280,10 @@ class BiasActPlugin:
     def bias_act_fwd_codes(self, x, b, dim, act, alpha, gain, clamp):
         """relu / lrelu forward that also emits 2-bit sign / clamp codes (uint8 [numel / 4]) for the backward pass.
         Returns (y, codes), or None when the kernel does not cover the call (other activations, odd sizes, fp64)."""
-        if not x.is_cuda or x.dtype not in (torch.float16, torch.float32) or x.numel() == 0 or not _is_dense(x):
+        if not x.is_cuda or x.dtype not in (torch.float16, torch.float32) or x.numel() == 0 or not is_dense(x):
             return None
         size_b, step_b = 1, 1
-        if not _absent(b):
+        if not is_absent(b):
             if b.dtype != x.dtype or b.device != x.device or b.ndim != 1 or b.numel() != x.shape[dim] or not b.is_contiguous():
                 return None         # let the general entry point produce the reference's error message
             size_b, step_b = b.numel(), max(x.stride(dim), 1)
@@ -289,11 +292,11 @@ class BiasActPlugin:
         if nbytes < 0:
             return None
         codes = torch.empty([int(nbytes)], dtype=torch.uint8, device=x.device)
-        with _DeviceGuard(x):
-            rc = _check(self._lib.lvg_bias_act_fwd_codes(_ptr(x), _ptr(b), _ptr(y), _ptr(codes), _dtype_code(x, 'bias_act'),
-                                                         x.numel(), size_b, step_b, int(act), float(alpha), float(gain),
-                                                         float(clamp), _stream(x)), 'bias_act_fwd_codes')
-        return None if rc == LVG_UNSUPPORTED else (y, codes)
+        if not _launch('bias_act_fwd_codes', self._lib.lvg_bias_act_fwd_codes, x, _ptr(x), _ptr(b), _ptr(y), _ptr(codes),
+                       _dtype_code(x, 'bias_act'), x.numel(), size_b, step_b, int(act), float(alpha), float(gain), float(clamp),
+                       optional=True):
+            return None
+        return y, codes
 
     def bias_act_bwd_codes(self, dy, codes, dim, act, alpha, gain, clamp, want_db):
         """dx (and the bias gradient when want_db and the layout allows fusing it) from dy and the forward's codes.
@@ -303,12 +306,8 @@ class BiasActPlugin:
         size_b, step_b = dy.shape[dim], max(dy.stride(dim), 1)
         pack = 8 if dy.dtype == torch.float16 else 4
         db = torch.zeros([size_b], dtype=torch.float32, device=dy.device) if (want_db and step_b % pack == 0) else None
-        with _DeviceGuard(dy):
-            rc = _check(self._lib.lvg_bias_act_bwd_codes(_ptr(dy), _ptr(codes), _ptr(dx), _ptr(db), code, dy.numel(), size_b, step_b,
-                                                         int(act), float(alpha), float(gain), float(clamp), _stream(dy)),
-                        'bias_act_bwd_codes')
-        if rc == LVG_UNSUPPORTED:
-            raise RuntimeError('bias_act_bwd_codes: ' + self._lib.lvg_last_error().decode())
+        _launch('bias_act_bwd_codes', self._lib.lvg_bias_act_bwd_codes, dy, _ptr(dy), _ptr(codes), _ptr(dx), _ptr(db), code,
+                dy.numel(), size_b, step_b, int(act), float(alpha), float(gain), float(clamp))
         return dx, (db.to(dy.dtype) if db is not None else None)
 
 
@@ -358,10 +357,8 @@ class Upfirdn2dPlugin:
         fh, fw = f.shape
         oh, ow = self._out_size(x, fw, fh, upx, upy, downx, downy, padx0, padx1, pady0, pady1)
         y = self._alloc_like(x, oh, ow)
-        with _DeviceGuard(x):
-            _check(self._lib.lvg_upfirdn2d(_ptr(x), _ptr(f), _ptr(y), code, _i4(x.shape), _i4(x.stride()), _i4(y.shape),
-                                           _i4(y.stride()), fw, fh, f.stride(1), f.stride(0), upx, upy, downx, downy,
-                                           padx0, pady0, int(bool(flip)), float(gain), _stream(x)), 'upfirdn2d')
+        _launch('upfirdn2d', self._lib.lvg_upfirdn2d, x, _ptr(x), _ptr(f), _ptr(y), code, _i4(x.shape), _i4(x.stride()), _i4(y.shape),
+                _i4(y.stride()), fw, fh, f.stride(1), f.stride(0), upx, upy, downx, downy, padx0, pady0, int(bool(flip)), float(gain))
         return y
 
     def upfirdn2d_sep(self, x, fx, fy, upx, upy, downx, downy, padx0, padx1, pady0, pady1, flip, gain):
@@ -377,11 +374,11 @@ class Upfirdn2dPlugin:
         fh = fy.numel() if fy is not None else 1
         oh, ow = self._out_size(x, fw, fh, upx, upy, downx, downy, padx0, padx1, pady0, pady1)
         y = self._alloc_like(x, oh, ow)
-        with _DeviceGuard(x):
-            rc = _check(self._lib.lvg_upfirdn2d_sep(_ptr(x), _ptr(fx), _ptr(fy), _ptr(y), code, _i4(x.shape), _i4(x.stride()),
-                                                    _i4(y.shape), _i4(y.stride()), fw, fh, upx, upy, downx, downy,
-                                                    padx0, pady0, int(bool(flip)), float(gain), _stream(x)), 'upfirdn2d_sep')
-        return None if rc == LVG_UNSUPPORTED else y
+        if not _launch('upfirdn2d_sep', self._lib.lvg_upfirdn2d_sep, x, _ptr(x), _ptr(fx), _ptr(fy), _ptr(y), code, _i4(x.shape),
+                       _i4(x.stride()), _i4(y.shape), _i4(y.stride()), fw, fh, upx, upy, downx, downy, padx0, pady0, int(bool(flip)),
+                       float(gain), optional=True):
+            return None
+        return y
 
 
 class FilteredLReluPlugin:
@@ -434,7 +431,7 @@ class FilteredLReluPlugin:
         y = torch.empty([x.shape[0], x.shape[1], yh, yw], dtype=x.dtype, device=x.device, memory_format=fmt)
 
         so = None
-        s = si if not _absent(si) else None
+        s = si if not is_absent(si) else None
         read_signs = s is not None
         if writeSigns:
             if read_signs:
@@ -455,13 +452,11 @@ class FilteredLReluPlugin:
             s = padded
         s_h, s_wb = (s.shape[2], s.shape[3]) if s is not None else (0, 0)
         fu_c, fd_c, b_c = fu.contiguous(), fd.contiguous(), b.contiguous()
-        with _DeviceGuard(x):
-            rc = _check(self._lib.lvg_filtered_lrelu(
-                _ptr(x), _ptr(fu_c), _ptr(fd_c), _ptr(b_c), _ptr(s) if read_signs else None, _ptr(y),
-                _ptr(so) if writeSigns else None, code, _i4(x.shape), _i4(x.stride()), _i4(y.shape), _i4(y.stride()),
-                fu_w, fu_h, fd_w, fd_h, up, down, px0, py0, s_h, s_wb, sx, sy, float(gain), float(slope),
-                float(clamp), int(bool(flip_filters)), int(bool(writeSigns)), _stream(x)), 'filtered_lrelu')
-        if rc == LVG_UNSUPPORTED:
+        if not _launch('filtered_lrelu', self._lib.lvg_filtered_lrelu, x,
+                       _ptr(x), _ptr(fu_c), _ptr(fd_c), _ptr(b_c), _ptr(s) if read_signs else None, _ptr(y),
+                       _ptr(so) if writeSigns else None, code, _i4(x.shape), _i4(x.stride()), _i4(y.shape), _i4(y.stride()),
+                       fu_w, fu_h, fd_w, fd_h, up, down, px0, py0, s_h, s_wb, sx, sy, float(gain), float(slope),
+                       float(clamp), int(bool(flip_filters)), int(bool(writeSigns)), optional=True):
             return None, None, -1
         return y, so, 0
 
@@ -474,7 +469,7 @@ class FilteredLReluPlugin:
             raise RuntimeError('x is empty')
         code = _dtype_code(x, 'filtered_lrelu_act_')
         so = None
-        s = si if not _absent(si) else None
+        s = si if not is_absent(si) else None
         read_signs = s is not None
         if writeSigns:
             sw = (x.shape[3] + 15) & ~15
@@ -484,11 +479,9 @@ class FilteredLReluPlugin:
                     and s.shape[0] == x.shape[0] and s.shape[1] == x.shape[1]):
                 raise RuntimeError('signs must be a contiguous uint8 [N, C, H, W/4] tensor on the same device as x')
         s_h, s_wb = (s.shape[2], s.shape[3]) if s is not None else (0, 0)
-        with _DeviceGuard(x):
-            _check(self._lib.lvg_filtered_lrelu_act(_ptr(x), _ptr(s) if (read_signs and not writeSigns) else None,
-                                                    _ptr(so) if writeSigns else None, code, _i4(x.shape), _i4(x.stride()),
-                                                    s_h, s_wb, sx, sy, float(gain), float(slope), float(clamp),
-                                                    int(bool(writeSigns)), _stream(x)), 'filtered_lrelu_act_')
+        _launch('filtered_lrelu_act_', self._lib.lvg_filtered_lrelu_act, x, _ptr(x), _ptr(s) if (read_signs and not writeSigns) else None,
+                _ptr(so) if writeSigns else None, code, _i4(x.shape), _i4(x.stride()), s_h, s_wb, sx, sy, float(gain), float(slope),
+                float(clamp), int(bool(writeSigns)))
         return so
 
 
@@ -512,11 +505,9 @@ class FmaPlugin:
             return out
         ae, be, ce = a.expand(shape), b.expand(shape), c.expand(shape)
         pad = [0] * (6 - len(shape))
-        with _DeviceGuard(out):
-            _check(self._lib.lvg_fma(_ptr(ae), _ptr(be), _ptr(ce), _ptr(out), code, len(shape),
-                                     _I64x6(*(list(shape) + [1] * len(pad))), _I64x6(*(list(ae.stride()) + pad)),
-                                     _I64x6(*(list(be.stride()) + pad)), _I64x6(*(list(ce.stride()) + pad)),
-                                     _stream(out)), 'fma')
+        _launch('fma', self._lib.lvg_fma, out, _ptr(ae), _ptr(be), _ptr(ce), _ptr(out), code, len(shape),
+                _I64x6(*(list(shape) + [1] * len(pad))), _I64x6(*(list(ae.stride()) + pad)),
+                _I64x6(*(list(be.stride()) + pad)), _I64x6(*(list(ce.stride()) + pad)))
         return out
 
 
@@ -527,7 +518,6 @@ class ConvNdPlugin:
 
     def __init__(self, lib):
         self._lib = lib
-        self._ws = {}
 
     @staticmethod
     def _pad3(padding, nd):
@@ -561,15 +551,6 @@ class ConvNdPlugin:
         out = [s + 2 * p - kk + 1 for s, p, kk in zip(sp, pad, k)]
         return min(out) >= 1 and out[2] <= 4 * (128 - k[2] + 1)
 
-    def _workspace(self, device, need):
-        if need < 0:
-            raise RuntimeError('convnd: configuration outside the tensor-core kernel envelope')
-        buf = self._ws.get(device)
-        if buf is None or buf.numel() < need:
-            buf = torch.empty(max(int(need), 1 << 22), dtype=torch.uint8, device=device)
-            self._ws[device] = buf      # stream-ordered reuse: every call re-tiles its operands before it reads them
-        return buf
-
     def _args(self, x_shape, w_shape, padding, groups, dtype):
         nd = len(x_shape) - 2
         sp = [1] * (3 - nd) + list(x_shape[2:])
@@ -593,25 +574,19 @@ class ConvNdPlugin:
         st3 = [1, stride, stride] if x.ndim >= 4 else [1, 1, 1]
         out_sp = [(s + 2 * p - kk) // q + 1 for s, p, kk, q in zip(sp, pad, k, st3)][3 - (x.ndim - 2):]
         y = torch.empty([x.shape[0], w.shape[0]] + out_sp, dtype=x.dtype, device=x.device)
-        ws = self._workspace(x.device, self._lib.lvg_convnd_workspace(*a))
+        ws = _workspace(x.device, self._lib.lvg_convnd_workspace(*a))
         if bias is not None:
             bias = bias.to(torch.float32).contiguous()
-        with _DeviceGuard(x):
-            rc = _check(self._lib.lvg_convnd_fprop(_ptr(x), _ptr(w), _ptr(y), *a, int(stride), _ptr(bias), int(act), float(alpha), float(gain),
-                                                   float(clamp), _ptr(ws), ws.numel(), _stream(x)), 'convnd_fprop')
-        if rc == LVG_UNSUPPORTED:
-            raise RuntimeError('convnd_fprop: ' + self._lib.lvg_last_error().decode())
+        _launch('convnd_fprop', self._lib.lvg_convnd_fprop, x, _ptr(x), _ptr(w), _ptr(y), *a, int(stride), _ptr(bias), int(act), float(alpha),
+                float(gain), float(clamp), _ptr(ws), ws.numel())
         return y
 
     def dgrad(self, dy, w, x_shape, padding, groups, stride=1):
         dy, w = dy.contiguous(), w.contiguous()
         a, sp, k, pad = self._args(tuple(x_shape), tuple(w.shape), padding, groups, dy.dtype)
         dx = torch.empty(list(x_shape), dtype=dy.dtype, device=dy.device)
-        ws = self._workspace(dy.device, self._lib.lvg_convnd_workspace(*a))
-        with _DeviceGuard(dy):
-            rc = _check(self._lib.lvg_convnd_dgrad(_ptr(dy), _ptr(w), _ptr(dx), *a, int(stride), _ptr(ws), ws.numel(), _stream(dy)), 'convnd_dgrad')
-        if rc == LVG_UNSUPPORTED:
-            raise RuntimeError('convnd_dgrad: ' + self._lib.lvg_last_error().decode())
+        ws = _workspace(dy.device, self._lib.lvg_convnd_workspace(*a))
+        _launch('convnd_dgrad', self._lib.lvg_convnd_dgrad, dy, _ptr(dy), _ptr(w), _ptr(dx), *a, int(stride), _ptr(ws), ws.numel())
         return dx
 
     def fir1d_depthwise(self, x, w):
@@ -621,19 +596,15 @@ class ConvNdPlugin:
         k = w.shape[2]
         y = torch.empty([n, g, lin - k + 1], dtype=x.dtype, device=x.device)
         ws = torch.empty([g + 4], dtype=torch.int32, device=x.device)
-        with _DeviceGuard(x):
-            _check(self._lib.lvg_fir1d_depthwise(_ptr(x), _ptr(w), _ptr(y), n, g, lin, k, _ptr(ws), ws.numel() * 4, _stream(x)), 'fir1d_depthwise')
+        _launch('fir1d_depthwise', self._lib.lvg_fir1d_depthwise, x, _ptr(x), _ptr(w), _ptr(y), n, g, lin, k, _ptr(ws), ws.numel() * 4)
         return y
 
     def wgrad(self, x, dy, w_shape, padding, groups, stride=1):
         x, dy = x.contiguous(), dy.contiguous()
         a, sp, k, pad = self._args(tuple(x.shape), tuple(w_shape), padding, groups, x.dtype)
         dw = torch.empty(list(w_shape), dtype=x.dtype, device=x.device)
-        ws = self._workspace(x.device, self._lib.lvg_convnd_wgrad_workspace(*a))
-        with _DeviceGuard(x):
-            rc = _check(self._lib.lvg_convnd_wgrad(_ptr(x), _ptr(dy), _ptr(dw), *a, int(stride), _ptr(ws), ws.numel(), _stream(x)), 'convnd_wgrad')
-        if rc == LVG_UNSUPPORTED:
-            raise RuntimeError('convnd_wgrad: ' + self._lib.lvg_last_error().decode())
+        ws = _workspace(x.device, self._lib.lvg_convnd_wgrad_workspace(*a))
+        _launch('convnd_wgrad', self._lib.lvg_convnd_wgrad, x, _ptr(x), _ptr(dy), _ptr(dw), *a, int(stride), _ptr(ws), ws.numel())
         return dw
 
     def backward(self, x, dy, w, padding, groups, stride=1):
@@ -642,12 +613,9 @@ class ConvNdPlugin:
         a, sp, k, pad = self._args(tuple(x.shape), tuple(w.shape), padding, groups, x.dtype)
         dx = torch.empty_like(x)
         dw = torch.empty_like(w)
-        ws = self._workspace(x.device, self._lib.lvg_convnd_backward_workspace(*a))
-        with _DeviceGuard(x):
-            rc = _check(self._lib.lvg_convnd_backward(_ptr(x), _ptr(dy), _ptr(w), _ptr(dx), _ptr(dw), *a, int(stride), _ptr(ws), ws.numel(),
-                                                      _stream(x)), 'convnd_backward')
-        if rc == LVG_UNSUPPORTED:
-            raise RuntimeError('convnd_backward: ' + self._lib.lvg_last_error().decode())
+        ws = _workspace(x.device, self._lib.lvg_convnd_backward_workspace(*a))
+        _launch('convnd_backward', self._lib.lvg_convnd_backward, x, _ptr(x), _ptr(dy), _ptr(w), _ptr(dx), _ptr(dw), *a, int(stride), _ptr(ws),
+                ws.numel())
         return dx, dw
 
     def _modconv_args(self, x, w, padding):
@@ -675,12 +643,8 @@ class ConvNdPlugin:
         if d is not None:
             d = self._factor(d, (x.shape[0], w.shape[0], out_sp[0]), 'modconv_fprop: d')
         y = torch.empty([x.shape[0], w.shape[0]] + out_sp[3 - (x.ndim - 2):], dtype=x.dtype, device=x.device)
-        ws = self._workspace(x.device, self._lib.lvg_modconv_workspace(*args))
-        with _DeviceGuard(x):
-            rc = _check(self._lib.lvg_modconv_fprop(_ptr(x), _ptr(w), _ptr(a), _ptr(d), _ptr(y), *args, _ptr(ws), ws.numel(), _stream(x)),
-                        'modconv_fprop')
-        if rc == LVG_UNSUPPORTED:
-            raise RuntimeError('modconv_fprop: ' + self._lib.lvg_last_error().decode())
+        ws = _workspace(x.device, self._lib.lvg_modconv_workspace(*args))
+        _launch('modconv_fprop', self._lib.lvg_modconv_fprop, x, _ptr(x), _ptr(w), _ptr(a), _ptr(d), _ptr(y), *args, _ptr(ws), ws.numel())
         return y
 
     def modconv_backward(self, x, w, a, d, y, dy, padding, want_dw=True):
@@ -697,12 +661,9 @@ class ConvNdPlugin:
             d = self._factor(d, (x.shape[0], w.shape[0], dy.shape[2] if dy.ndim == 5 else 1), 'modconv_backward: d')
             y = y.contiguous()
             dyy = torch.empty(d.shape, dtype=torch.float32, device=x.device)
-        ws = self._workspace(x.device, self._lib.lvg_modconv_workspace(*args))
-        with _DeviceGuard(x):
-            rc = _check(self._lib.lvg_modconv_backward(_ptr(x), _ptr(w), _ptr(a), _ptr(d), _ptr(y) if d is not None else None, _ptr(dy), _ptr(dx),
-                                                       _ptr(dw), _ptr(da), _ptr(dyy), *args, _ptr(ws), ws.numel(), _stream(x)), 'modconv_backward')
-        if rc == LVG_UNSUPPORTED:
-            raise RuntimeError('modconv_backward: ' + self._lib.lvg_last_error().decode())
+        ws = _workspace(x.device, self._lib.lvg_modconv_workspace(*args))
+        _launch('modconv_backward', self._lib.lvg_modconv_backward, x, _ptr(x), _ptr(w), _ptr(a), _ptr(d), _ptr(y) if d is not None else None,
+                _ptr(dy), _ptr(dx), _ptr(dw), _ptr(da), _ptr(dyy), *args, _ptr(ws), ws.numel())
         return dx, dw, da, dyy
 
 
@@ -732,9 +693,8 @@ class Fir3dPlugin:
             raise RuntimeError(f'fir3d: x has shape {list(x.shape)}, expected {want}')
         y = torch.empty([n, c * (2 if fold_dst else 1), dst[0] // (2 if fold_dst else 1), dst[1], dst[2]], dtype=x.dtype, device=x.device)
         fn = self._lib.lvg_fir3d_adjoint if adjoint else self._lib.lvg_fir3d
-        with _DeviceGuard(x):
-            _check(fn(_ptr(x), _ptr(f), _ptr(y), code, n, c, *ins, *outs, *[a[0] for a in axes], *[a[1] for a in axes],
-                      *[a[2] for a in axes], int(bool(fold)), _stream(x)), 'fir3d')
+        _launch('fir3d', fn, x, _ptr(x), _ptr(f), _ptr(y), code, n, c, *ins, *outs, *[a[0] for a in axes], *[a[1] for a in axes],
+                *[a[2] for a in axes], int(bool(fold)))
         return y
 
 
@@ -765,14 +725,13 @@ class VideoAugmentPlugin:
         x, params = x.contiguous(), params.contiguous()
         y = torch.empty([n, c, t_other, h, w], dtype=x.dtype, device=x.device)
         ws = torch.empty([nbytes // 4], dtype=torch.float32, device=x.device)
-        with _DeviceGuard(x):
-            if adjoint:
-                rc = self._lib.lvg_video_augment_adjoint(_ptr(x), _ptr(params), _ptr(y), _ptr(ws), n, c, t_in, h, w, t_out, _stream(x))
-            else:
-                rc = self._lib.lvg_video_augment(_ptr(x), _ptr(params), _ptr(y), _ptr(ws), n, c, t_in, h, w, t_out, int(bool(linear)),
-                                                 _stream(x))
-            _check(rc, 'video_augment')
-        return None if rc == LVG_UNSUPPORTED else y
+        if adjoint:
+            ok = _launch('video_augment', self._lib.lvg_video_augment_adjoint, x, _ptr(x), _ptr(params), _ptr(y), _ptr(ws), n, c, t_in, h, w,
+                         t_out, optional=True)
+        else:
+            ok = _launch('video_augment', self._lib.lvg_video_augment, x, _ptr(x), _ptr(params), _ptr(y), _ptr(ws), n, c, t_in, h, w, t_out,
+                         int(bool(linear)), optional=True)
+        return y if ok else None
 
 
 class AugmentPipePlugin:
@@ -804,16 +763,19 @@ class AugmentPipePlugin:
         x, params, f = x.contiguous(), params.contiguous(), f.contiguous()
         noise = None if noise is None else noise.contiguous()
         y = torch.empty_like(x)
-        with _DeviceGuard(x):
-            if adjoint:
-                ws = torch.empty([max(nbytes // 4, 1)], dtype=torch.float32, device=x.device)
-                rc = self._lib.lvg_augment_pipe_adjoint(_ptr(x), _ptr(params), _ptr(f), f.numel(), _ptr(y), _ptr(ws), n, c, t, h, w,
-                                                        int(flags), _stream(x))
-            else:
-                rc = self._lib.lvg_augment_pipe(_ptr(x), _ptr(params), _ptr(f), f.numel(), _ptr(noise), _ptr(y), n, c, t, h, w,
-                                                int(flags), _stream(x))
-            _check(rc, 'augment_pipe')
-        return None if rc == LVG_UNSUPPORTED else y
+        if adjoint:
+            ws = torch.empty([max(nbytes // 4, 1)], dtype=torch.float32, device=x.device)
+            ok = _launch('augment_pipe', self._lib.lvg_augment_pipe_adjoint, x, _ptr(x), _ptr(params), _ptr(f), f.numel(), _ptr(y), _ptr(ws),
+                         n, c, t, h, w, int(flags), optional=True)
+        else:
+            ok = _launch('augment_pipe', self._lib.lvg_augment_pipe, x, _ptr(x), _ptr(params), _ptr(f), f.numel(), _ptr(noise), _ptr(y),
+                         n, c, t, h, w, int(flags), optional=True)
+        return y if ok else None
+
+
+def _check_5d(op, what, x):
+    if not x.is_cuda or x.dtype not in (torch.float16, torch.float32) or x.ndim != 5:
+        raise RuntimeError(f'{op}: {what} must be a 5-D float16 / float32 CUDA tensor')
 
 
 class GblockTailPlugin:
@@ -831,14 +793,9 @@ class GblockTailPlugin:
         """Workspace bytes of the adjoint, or -1 where the kernels do not take the shape."""
         return int(self._lib.lvg_gblock_tail_workspace(n, c, t, h, w, t_out, h_out, w_out, flags))
 
-    @staticmethod
-    def _check(x, what):
-        if not x.is_cuda or x.dtype not in (torch.float16, torch.float32) or x.ndim != 5:
-            raise RuntimeError(f'gblock_tail: {what} must be a 5-D float16 / float32 CUDA tensor')
-
     def forward(self, s, h, b, out_size, flags, act, alpha, gain, clamp, want_codes):
         """(z [N, C, *out_size], codes or None) from s and h [N, C, T, H, W] (one dtype and shape) and b (fp32 [C] or None)."""
-        self._check(s, 's')
+        _check_5d('gblock_tail', 's', s)
         if h.dtype != s.dtype or h.shape != s.shape or h.device != s.device:
             raise RuntimeError('gblock_tail: s and h must have one shape, dtype and device')
         n, c, t, hh, ww = s.shape
@@ -854,16 +811,13 @@ class GblockTailPlugin:
         if want_codes:
             codes = torch.empty([int(self._lib.lvg_bias_act_codes_bytes(_dtype_code(s, 'gblock_tail'), z.numel()))], dtype=torch.uint8,
                                 device=s.device)
-        with _DeviceGuard(s):
-            if _check(self._lib.lvg_gblock_tail(_ptr(s), _ptr(h), _ptr(b), _ptr(z), _ptr(codes), _dtype_code(s, 'gblock_tail'), n, c, t,
-                                             hh, ww, to, ho, wo, int(flags), int(act), float(alpha), float(gain), float(clamp),
-                                             _stream(s)), 'gblock_tail') == LVG_UNSUPPORTED:
-                raise RuntimeError('gblock_tail: ' + self._lib.lvg_last_error().decode())
+        _launch('gblock_tail', self._lib.lvg_gblock_tail, s, _ptr(s), _ptr(h), _ptr(b), _ptr(z), _ptr(codes), _dtype_code(s, 'gblock_tail'),
+                n, c, t, hh, ww, to, ho, wo, int(flags), int(act), float(alpha), float(gain), float(clamp))
         return z, codes
 
     def adjoint(self, dz, codes, in_size, flags, act, alpha, gain):
         """(dm [N, C, *in_size], db fp32 [C]) from dz [N, C, T_out, H_out, W_out] and the forward's codes."""
-        self._check(dz, 'dz')
+        _check_5d('gblock_tail', 'dz', dz)
         n, c, to, ho, wo = dz.shape
         t, hh, ww = (int(v) for v in in_size)
         nbytes = self.workspace(n, c, t, hh, ww, to, ho, wo, flags)
@@ -876,11 +830,8 @@ class GblockTailPlugin:
         dm = torch.empty([n, c, t, hh, ww], dtype=dz.dtype, device=dz.device)
         db = torch.empty([c], dtype=torch.float32, device=dz.device)
         ws = torch.empty([nbytes // 4], dtype=torch.float32, device=dz.device)
-        with _DeviceGuard(dz):
-            if _check(self._lib.lvg_gblock_tail_adjoint(_ptr(dz), _ptr(codes), _ptr(dm), _ptr(db), _ptr(ws), nbytes,
-                                                     _dtype_code(dz, 'gblock_tail'), n, c, t, hh, ww, to, ho, wo, int(flags), int(act),
-                                                     float(alpha), float(gain), _stream(dz)), 'gblock_tail_adjoint') == LVG_UNSUPPORTED:
-                raise RuntimeError('gblock_tail_adjoint: ' + self._lib.lvg_last_error().decode())
+        _launch('gblock_tail_adjoint', self._lib.lvg_gblock_tail_adjoint, dz, _ptr(dz), _ptr(codes), _ptr(dm), _ptr(db), _ptr(ws), nbytes,
+                _dtype_code(dz, 'gblock_tail'), n, c, t, hh, ww, to, ho, wo, int(flags), int(act), float(alpha), float(gain))
         return dm, db
 
 
@@ -909,19 +860,19 @@ class DblockTailPlugin:
         t, h, w = in_size
         return (t // 2 if flags & 1 else t, h // 2 if flags & 2 else h, w // 2 if flags & 2 else w)
 
-    @staticmethod
-    def _check(x, what):
-        if not x.is_cuda or x.dtype not in (torch.float16, torch.float32) or x.ndim != 5:
-            raise RuntimeError(f'dblock_tail: {what} must be a 5-D float16 / float32 CUDA tensor')
-
     def _check_codes(self, codes, ref, need):
         if codes.dtype != torch.uint8 or codes.device != ref.device or codes.numel() != need or not codes.is_contiguous():
             raise RuntimeError(f'dblock_tail: codes must be a contiguous uint8 buffer of {need} bytes on the device of the data')
 
+    def _check_taps(self, op, f, flags, ref, name):
+        if f is None and flags & (self.TDOWN | self.SDOWN) or f is not None and (f.dtype != torch.float32 or f.numel() != 4
+                                                                                  or f.device != ref.device):
+            raise RuntimeError(f'{op}: f must hold 4 float32 taps on the device of {name} (None where no axis is filtered)')
+
     def forward(self, y, s, b, f, flags, act, alpha, gain, clamp, mode, codes=None):
         """(z, codes) from y [N, C, T, H, W], s [N, C, T', H', W'] or None, b ([C], passed as fp32, or None) and the 4 fp32 taps f. WRITE
         returns new codes, READ takes ``codes``, NONE returns None for them."""
-        self._check(y, 'y')
+        _check_5d('dblock_tail', 'y', y)
         n, c, t, h, w = y.shape
         nbytes = self.codes_bytes(n, c, t, h, w, flags)
         if nbytes < 0:
@@ -931,9 +882,7 @@ class DblockTailPlugin:
             raise RuntimeError(f'dblock_tail: s must be a {y.dtype} tensor of shape {out} on the device of y, with MERGE')
         if b is not None and (tuple(b.shape) != (c,) or b.device != y.device):
             raise RuntimeError(f'dblock_tail: b must be a [{c}] tensor on the device of y')
-        if f is None and flags & (self.TDOWN | self.SDOWN) or f is not None and (f.dtype != torch.float32 or f.numel() != 4
-                                                                                  or f.device != y.device):
-            raise RuntimeError('dblock_tail: f must hold 4 float32 taps on the device of y (None where no axis is filtered)')
+        self._check_taps('dblock_tail', f, flags, y, 'y')
         y, f = y.contiguous(), (None if f is None else f.contiguous())
         s = None if s is None else s.contiguous()
         b = None if b is None else b.float().contiguous()
@@ -944,35 +893,27 @@ class DblockTailPlugin:
         else:
             codes = None
         z = torch.empty(out, dtype=y.dtype, device=y.device)
-        with _DeviceGuard(y):
-            if _check(self._lib.lvg_dblock_tail(_ptr(y), _ptr(s), _ptr(b), _ptr(f), _ptr(z), _ptr(codes), int(mode),
-                                             _dtype_code(y, 'dblock_tail'), n, c, t, h, w, int(flags), int(act), float(alpha),
-                                             float(gain), float(clamp), _stream(y)), 'dblock_tail') == LVG_UNSUPPORTED:
-                raise RuntimeError('dblock_tail: ' + self._lib.lvg_last_error().decode())
+        _launch('dblock_tail', self._lib.lvg_dblock_tail, y, _ptr(y), _ptr(s), _ptr(b), _ptr(f), _ptr(z), _ptr(codes), int(mode),
+                _dtype_code(y, 'dblock_tail'), n, c, t, h, w, int(flags), int(act), float(alpha), float(gain), float(clamp))
         return z, codes
 
     def adjoint(self, dz, codes, f, in_size, flags, act, alpha, gain, want_ds):
         """(dy [N, C, *in_size], ds like dz or None, db fp32 [C]) from dz [N, C, T', H', W'] and the forward's codes."""
-        self._check(dz, 'dz')
+        _check_5d('dblock_tail', 'dz', dz)
         n, c = dz.shape[:2]
         t, h, w = (int(v) for v in in_size)
         nbytes = self.workspace(n, c, t, h, w, flags)
         if nbytes < 0 or list(dz.shape[2:]) != list(self.out_size((t, h, w), flags)):
             raise RuntimeError(f'dblock_tail_adjoint: no kernel for {[t, h, w]} -> {list(dz.shape)} (flags {flags})')
         self._check_codes(codes, dz, self.codes_bytes(n, c, t, h, w, flags))
-        if f is None and flags & (self.TDOWN | self.SDOWN) or f is not None and (f.dtype != torch.float32 or f.numel() != 4
-                                                                                  or f.device != dz.device):
-            raise RuntimeError('dblock_tail_adjoint: f must hold 4 float32 taps on the device of dz (None where no axis is filtered)')
+        self._check_taps('dblock_tail_adjoint', f, flags, dz, 'dz')
         dz, f = dz.contiguous(), (None if f is None else f.contiguous())
         dy = torch.empty([n, c, t, h, w], dtype=dz.dtype, device=dz.device)
         ds = torch.empty_like(dz) if want_ds else None
         db = torch.empty([c], dtype=torch.float32, device=dz.device)
         ws = torch.empty([nbytes // 4], dtype=torch.float32, device=dz.device)
-        with _DeviceGuard(dz):
-            if _check(self._lib.lvg_dblock_tail_adjoint(_ptr(dz), _ptr(codes), _ptr(f), _ptr(dy), _ptr(ds), _ptr(db), _ptr(ws), nbytes,
-                                                     _dtype_code(dz, 'dblock_tail'), n, c, t, h, w, int(flags), int(act),
-                                                     float(alpha), float(gain), _stream(dz)), 'dblock_tail_adjoint') == LVG_UNSUPPORTED:
-                raise RuntimeError('dblock_tail_adjoint: ' + self._lib.lvg_last_error().decode())
+        _launch('dblock_tail_adjoint', self._lib.lvg_dblock_tail_adjoint, dz, _ptr(dz), _ptr(codes), _ptr(f), _ptr(dy), _ptr(ds), _ptr(db),
+                _ptr(ws), nbytes, _dtype_code(dz, 'dblock_tail'), n, c, t, h, w, int(flags), int(act), float(alpha), float(gain))
         return dy, ds, db
 
 
@@ -1032,12 +973,9 @@ class SresCondPlugin:
             ms = torch.empty([], dtype=torch.float32, device=lr.device)
             ws = torch.empty([nbytes // 8], dtype=torch.float64, device=lr.device)
         strides = (_c_i64 * 5)(*lr.stride())
-        with _DeviceGuard(lr):
-            if _check(self._lib.lvg_sres_cond(_ptr(x), _ptr(lr), _ptr(f_h), _ptr(f_w), _ptr(z), _ptr(ms), _ptr(ws), nbytes,
-                                              _DTYPE_CODE[x.dtype] if x is not None else _DTYPE_CODE[dtype], _DTYPE_CODE[dtype],
-                                              n, t, c, c_lr, window, t_lr, h_lr, w_lr, strides, ph, pw, float(gain_h),
-                                              float(gain_w), _stream(lr)), 'sres_cond') == LVG_UNSUPPORTED:
-                raise RuntimeError('sres_cond: ' + self._lib.lvg_last_error().decode())
+        _launch('sres_cond', self._lib.lvg_sres_cond, lr, _ptr(x), _ptr(lr), _ptr(f_h), _ptr(f_w), _ptr(z), _ptr(ms), _ptr(ws), nbytes,
+                _DTYPE_CODE[x.dtype] if x is not None else _DTYPE_CODE[dtype], _DTYPE_CODE[dtype], n, t, c, c_lr, window, t_lr, h_lr, w_lr,
+                strides, ph, pw, float(gain_h), float(gain_w))
         return z, ms
 
 class SresDblockPlugin:
@@ -1047,14 +985,6 @@ class SresDblockPlugin:
 
     def __init__(self, lib):
         self._lib = lib
-        self._ws = {}
-
-    def _workspace(self, device, need):
-        buf = self._ws.get(device)
-        if buf is None or buf.numel() < need:
-            buf = torch.empty(max(int(need), 1 << 22), dtype=torch.uint8, device=device)
-            self._ws[device] = buf      # stream-ordered reuse: every call re-tiles its operands before it reads them
-        return buf
 
     def conv1_workspace(self, dtype, n, cin, cout, h, w):
         return int(self._lib.lvg_sres_dblock_conv1_workspace(_DTYPE_CODE.get(dtype, -1), n, cin, cout, h, w))
@@ -1071,15 +1001,11 @@ class SresDblockPlugin:
         if need < 0:
             raise RuntimeError('sres_dblock_conv1: outside the kernels\' envelope')
         y = torch.empty([n, cout, (h - 2) // 2 + 1, (wd - 2) // 2 + 1], dtype=x.dtype, device=x.device)
-        ws = self._workspace(x.device, need)
+        ws = _workspace(x.device, need)
         if b is not None:
             b = b.to(torch.float32).contiguous()
-        with _DeviceGuard(x):
-            rc = _check(self._lib.lvg_sres_dblock_conv1(_ptr(x), _ptr(fx), _ptr(fy), int(bool(flip)), _ptr(w), _ptr(b), _ptr(y), _DTYPE_CODE[x.dtype],
-                                                   n, cin, cout, h, wd, int(act), float(alpha), float(gain), float(clamp), _ptr(ws), ws.numel(),
-                                                   _stream(x)), 'sres_dblock_conv1')
-        if rc == LVG_UNSUPPORTED:
-            raise RuntimeError('sres_dblock_conv1: ' + self._lib.lvg_last_error().decode())
+        _launch('sres_dblock_conv1', self._lib.lvg_sres_dblock_conv1, x, _ptr(x), _ptr(fx), _ptr(fy), int(bool(flip)), _ptr(w), _ptr(b), _ptr(y),
+                _DTYPE_CODE[x.dtype], n, cin, cout, h, wd, int(act), float(alpha), float(gain), float(clamp), _ptr(ws), ws.numel())
         return y
 
     def conv1_backward(self, x, fx, fy, flip, dy, w, want_dx=True, want_dw=True):
@@ -1093,13 +1019,9 @@ class SresDblockPlugin:
             raise RuntimeError('sres_dblock_conv1_backward: outside the kernels\' envelope')
         dhf = torch.empty([n, cin, h + 1, wd + 1], dtype=x.dtype, device=x.device) if want_dx else None
         dw = torch.empty_like(w) if want_dw else None
-        ws = self._workspace(x.device, need)
-        with _DeviceGuard(x):
-            rc = _check(self._lib.lvg_sres_dblock_conv1_backward(_ptr(x), _ptr(fx), _ptr(fy), int(bool(flip)), _ptr(dy), _ptr(w), _ptr(dhf), _ptr(dw),
-                                                            _DTYPE_CODE[x.dtype], n, cin, cout, h, wd, _ptr(ws), ws.numel(), _stream(x)),
-                        'sres_dblock_conv1_backward')
-        if rc == LVG_UNSUPPORTED:
-            raise RuntimeError('sres_dblock_conv1_backward: ' + self._lib.lvg_last_error().decode())
+        ws = _workspace(x.device, need)
+        _launch('sres_dblock_conv1_backward', self._lib.lvg_sres_dblock_conv1_backward, x, _ptr(x), _ptr(fx), _ptr(fy), int(bool(flip)), _ptr(dy),
+                _ptr(w), _ptr(dhf), _ptr(dw), _DTYPE_CODE[x.dtype], n, cin, cout, h, wd, _ptr(ws), ws.numel())
         return dhf, dw
 
     def fir_adjoint_act_workspace(self, dtype, n, c, h, w):
@@ -1115,12 +1037,9 @@ class SresDblockPlugin:
         dz = torch.empty_like(h0)
         db = torch.empty([c], dtype=torch.float32, device=h0.device) if want_db else None
         ws = torch.empty([need], dtype=torch.uint8, device=h0.device)
-        with _DeviceGuard(h0):
-            rc = _check(self._lib.lvg_sres_dblock_fir_adjoint_act(_ptr(dhf), _ptr(h0), _ptr(fx), _ptr(fy), int(bool(flip)), _ptr(dz), _ptr(db),
-                                                             _ptr(ws), ws.numel(), _DTYPE_CODE[h0.dtype], n, c, h, w, int(act), float(alpha),
-                                                             float(gain), float(clamp), _stream(h0)), 'sres_dblock_fir_adjoint_act')
-        if rc == LVG_UNSUPPORTED:
-            raise RuntimeError('sres_dblock_fir_adjoint_act: ' + self._lib.lvg_last_error().decode())
+        _launch('sres_dblock_fir_adjoint_act', self._lib.lvg_sres_dblock_fir_adjoint_act, h0, _ptr(dhf), _ptr(h0), _ptr(fx), _ptr(fy),
+                int(bool(flip)), _ptr(dz), _ptr(db), _ptr(ws), ws.numel(), _DTYPE_CODE[h0.dtype], n, c, h, w, int(act), float(alpha),
+                float(gain), float(clamp))
         return dz, db
 
     def skip(self, x, w, r, rscale):
@@ -1132,12 +1051,9 @@ class SresDblockPlugin:
         if need < 0:
             raise RuntimeError('sres_dblock_skip: outside the kernel\'s envelope')
         y = torch.empty([n, cout, h, wd], dtype=x.dtype, device=x.device)
-        ws = self._workspace(x.device, need)
-        with _DeviceGuard(x):
-            rc = _check(self._lib.lvg_sres_dblock_skip(_ptr(x), _ptr(w), _ptr(r), _ptr(y), _DTYPE_CODE[x.dtype], n, cin, cout, h * wd, float(rscale),
-                                                  _ptr(ws), ws.numel(), _stream(x)), 'sres_dblock_skip')
-        if rc == LVG_UNSUPPORTED:
-            raise RuntimeError('sres_dblock_skip: ' + self._lib.lvg_last_error().decode())
+        ws = _workspace(x.device, need)
+        _launch('sres_dblock_skip', self._lib.lvg_sres_dblock_skip, x, _ptr(x), _ptr(w), _ptr(r), _ptr(y), _DTYPE_CODE[x.dtype], n, cin, cout,
+                h * wd, float(rscale), _ptr(ws), ws.numel())
         return y
 
 

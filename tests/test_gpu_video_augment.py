@@ -6,6 +6,7 @@ Exact tier: color neutral, small-integer video and dy, dyadic reciprocal scales 
 library's results must equal float64 bit for bit; outputs are NaN-filled and followed by guards, and the workspace has
 exactly lvg_video_augment_workspace bytes. <A x, y> = <x, A^T y>. The installed unmodified run_D against the reference's
 under the same seeds; no host synchronisation; determinism; CUDA-graph capture; the profiler sees the kernels."""
+import json
 import os
 import subprocess
 import sys
@@ -172,29 +173,45 @@ def test_cuda_graph_capture_replays_equal_to_eager():
     assert torch.equal(y_static, y_eager) and torch.equal(gx_static, gx_eager)
 
 
-def test_profiler_sees_every_kernel():
-    """Each kernel instance shows up under torch.profiler. Each instance launches once per sequence, and a profile taken
-    late in a long single-process run of the suite has missed such a single launch, so the sequence runs three times in
-    the session; the library's own launch counter checks the launches independently of the profiler."""
-    n, c, t, h, w = 2, 3, 16, 12, 20
-    p = params(n, t, t, h, w, 0.8, -2, 1, 1, (2, 5, 2, 5)).to(DEV)
-    x = torch.rand(n, c, t, h, w, device=DEV).requires_grad_(True)
-    dy = torch.randn(n, c, t, h, w, device=DEV).requires_grad_(True)
+_PROFILE = r"""
+import json, sys, torch
+sys.path[:0] = sys.argv[1:]
+from torch_utils import custom_ops
+from torch_utils.ops import video_augment as va
+from test_gpu_video_augment import DEV, params
+n, c, t, h, w = 2, 3, 16, 12, 20
+p = params(n, t, t, h, w, 0.8, -2, 1, 1, (2, 5, 2, 5)).to(DEV)
+x = torch.rand(n, c, t, h, w, device=DEV).requires_grad_(True)
+dy = torch.randn(n, c, t, h, w, device=DEV).requires_grad_(True)
 
-    def sequence():                 # forward, adjoint, and the adjoint's backward (the linear forward): 3 calls, 6 launches
-        y = va.apply(x, p, t)
-        gx, = torch.autograd.grad(y, [x], dy, create_graph=True)
-        torch.autograd.grad(gx.square().sum(), [dy])
+def sequence():     # forward, adjoint, and the adjoint's backward (the linear forward): 3 calls, 6 launches
+    y = va.apply(x, p, t)
+    gx, = torch.autograd.grad(y, [x], dy, create_graph=True)
+    torch.autograd.grad(gx.square().sum(), [dy])
 
-    sequence()
+sequence()
+torch.cuda.synchronize()
+before = custom_ops.launch_count()
+with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+    for _ in range(3):
+        sequence()
     torch.cuda.synchronize()
-    before = custom_ops.launch_count()
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        for _ in range(3):
-            sequence()
-        torch.cuda.synchronize()
-    assert custom_ops.launch_count() - before == 3 * 6
-    names = sorted({e.name.replace(' ', '') for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA})
+launches = custom_ops.launch_count() - before
+names = sorted({e.name.replace(' ', '') for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA})
+print(json.dumps(dict(launches=launches, names=names)))
+"""
+
+
+def test_profiler_sees_every_kernel():
+    """Each kernel instance shows up under torch.profiler, and the library's launch counter counts 6 launches per sequence.
+    The profile runs in a process of its own: taken late in a long single-process run of the suite, the profiler has missed
+    a kernel that the launch counter saw."""
+    r = subprocess.run([sys.executable, '-c', _PROFILE, os.path.dirname(os.path.abspath(__file__)), PKG], stdout=subprocess.PIPE,
+                       stderr=subprocess.STDOUT, text=True, timeout=600)
+    assert r.returncode == 0, r.stdout[-3000:]
+    res = json.loads(r.stdout.strip().splitlines()[-1])
+    assert res['launches'] == 3 * 6
+    names = res['names']
     if not names:
         pytest.skip('torch.profiler reported no CUDA kernels on this machine, so launches cannot be observed')
     for k in ('video_augment_reduce_kernel<0>', 'video_augment_reduce_kernel<1>', 'video_augment_fwd_kernel<3,false>',
