@@ -8,7 +8,9 @@ dblock_tail.install against the original method. argv: <out file> <mode>:
   cuda       the whole D (seq_length 16, 64 x 64, batch 2) on the GPU in fp32 and with num_fp16_res=4: without install, with
              install (the conv_bias_act layers) and with install(tail=True) (also every block on the op);
              conv_nd.install_functional and conv3d_down.install on all sides; the kernel names torch.profiler sees in one
-             R1 step and one forward without grad of the last"""
+             R1 step and one forward without grad of the last
+  orient     the whole fp32 D as in cuda with every Downsample3d filter set to the asymmetric [1, 2, 4, 1] / 8: without
+             conv3d_down / dblock_tail, then with both installed (tail=True); the kernel names of one installed R1 step"""
 import sys
 import types
 import warnings
@@ -111,9 +113,10 @@ if mode in ('install_a', 'install_b'):
     torch.save('ok', out_file)
     sys.exit(0)
 
-assert mode == 'cuda'
+assert mode in ('cuda', 'orient')
 conv_nd.install_functional(dl)
-conv3d_down.install(dl)
+if mode == 'cuda':
+    conv3d_down.install(dl)
 x = (torch.rand(2, 3, 16, 64, 64, generator=torch.Generator().manual_seed(12)) * 2 - 1).cuda().requires_grad_(True)
 
 
@@ -130,6 +133,25 @@ def step(D):
     return {'logits': logits.detach().double().cpu(), 'r1_gx': gx.detach().double().cpu(), 'gx': x.grad.double().cpu(),
             'grad': grads.cpu(), 'nograd_logits': plain.double().cpu()}
 
+
+if mode == 'orient':
+    torch.manual_seed(2)
+    D = dl.VideoDiscriminator(seq_length=16, max_edge=64).cuda()
+    filters = [m._downsample_filter for m in D.modules() if type(m).__name__ == 'Downsample3d']
+    with torch.no_grad():
+        for f in filters:
+            f.copy_(torch.tensor([1., 2., 4., 1.]) / 8)
+    out = {'filters': len(filters), 'ref': step(D)}
+    conv3d_down.install(dl)
+    dblock_tail.install(dl, tail=True)
+    out['ours'] = step(D)
+    torch.cuda.synchronize()
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+        step(D)
+        torch.cuda.synchronize()
+    out['kernels'] = sorted({e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA})
+    torch.save(out, out_file)
+    sys.exit(0)
 
 out, nets = {}, {}
 for name, nfp16 in (('fp32', 0), ('fp16', 4)):

@@ -6,7 +6,9 @@ at oracle/_ref/src) with this repository's ops and compares it with and without 
            the installed forward took; kernel names torch.profiler sees in one installed R1 step
   run_D    SuperResVideoGAN.run_D + R1 with augment_pipe.install, then also sres_dblock.install, on the same GAN object
   kernels  kernel names torch.profiler sees in forward + backward passes of four block shapes (fp16 / fp32, 64- / 128-row skips)
-  cpu      install() conventions and the CPU forward of the installed D (bitwise the original)"""
+  cpu      install() conventions and the CPU forward of the installed D (bitwise the original)
+  orient   the all-fp32 D of cuda with every resample_filter set to setup_filter([1, 2, 4, 1]), without and with install;
+           which blocks the installed forward took; kernel names of one installed forward + first-order backward"""
 import pickle
 import sys
 import types
@@ -85,6 +87,33 @@ if mode == 'cuda':
     res['kernels'] = sorted({e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA})
     ds.DiscriminatorBlock.forward = ds.DiscriminatorBlock.forward.lvg_sres_dblock
     ds.Conv2dLayer.forward = ds.Conv2dLayer.forward.lvg_sres_dblock
+elif mode == 'orient':
+    from torch.profiler import ProfilerActivity, profile
+    from torch_utils.ops import upfirdn2d
+    D = make_D(0, seq_length=4, lr_height=16, lr_width=16, hr_height=64, hr_width=64, num_fp16_res=0).cuda()
+    filters = [m.resample_filter for m in D.modules() if getattr(m, 'resample_filter', None) is not None]
+    with torch.no_grad():
+        for f in filters:
+            f.copy_(upfirdn2d.setup_filter([1, 2, 4, 1]))
+    res['filters'] = len(filters)
+    lr, hr = videos(2, 1, 'cuda')
+    res['ref'] = [step(D, lr, hr, r1) for r1 in (False, True)]
+    sres_dblock.install(D)
+    took = []
+    orig_op = sres_dblock.sres_dblock
+
+    def counted(x, *a, **k):
+        took.append(sres_dblock.native(x, a[0], a[1], a[3], a[5], a[6], k.get('act', 'lrelu')))
+        return orig_op(x, *a, **k)
+    sres_dblock.sres_dblock = counted
+    res['ours'] = [step(D, lr, hr, r1) for r1 in (False, True)]
+    sres_dblock.sres_dblock = orig_op
+    res['took'] = took
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        step(D, lr, hr, False)
+        torch.cuda.synchronize()
+    res['kernels'] = sorted({e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA})
 elif mode == 'run_D':
     from model import video_gan_sres as vs
     from model import ada_augment

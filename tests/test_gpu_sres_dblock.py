@@ -144,10 +144,10 @@ def block_params(cin, cout, dtype, seed):
     return {k: v.to(DEV, dtype) for k, v in p.items()}
 
 
-def run_block(fn, x, p, r1):
+def run_block(fn, x, p, r1, f=None):
     x = x.clone().requires_grad_(True)
     q = {k: v.clone().requires_grad_(True) for k, v in p.items()}
-    f = filt()
+    f = filt() if f is None else f
     out = fn(x, q['w_skip'], q['w0'], q['b0'], q['w1'], q['b1'], f, f, act='lrelu', gain=float(np.sqrt(2)), clamp=256)
     if r1:
         gx, = torch.autograd.grad(out.float().square().sum(), [x], create_graph=True)
