@@ -17,7 +17,7 @@ import numpy as np
 import torch
 
 from .. import custom_ops
-from . import grid_sample_gradfix, upfirdn2d
+from . import _install, grid_sample_gradfix, upfirdn2d
 
 NPAR = 23
 GEOM = 1            # LVG_AUGMENT_PIPE_GEOM
@@ -323,23 +323,14 @@ def _forward(orig):
         if not applies(self, videos, debug_percentile):
             return orig(self, videos, debug_percentile)
         return augment(self, videos)
-    forward.lvg_augment_pipe = orig
     return forward
 
 
 def install(*targets):
-    """Make ``AugmentPipe.forward`` run this op. ``targets``: the module ``model.ada_augment`` or ``model.video_gan_sres``
-    (their ``AugmentPipe``), or AugmentPipe instances (their class is patched, which covers pipes reconstructed by
-    ``persistence``). Calls the op does not take (``applies``) run the original method. Opt-in and idempotent; the
-    original stays reachable as ``AugmentPipe.forward.lvg_augment_pipe``. Returns the patched classes."""
-    classes = []
-    for t in targets:
-        cls = getattr(t, 'AugmentPipe', None)
-        if cls is None and isinstance(t, torch.nn.Module) and hasattr(t, 'Hz_geom'):
-            cls = type(t)
-        if cls is not None and not any(cls is k for k in classes):
-            classes.append(cls)
+    """Make ``AugmentPipe.forward`` run this op. ``targets``: the module ``model.ada_augment`` or ``model.video_gan_sres``,
+    or pipes and modules holding them, found by ``_install.find_classes``. Calls ``applies`` rejects run the original
+    method. Idempotent; the original stays reachable as ``.forward.lvg_augment_pipe``. Returns the patched classes."""
+    classes = _install.find_classes(targets, 'AugmentPipe')
     for cls in classes:
-        if getattr(cls.forward, 'lvg_augment_pipe', None) is None:
-            cls.forward = _forward(cls.forward)
+        _install.wrap(cls, 'forward', 'lvg_augment_pipe', _forward)
     return classes

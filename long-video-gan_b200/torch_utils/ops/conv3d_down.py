@@ -25,7 +25,7 @@ slice updates; bias_act), as the R1 penalty needs. ``install(...)`` makes an unm
 """
 import torch
 
-from . import bias_act, conv_nd, upfirdn2d
+from . import _install, bias_act, conv_nd, upfirdn2d
 from .. import custom_ops
 
 # ---------------------------------------------------------------------------------------------------- FIR pair
@@ -275,46 +275,14 @@ def _conv3d_layer_forward(orig):
         bias = self._bias.type(input.dtype) if self.bias else None
         return conv3d_down(input, weight, bias, self.padding, self.spatial_down, self.temporal_down,
                            self.downsample._downsample_filter, act=self.activation, clamp=self.conv_clamp)
-    forward.lvg_conv3d_down = orig
     return forward
 
 
-_WRAPPERS = ('lvg_conv3d_down', 'lvg_conv_bias_act')      # attributes under which an install keeps the method it replaced
-
-
-def wrapped_by(forward, attr):
-    """``forward`` or a method below it in the chain of installed wrappers carries ``attr``. conv3d_down.install (layers with
-    downsampling) and dblock_tail.install (layers without) both replace Conv3dLayer.forward, each calling the method it
-    replaced for the other's layers, in either order."""
-    while forward is not None:
-        if hasattr(forward, attr):
-            return True
-        forward = next((getattr(forward, a) for a in _WRAPPERS if hasattr(forward, a)), None)
-    return False
-
-
-def _patch(cls):
-    if not wrapped_by(cls.forward, 'lvg_conv3d_down'):
-        cls.forward = _conv3d_layer_forward(cls.forward)
-
-
 def install(*targets):
-    """Make the downsampling ``Conv3dLayer``s of reference discriminators run ``conv3d_down``.
-
-    ``targets``: modules (``model.discriminator_lres``, whose ``Conv3dLayer`` class is patched) or ``nn.Module`` instances
-    (the class of every submodule named ``Conv3dLayer`` is patched, which reaches unpickled discriminators whose class
-    source ``persistence`` executed into a module of its own). The new ``forward`` reads the attributes the reference's
-    does; layers without ``spatial_down`` / ``temporal_down`` run the original method. Idempotent. Returns the classes
-    that run it."""
-    classes = []
-    for t in targets:
-        if isinstance(t, torch.nn.Module):
-            classes += [type(m) for m in t.modules() if type(m).__name__ == 'Conv3dLayer']
-        elif getattr(t, 'Conv3dLayer', None) is not None:
-            classes.append(t.Conv3dLayer)
-    done = []
+    """Make the downsampling ``Conv3dLayer``s of reference discriminators run ``conv3d_down``. ``targets``: the module
+    ``model.discriminator_lres`` or discriminator instances, found by ``_install.find_classes``. Other layers run the method
+    it replaced. Idempotent; the original stays reachable as ``.forward.lvg_conv3d_down``. Returns the patched classes."""
+    classes = _install.find_classes(targets, 'Conv3dLayer')
     for cls in classes:
-        if not any(cls is c for c in done):
-            _patch(cls)
-            done.append(cls)
-    return done
+        _install.wrap(cls, 'forward', 'lvg_conv3d_down', _conv3d_layer_forward)
+    return classes

@@ -259,6 +259,17 @@ def conv_bias_act(x, w, b=None, stride=1, padding=0, groups=1, act='linear', alp
     return _ConvBiasAct.apply(x, w, b, pd, groups, st, act, alpha, gain, clamp)
 
 
+def engine_takes(x, w_shape, padding):
+    """The stride-1 convolution of x with weights of ``w_shape`` and ``padding`` (one int per spatial axis) runs on the
+    engine without being asked for the epilogue: LVG_NATIVE_CONV on for x's device, the engine's envelope, and route
+    ``engine`` of ``lvg_convnd_route``. Layers that move bias_act into the epilogue (``conv_bias_act``) only where this
+    holds never leave a faster route for it: 1x1 layers stay on the streaming kernels, which have no epilogue."""
+    from .. import custom_ops
+    x_shape, w_shape, pad = tuple(x.shape), tuple(w_shape), tuple(int(p) for p in padding)
+    return (enabled_for(x) and custom_ops.ConvNdPlugin._in_envelope(x_shape, w_shape, x.dtype, 1, pad, 1, 1)
+            and _get_plugin().route('fprop', x_shape, w_shape, pad, 1, x.dtype, epilogue=False) == 'engine')
+
+
 class _FunctionalProxy:
     """Stands in for the module-level name ``F`` of a reference model file: conv1d / conv2d / conv3d / conv_transpose2d go
     to the tensor-core engine, every other attribute to torch.nn.functional."""

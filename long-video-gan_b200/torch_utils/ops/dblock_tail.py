@@ -27,7 +27,7 @@ import torch
 
 from .. import custom_ops
 from . import bias_act as _bias_act
-from . import conv3d_down, conv_nd, upfirdn2d
+from . import _install, conv3d_down, conv_nd, upfirdn2d
 
 _P = custom_ops.DblockTailPlugin
 _ACTS = {'lrelu': 3, 'linear': 1}           # LVG_ACT_LRELU, LVG_ACT_LINEAR
@@ -211,7 +211,6 @@ def _forward(orig):
         if not routed(self, input, forward.tail):
             return orig(self, input)
         return block_forward(self, input)
-    forward.lvg_dblock_tail = orig
     forward.tail = False
     return forward
 
@@ -227,21 +226,14 @@ def epilogue_faster(layer, input):
 
 
 def epilogue_applies(layer, input):
-    """``Conv3dLayer.forward`` runs ``conv_nd.conv_bias_act``: a layer without downsampling, lrelu or linear, a CUDA fp16 /
-    fp32 input, and a convolution the engine takes without being asked for the epilogue (route ``engine`` of
-    ``lvg_convnd_route``), so that asking for it never takes a layer off a faster route: the 1x1x1 ``conv_vid`` stays on the
-    streaming kernels, which have no epilogue."""
+    """``Conv3dLayer.forward`` runs ``conv_nd.conv_bias_act``: a layer without downsampling, lrelu or linear, a 5-D input
+    whose convolution ``conv_nd.engine_takes`` (the 1x1x1 ``conv_vid`` stays on the streaming kernels), and
+    ``epilogue_faster``."""
     if layer.spatial_down or layer.temporal_down or layer.activation not in _ACTS:
         return False
-    if not (isinstance(input, torch.Tensor) and input.ndim == 5 and input.dtype in (torch.float16, torch.float32)
-            and conv_nd.enabled_for(input)):
+    if not (isinstance(input, torch.Tensor) and input.ndim == 5):
         return False
-    pad = tuple(int(p) for p in layer.padding)
-    if not custom_ops.ConvNdPlugin._in_envelope(tuple(input.shape), tuple(layer.weight.shape), input.dtype, 1, pad, 1, 1):
-        return False
-    if conv_nd._get_plugin().route('fprop', tuple(input.shape), tuple(layer.weight.shape), pad, 1, input.dtype, epilogue=False) != 'engine':
-        return False
-    return epilogue_faster(layer, input)
+    return conv_nd.engine_takes(input, layer.weight.shape, layer.padding) and epilogue_faster(layer, input)
 
 
 def _layer_forward(orig):
@@ -251,37 +243,21 @@ def _layer_forward(orig):
         weight = (self.weight * self.weight_gain).type(input.dtype)
         bias = self._bias.type(input.dtype) if self.bias else None
         return conv_nd.conv_bias_act(input, weight, bias, padding=self.padding, act=self.activation, clamp=self.conv_clamp)
-    forward.lvg_conv_bias_act = orig
     return forward
 
 
 def install(*targets, tail=False):
-    """Patch the classes of an unmodified low-res discriminator. ``targets``: the module ``model.discriminator_lres`` or
-    ``nn.Module`` instances (the classes of their submodules are found by name, which reaches networks that ``persistence``
-    reconstructed from a pickle).
-
-    ``Conv3dLayer.forward``: layers inside ``epilogue_applies`` run ``conv_nd.conv_bias_act``; every other layer runs the
-    method this one replaced, so ``conv3d_down.install`` (the layers with downsampling) wraps or is wrapped by it in either
-    order. ``DiscriminatorBlock.forward``: blocks inside ``routed`` run ``block_forward`` with ``conv_vid``, ``conv_0`` and
-    ``conv_skip`` as the block's modules; ``tail=True`` routes every block the op takes to it although it measured slower
-    (DESIGN.md 7g), for its bitwise reproducible bias gradient. Opt-in and idempotent (a later call sets ``tail`` anew); the
-    originals stay reachable as ``.forward.lvg_dblock_tail`` and ``.forward.lvg_conv_bias_act``. Returns the patched
-    classes, blocks first."""
-    blocks, layers = [], []
-    for t in targets:
-        for name, into in (('DiscriminatorBlock', blocks), ('Conv3dLayer', layers)):
-            if isinstance(t, torch.nn.Module):
-                found = [type(m) for m in t.modules() if type(m).__name__ == name]
-            else:
-                found = [getattr(t, name)] if getattr(t, name, None) is not None else []
-            for cls in found:
-                if not any(cls is c for c in into):
-                    into.append(cls)
+    """Patch the classes of an unmodified low-res discriminator, found by ``_install.find_classes`` in ``targets`` (the
+    module ``model.discriminator_lres`` or discriminator / block instances). ``Conv3dLayer.forward``: layers inside
+    ``epilogue_applies`` run ``conv_nd.conv_bias_act``, every other layer the method it replaced (``conv3d_down.install``
+    wraps the same method). ``DiscriminatorBlock.forward``: blocks inside ``routed`` run ``block_forward``; ``tail=True``
+    routes every block the op takes to it although it measured slower (DESIGN.md 7g), for its bitwise reproducible bias
+    gradient. Idempotent (a later call sets ``tail`` anew); the originals stay reachable as ``.forward.lvg_dblock_tail``
+    and ``.forward.lvg_conv_bias_act``. Returns the patched classes, blocks first."""
+    blocks = _install.find_classes(targets, 'DiscriminatorBlock')
+    layers = _install.find_classes(targets, 'Conv3dLayer')
     for cls in blocks:
-        if getattr(cls.forward, 'lvg_dblock_tail', None) is None:
-            cls.forward = _forward(cls.forward)
-        cls.forward.tail = bool(tail)
+        _install.wrap(cls, 'forward', 'lvg_dblock_tail', _forward).tail = bool(tail)
     for cls in layers:
-        if not conv3d_down.wrapped_by(cls.forward, 'lvg_conv_bias_act'):
-            cls.forward = _layer_forward(cls.forward)
+        _install.wrap(cls, 'forward', 'lvg_conv_bias_act', _layer_forward)
     return blocks + layers

@@ -25,6 +25,7 @@ import math
 import torch
 
 from .. import custom_ops
+from . import _install
 from . import bias_act as _bias_act
 from . import conv_nd
 from . import upfirdn2d
@@ -220,33 +221,22 @@ def block_forward(block, g, input, latent, magnitude_ema_beta=1.0, out_seq_lengt
 
 
 def _forward(orig):
+    g = _install.reference_function(orig).__globals__
+
     def forward(self, input, latent, magnitude_ema_beta=1.0, out_seq_length=None, dtype=None):
         dt = dtype if dtype is not None else (torch.float16 if self.use_float16 and input.is_cuda else torch.float32)
         if not applies(self, input, dt, out_seq_length):
             return orig(self, input, latent, magnitude_ema_beta, out_seq_length, dtype)
-        return block_forward(self, orig.__globals__, input, latent, magnitude_ema_beta, out_seq_length, dtype)
-    forward.lvg_gblock_tail = orig
+        return block_forward(self, g, input, latent, magnitude_ema_beta, out_seq_length, dtype)
     return forward
 
 
 def install(*targets):
-    """Make ``Synthesis3dResBlock.forward`` run ``block_forward``. ``targets``: the module ``model.generator_lres`` (its
-    ``Synthesis3dResBlock``) or ``nn.Module`` instances (the class of every Synthesis3dResBlock among their submodules is
-    patched, which reaches blocks that ``persistence`` reconstructed from a pickle). Calls outside the op's envelope
-    (``applies``: CPU tensors, fp64, other activations, resamplers with padding or another scale) run the original method.
-    Opt-in and idempotent; the original stays reachable as ``Synthesis3dResBlock.forward.lvg_gblock_tail``. Returns the
-    patched classes."""
-    classes = []
-    for t in targets:
-        found = []
-        if isinstance(t, torch.nn.Module):
-            found = [type(m) for m in t.modules() if type(m).__name__ == 'Synthesis3dResBlock']
-        elif getattr(t, 'Synthesis3dResBlock', None) is not None:
-            found = [t.Synthesis3dResBlock]
-        for cls in found:
-            if not any(cls is c for c in classes):
-                classes.append(cls)
+    """Make ``Synthesis3dResBlock.forward`` run ``block_forward``. ``targets``: the module ``model.generator_lres`` or
+    generator / block instances, found by ``_install.find_classes``. Calls outside ``applies`` (CPU tensors, fp64, other
+    activations, resamplers with padding or another scale) run the original method. Idempotent; the original stays
+    reachable as ``.forward.lvg_gblock_tail``. Returns the patched classes."""
+    classes = _install.find_classes(targets, 'Synthesis3dResBlock')
     for cls in classes:
-        if getattr(cls.forward, 'lvg_gblock_tail', None) is None:
-            cls.forward = _forward(cls.forward)
+        _install.wrap(cls, 'forward', 'lvg_gblock_tail', _forward)
     return classes

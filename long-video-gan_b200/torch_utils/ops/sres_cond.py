@@ -32,6 +32,7 @@ import numpy as np
 import torch
 
 from .. import custom_ops
+from . import _install
 
 MAX_TAPS = 64                                      # kMaxTaps of csrc/sres_cond.cu
 
@@ -290,39 +291,28 @@ def generator_forward(G, g, z, cond, truncation_psi=1, truncation_cutoff=None, u
 
 
 def _forward(orig):
+    g = _install.reference_function(orig).__globals__
+
     def forward(self, z, cond, truncation_psi=1, truncation_cutoff=None, update_emas=False, **synthesis_kwargs):
         lr_plans = plans(self, cond.size(3), cond.size(4)) if isinstance(cond, torch.Tensor) and cond.ndim == 5 else None
         if lr_plans is None or not applies(self, cond, lr_plans):
             return orig(self, z, cond, truncation_psi, truncation_cutoff, update_emas, **synthesis_kwargs)
-        return generator_forward(self, orig.__globals__, z, cond, truncation_psi, truncation_cutoff, update_emas,
-                                 lr_plans=lr_plans, **synthesis_kwargs)
-    forward.lvg_sres_cond = orig
+        return generator_forward(self, g, z, cond, truncation_psi, truncation_cutoff, update_emas, lr_plans=lr_plans,
+                                 **synthesis_kwargs)
     return forward
 
 
-def _is_generator(cls):
-    return cls.__name__ == 'Generator' and all(hasattr(cls, a) for a in ('prep_cond', 'forward'))
+def _is_generator(m):
+    return all(hasattr(m, a) for a in ('prep_cond', 'synthesis', 'resamples'))
 
 
 def install(*targets):
     """Make ``Generator.forward`` of generator_sres run ``generator_forward``. ``targets``: the module
-    ``model.generator_sres`` (its ``Generator``) or ``nn.Module`` instances (the class of every such Generator among their
-    submodules is patched, which reaches generators that ``persistence`` reconstructed from a pickle). A class counts when
-    it is named ``Generator``, has ``prep_cond`` and its instances have ``synthesis`` and ``resamples``. Calls outside the
-    op's envelope (``applies``: CPU tensors, a low-res video that is not fp32 or needs a gradient, other resamplers, longer
-    filters, shapes the kernel rejects) run the original method. Opt-in and idempotent; the original stays reachable as
-    ``Generator.forward.lvg_sres_cond``. Returns the patched classes."""
-    classes = []
-    for t in targets:
-        found = []
-        if isinstance(t, torch.nn.Module):
-            found = [type(m) for m in t.modules() if _is_generator(type(m)) and hasattr(m, 'synthesis') and hasattr(m, 'resamples')]
-        elif getattr(t, 'Generator', None) is not None and _is_generator(t.Generator):
-            found = [t.Generator]
-        for cls in found:
-            if not any(cls is c for c in classes):
-                classes.append(cls)
+    ``model.generator_sres`` or instances holding a ``Generator`` with ``prep_cond``, ``synthesis`` and ``resamples``,
+    found by ``_install.find_classes``. Calls outside ``applies`` (CPU tensors, a low-res video that is not fp32 or needs a
+    gradient, other resamplers, longer filters, shapes the kernel rejects) run the original method. Idempotent; the
+    original stays reachable as ``.forward.lvg_sres_cond``. Returns the patched classes."""
+    classes = _install.find_classes(targets, 'Generator', _is_generator)
     for cls in classes:
-        if getattr(cls.forward, 'lvg_sres_cond', None) is None:
-            cls.forward = _forward(cls.forward)
+        _install.wrap(cls, 'forward', 'lvg_sres_cond', _forward)
     return classes

@@ -32,7 +32,7 @@ import torch
 
 from .. import custom_ops
 from . import bias_act as _bias_act
-from . import conv2d_resample, conv_nd, upfirdn2d
+from . import _install, conv2d_resample, conv_nd, upfirdn2d
 
 _SQRT_HALF = float(np.sqrt(0.5))             # the reference's factor, np.sqrt(0.5)
 
@@ -285,23 +285,17 @@ def _forward(orig):
         if not applies(self, x, img, force_fp32) or not faster(self.resolution):
             return orig(self, x, img, force_fp32)
         return block_forward(self, x, img, force_fp32)
-    forward.lvg_sres_dblock = orig
     return forward
 
 
 def layer_applies(layer, x):
-    """``Conv2dLayer.forward`` runs ``conv_nd.conv_bias_act``: no resampling or dropout, lrelu / linear, a CUDA fp16 /
-    fp32 NCHW input, and a convolution the engine takes without being asked for the epilogue (route ``engine``), so that
-    asking for it never moves a layer off the pointwise kernels (``fromrgb`` stays there)."""
+    """``Conv2dLayer.forward`` runs ``conv_nd.conv_bias_act``: no resampling or dropout, lrelu / linear, and a contiguous
+    NCHW input whose convolution ``conv_nd.engine_takes`` (``fromrgb`` stays on the pointwise kernels)."""
     if layer.up != 1 or layer.down != 1 or layer.dropout_p > 0 or layer.activation not in ('lrelu', 'linear'):
         return False
-    if not (isinstance(x, torch.Tensor) and x.ndim == 4 and x.dtype in (torch.float16, torch.float32) and x.is_contiguous()
-            and conv_nd.enabled_for(x)):
+    if not (isinstance(x, torch.Tensor) and x.ndim == 4 and x.is_contiguous()):
         return False
-    pad = (layer.padding, layer.padding)
-    if not custom_ops.ConvNdPlugin._in_envelope(tuple(x.shape), tuple(layer.weight.shape), x.dtype, 1, pad, 1, 1):
-        return False
-    return conv_nd._get_plugin().route('fprop', tuple(x.shape), tuple(layer.weight.shape), pad, 1, x.dtype, epilogue=False) == 'engine'
+    return conv_nd.engine_takes(x, layer.weight.shape, (layer.padding, layer.padding))
 
 
 def _layer_forward(orig):
@@ -311,30 +305,27 @@ def _layer_forward(orig):
         w, b = _layer_args(self, x.dtype)
         clamp = self.conv_clamp * gain if self.conv_clamp is not None else None
         return conv_nd.conv_bias_act(x, w, b, padding=self.padding, act=self.activation, gain=self.act_gain * gain, clamp=clamp)
-    forward.lvg_sres_dblock = orig
     return forward
 
 
+def _roots(module):
+    return [m for m in module.modules() if type(m).__name__ == 'VideoDiscriminator'] or [module]
+
+
+def _has_filter(module):
+    return hasattr(module, 'resample_filter')          # the low-res D's DiscriminatorBlock has none
+
+
 def install(*targets):
-    """Patch the classes of an unmodified super-res discriminator. ``targets``: the module ``model.discriminator_sres``, or
-    ``nn.Module`` instances (a ``VideoDiscriminator``, a block, a ``SuperResVideoGAN``): the classes of their submodules
-    are found by name, which reaches classes that ``persistence`` rebuilt from a pickle. Idempotent; the originals stay
-    reachable as ``.forward.lvg_sres_dblock``. Returns the patched classes, blocks first."""
-    blocks, layers = [], []
-    for t in targets:
-        for name, into in (('DiscriminatorBlock', blocks), ('Conv2dLayer', layers)):
-            if isinstance(t, torch.nn.Module):
-                roots = [m for m in t.modules() if type(m).__name__ == 'VideoDiscriminator'] or [t]
-                found = [type(m) for r in roots for m in r.modules() if type(m).__name__ == name and hasattr(m, 'resample_filter')]
-            else:
-                found = [getattr(t, name)] if getattr(t, name, None) is not None else []
-            for cls in found:
-                if not any(cls is c for c in into):
-                    into.append(cls)
+    """Patch ``DiscriminatorBlock.forward`` and ``Conv2dLayer.forward`` of an unmodified super-res discriminator.
+    ``targets``: the module ``model.discriminator_sres`` or discriminator / block instances, found by
+    ``_install.find_classes`` among the modules with a ``resample_filter``, below every ``VideoDiscriminator`` of a target
+    that holds one. Idempotent; the originals stay reachable as ``.forward.lvg_sres_dblock``. Returns the patched classes,
+    blocks first."""
+    blocks = _install.find_classes(targets, 'DiscriminatorBlock', _has_filter, _roots)
+    layers = _install.find_classes(targets, 'Conv2dLayer', _has_filter, _roots)
     for cls in blocks:
-        if getattr(cls.forward, 'lvg_sres_dblock', None) is None:
-            cls.forward = _forward(cls.forward)
+        _install.wrap(cls, 'forward', 'lvg_sres_dblock', _forward)
     for cls in layers:
-        if getattr(cls.forward, 'lvg_sres_dblock', None) is None:
-            cls.forward = _layer_forward(cls.forward)
+        _install.wrap(cls, 'forward', 'lvg_sres_dblock', _layer_forward)
     return blocks + layers

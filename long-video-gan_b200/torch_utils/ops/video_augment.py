@@ -21,6 +21,7 @@ import math
 import torch
 
 from .. import custom_ops
+from . import _install
 
 NPAR = 12
 STEPS = ('color', 'translation', 'cutout')
@@ -230,26 +231,22 @@ def applies(video, policy, temp_scale_augment, seq_length):
 
 
 def _run_D(orig):
+    g = _install.reference_function(orig).__globals__
+
     def run_D(self, video):
         if not applies(video, self.diffaug_policy, self.temp_scale_augment, self.seq_length):
             return orig(self, video)
-        orig.__globals__['misc'].assert_shape(video, (None, self.channels, self.seq_length, self.height, self.width))
+        g['misc'].assert_shape(video, (None, self.channels, self.seq_length, self.height, self.width))
         params = draw_params(video, self.diffaug_policy, self.temp_scale_augment, self.seq_length)
         return self.D(apply(video, params, self.seq_length))
-    run_D.lvg_video_augment = orig
     return run_D
 
 
 def install(*targets):
     """Make ``LowResVideoGAN.run_D`` build D's input with this op. ``targets``: the module ``model.video_gan_lres`` or
-    LowResVideoGAN instances (their class is patched). Inputs the op does not take (``applies``) run the original method.
-    Opt-in and idempotent. Returns the patched classes."""
-    classes = []
-    for t in targets:
-        cls = getattr(t, 'LowResVideoGAN', None) or (type(t) if callable(getattr(type(t), 'run_D', None)) else None)
-        if cls is not None and not any(cls is c for c in classes):
-            classes.append(cls)
+    LowResVideoGAN instances, found by ``_install.find_classes``. Inputs ``applies`` rejects run the original method.
+    Idempotent; the original stays reachable as ``.run_D.lvg_video_augment``. Returns the patched classes."""
+    classes = _install.find_classes(targets, 'LowResVideoGAN')
     for cls in classes:
-        if getattr(cls.run_D, 'lvg_video_augment', None) is None:
-            cls.run_D = _run_D(cls.run_D)
+        _install.wrap(cls, 'run_D', 'lvg_video_augment', _run_D)
     return classes

@@ -151,6 +151,11 @@ elif mode == 'install':
     assert ap.install(m) == [ada_augment.AugmentPipe] and ada_augment.AugmentPipe.forward.lvg_augment_pipe is orig
     from model import video_gan_sres as vs
     assert ap.install(vs) == [ada_augment.AugmentPipe] and ada_augment.AugmentPipe.forward.lvg_augment_pipe is orig
+    # pipes inside a container are reached; a module of another name is not, whatever its attributes
+    assert ap.install(torch.nn.ModuleList([m])) == [ada_augment.AugmentPipe]
+    other = torch.nn.Module()
+    other.register_buffer('Hz_geom', m.Hz_geom)
+    assert ap.install(other) == []
     calls = []
 
     def spy(self, v, debug_percentile=None):

@@ -7,8 +7,10 @@ fp32 layers (the flag `lvg_convnd_plan` reports in slot 47), for the pointwise w
 pixel-row pitch -- and every other call stays on the engine. Weight gradients run on the engine."""
 import ctypes
 import itertools
+import types
 
 import pytest
+import torch
 
 from torch_utils import custom_ops
 
@@ -62,3 +64,21 @@ def test_route_outside_envelope(lib):
     assert lib.lvg_convnd_route(0, 2, 1, 1, 8, 8, 1, 1, 8, 1, 1, 1, 0, 0, 0, 1, 0) == -1           # fp64
     assert lib.lvg_convnd_route(0, 0, 1, 1, 8, 8, 1, 8, 8, 1, 5, 2, 0, 0, 0, 1, 0) == -1           # kh * kw > 9
     assert lib.lvg_convnd_route(1, 0, 1, 1, 8, 8, 1, 8, 8, 1, 3, 3, 0, 3, 3, 1, 0) == -1           # dgrad padding > k - 1
+
+
+def test_engine_takes(monkeypatch):
+    """conv_nd.engine_takes, which decides where the installed Conv3dLayer / Conv2dLayer forwards move bias_act into the
+    epilogue: engine-routed calls only, never a 1x1 layer of the pointwise kernels, fp64 or the switch turned off."""
+    from torch_utils.ops import conv_nd
+
+    def x(*shape, dtype=torch.float16):
+        return types.SimpleNamespace(device=types.SimpleNamespace(type='cuda'), shape=shape, dtype=dtype)
+    assert conv_nd.engine_takes(x(2, 16, 4, 8, 8), (32, 16, 3, 3, 3), (1, 1, 1))
+    assert conv_nd.engine_takes(x(2, 16, 8, 8, dtype=torch.float32), (32, 16, 3, 3), (1, 1))
+    assert not conv_nd.engine_takes(x(2, 16, 4, 8, 8), (32, 16, 1, 1, 1), (0, 0, 0))            # pointwise kernels
+    assert not conv_nd.engine_takes(x(2, 16, 4, 8, 8, dtype=torch.float64), (32, 16, 3, 3, 3), (1, 1, 1))
+    assert not conv_nd.engine_takes(x(2, 16, 4, 8, 8), (32, 16, 3, 3, 3), (3, 1, 1))             # padding > k - 1
+    assert not conv_nd.engine_takes(types.SimpleNamespace(device=torch.device('cpu'), shape=(2, 16, 8, 8),
+                                                          dtype=torch.float16), (32, 16, 3, 3), (1, 1))
+    monkeypatch.setenv('LVG_NATIVE_CONV', '0')
+    assert not conv_nd.engine_takes(x(2, 16, 4, 8, 8), (32, 16, 3, 3, 3), (1, 1, 1))

@@ -117,6 +117,8 @@ elif mode == 'install':
     assert va.install(vg) == [vg.LowResVideoGAN] and vg.LowResVideoGAN.run_D.lvg_video_augment is orig    # idempotent
     g = gan('color,translation,cutout', 1.0, 3, 8, 6, 10)
     assert va.install(g) == [vg.LowResVideoGAN] and vg.LowResVideoGAN.run_D.lvg_video_augment is orig
+    # another class with a run_D (the super-res GAN's takes other arguments) is not reached
+    assert va.install(type('SuperResVideoGAN', (), {'run_D': lambda self, lr, hr: None})()) == []
     calls = []
 
     def spy(self, v):
