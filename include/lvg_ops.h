@@ -440,6 +440,34 @@ int lvg_sres_cond(const void* x, const float* lr, const float* f_h, const float*
                   float gain_w, void* stream);
 
 /*
+ * A super-res generator layer's modulated convolution with its input built inside the convolution's re-tiling pass
+ * (DESIGN.md 7j):  y = d (.) conv(a (.) z, w)  with  z = cat(x, cond(lr)).to(dtype)  as lvg_sres_cond defines it, z never
+ * stored. x, lr, f_h, f_w, x_dtype, n, t, c, c_lr, window, t_lr, h_lr, w_lr, lr_strides, plan_h, plan_w, gain_h, gain_w:
+ * as lvg_sres_cond (dtype = its z_dtype, the layer's). The convolution as lvg_modconv_fprop with cin = c + c_lr window,
+ * t = 1 and n t samples: w [cout][cin][kh][kw] (dtype), a fp32 [n t][cin], d fp32 [n t][cout] or NULL, y [n t][cout][ho][wo]
+ * (dtype). Bit for bit lvg_modconv_fprop of lvg_sres_cond's z. mean_sq (NULL = not wanted): as lvg_sres_cond's, from
+ * per-CTA partials folded in a fixed order (bitwise reproducible; not the same fold as lvg_sres_cond's). y NULL: mean_sq
+ * alone, from the same pass without its stores (w, a unused), for callers whose factor a depends on the statistic.
+ * lvg_sres_layer_backward: lvg_modconv_backward of that call with dx the gradient of x alone, written in x_dtype
+ * (x_dtype(dtype(a dx')), the cast of z's gradient; NULL = not wanted), dw (NULL = not wanted), da [n t][cin] over all
+ * channels, dyy (NULL = not wanted; needs y and d). One workspace size serves both calls; the size query returns -1 for
+ * anything the kernels do not take, and the ops then return LVG_UNSUPPORTED.
+ */
+int64_t lvg_sres_layer_workspace(int dtype, int n, int t, int c, int c_lr, int window, int t_lr, int h_lr, int w_lr,
+                                 const int* plan_h, const int* plan_w, int cout, int kh, int kw, int pad_h, int pad_w);
+int lvg_sres_layer_fprop(const void* x, const float* lr, const float* f_h, const float* f_w, const void* w, const float* a,
+                         const float* d, void* y, float* mean_sq, int x_dtype, int dtype, int n, int t, int c, int c_lr,
+                         int window, int t_lr, int h_lr, int w_lr, const int64_t* lr_strides, const int* plan_h,
+                         const int* plan_w, float gain_h, float gain_w, int cout, int kh, int kw, int pad_h, int pad_w,
+                         void* workspace, int64_t workspace_bytes, void* stream);
+int lvg_sres_layer_backward(const void* x, const float* lr, const float* f_h, const float* f_w, const void* w, const float* a,
+                            const float* d, const void* y, const void* dy, void* dx, void* dw, float* da, float* dyy,
+                            int x_dtype, int dtype, int n, int t, int c, int c_lr, int window, int t_lr, int h_lr, int w_lr,
+                            const int64_t* lr_strides, const int* plan_h, const int* plan_w, float gain_h, float gain_w,
+                            int cout, int kh, int kw, int pad_h, int pad_w, void* workspace, int64_t workspace_bytes,
+                            void* stream);
+
+/*
  * Layers of a super-res discriminator block (discriminator_sres.py DiscriminatorBlock, architecture 'resnet'; DESIGN.md 7i).
  *
  * lvg_sres_dblock_conv1: conv1, y = bias_act(conv2d(upfirdn2d(x, f, padding 2), w, stride 2), bias, act, alpha, gain,

@@ -9,6 +9,7 @@
 // resampler's FIR out[m] = gain * sum_k f[K - 1 - k] * zu[m down + k - pad0] over the zero-upsampled (by `up`) replicate-
 // padded frame, zero outside [0, zlen) (upfirdn2d's own zero padding), then sample v = j / up of that frame reads the
 // low-res row / column clamp(v - shift, 0, len - 1) (the nested replicate pads). Identity axes: K = 0 (one tap of 1).
+// The tap tables and both passes live in sres_cond.cuh: conv_pack_cond_kernel (conv_igemm.cu) evaluates the same sums.
 //
 // One launch: the first CTAs copy x_prev per sample (16-byte stores, loads as wide as the source's alignment allows,
 // scalar head and tail), the rest each own a (n', channel, run of output rows) tile of the conditioning: per-axis tap
@@ -19,22 +20,19 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "sres_cond.cuh"
 
 namespace lvg {
 namespace {
 
+using sres::Axis;
+using sres::axis_taps;
+using sres::read_axis;
+
 constexpr int kThreads = 256;
 constexpr int kVecPerThread = 4;             // 16-byte vectors per thread of a copy CTA
-constexpr int kMaxTaps = 64;                 // filter taps per axis
 constexpr int kRows = 16;                    // output rows per conditioning CTA
 constexpr int kSmemBytes = 48 * 1024;
-
-struct Axis {
-    int out, px0, mhi, x0, up, down, pad0, zlen, shift, ntaps, len;
-    int nt;                                  // taps per output: ceil(ntaps / up), 1 for identity
-    float gain;
-    const float* f;
-};
 
 struct CondParams {
     const void* x;
@@ -48,31 +46,6 @@ struct CondParams {
     int64_t copy_ctas;
     Axis ah, aw;
 };
-
-// taps of output index i along an axis: (source index, weight) for each of a.nt slots, weight 0 where unused
-__device__ __forceinline__ void axis_taps(const Axis& a, int i, int* src, float* wgt)
-{
-    const int m = a.x0 + min(max(i - a.px0, 0), a.mhi);
-    if (a.ntaps == 0) {
-        src[0] = min(max(m - a.shift, 0), a.len - 1);
-        wgt[0] = 1.f;
-        return;
-    }
-    const int base = m * a.down - a.pad0;                    // zu index of tap k = base + k
-    int k = ((-base) % a.up + a.up) % a.up;                   // first tap on a nonzero (non-inserted) sample
-    int slot = 0;
-    for (; k < a.ntaps; k += a.up, slot++) {
-        const int j = base + k;
-        const bool in = j >= 0 && j < a.zlen;
-        const int v = in ? j / a.up : 0;
-        src[slot] = min(max(v - a.shift, 0), a.len - 1);
-        wgt[slot] = in ? a.gain * __ldg(a.f + a.ntaps - 1 - k) : 0.f;
-    }
-    for (; slot < a.nt; slot++) {
-        src[slot] = 0;
-        wgt[slot] = 0.f;
-    }
-}
 
 template <class T> __device__ __forceinline__ float ld1(const T* p) { return to_acc(__ldg(p)); }
 
@@ -198,12 +171,7 @@ __device__ void cond_cta(const CondParams& p, int64_t b, unsigned char* smem)
     const float* __restrict__ L = p.lr + n * p.s_n + c * p.s_c + (int64_t)(t + s) * p.s_t;
     for (int idx = threadIdx.x; idx < rows * wl; idx += kThreads) {
         const int r = idx / wl, x = idx - r * wl;
-        float acc = 0.f;
-        for (int k = 0; k < nth; k++) {
-            const float wk = wh[r * nth + k];
-            if (wk != 0.f) acc += wk * __ldg(L + sh[r * nth + k] * p.s_h + x * p.s_w);
-        }
-        inter[idx] = acc;
+        inter[idx] = sres::vertical_tap_sum(L, p.s_h, p.s_w, x, wh + r * nth, sh + r * nth, nth);
     }
     __syncthreads();
 
@@ -213,12 +181,7 @@ __device__ void cond_cta(const CondParams& p, int64_t b, unsigned char* smem)
     float sq = 0.f;
     for (int idx = threadIdx.x; idx < rows * wout; idx += kThreads) {
         const int r = idx / wout, i = idx - r * wout;
-        const float* row = inter + r * wl;
-        float acc = 0.f;
-        for (int k = 0; k < ntw; k++) {
-            const float wk = ww[i * ntw + k];
-            if (wk != 0.f) acc += wk * row[sw[i * ntw + k]];
-        }
+        const float acc = sres::horizontal_tap_sum(inter + r * wl, ww + i * ntw, sw + i * ntw, ntw);
         sq += acc * acc;
         out[idx] = from_acc<TO>(acc);
     }
@@ -258,22 +221,6 @@ struct Plan {
     int64_t copy_ctas, ctas;
     int smem;
 };
-
-bool read_axis(const int* q, int len, Axis& a)
-{
-    a.out = q[0]; a.px0 = q[1]; a.mhi = q[2]; a.x0 = q[3]; a.up = q[4]; a.down = q[5]; a.pad0 = q[6]; a.zlen = q[7];
-    a.shift = q[8]; a.ntaps = q[9]; a.len = len;
-    if (a.out < 1 || a.out > (1 << 20) || a.mhi < 0 || a.x0 < 0 || a.up < 1 || a.down < 1 || a.zlen < 1 || len < 1
-        || a.ntaps < 0 || a.ntaps > kMaxTaps || a.up > kMaxTaps || a.down > kMaxTaps)
-        return false;
-    if (a.ntaps == 0 && (a.up != 1 || a.down != 1 || a.pad0 != 0)) return false;
-    a.nt = a.ntaps == 0 ? 1 : (a.ntaps + a.up - 1) / a.up;
-    // every index the kernel forms stays far inside int
-    const int64_t mmax = (int64_t)a.x0 + a.mhi;
-    if (mmax * a.down + a.ntaps + (a.pad0 < 0 ? -(int64_t)a.pad0 : (int64_t)a.pad0) > (1 << 28)) return false;
-    if (a.px0 < -(1 << 20) || a.px0 > (1 << 20) || a.shift < -(1 << 20) || a.shift > (1 << 20)) return false;
-    return true;
-}
 
 bool make_plan(int n, int t, int c, int c_lr, int window, int t_lr, int h_lr, int w_lr, int z_dtype, const int* plan_h,
                const int* plan_w, Axis& ah, Axis& aw, Plan& pl)

@@ -93,6 +93,11 @@ _SIGNATURES = {
     'lvg_dblock_tail_adjoint': (_c_int, [_c_void_p] * 7 + [_c_i64] + [_c_int] * 8 + [_c_float] * 2 + [_c_void_p]),
     'lvg_sres_cond_workspace': (_c_i64, [_c_int] * 9 + [_c_void_p] * 2),
     'lvg_sres_cond': (_c_int, [_c_void_p] * 7 + [_c_i64] + [_c_int] * 10 + [_c_void_p] * 3 + [_c_float] * 2 + [_c_void_p]),
+    'lvg_sres_layer_workspace': (_c_i64, [_c_int] * 9 + [_c_void_p] * 2 + [_c_int] * 5),
+    'lvg_sres_layer_fprop': (_c_int, [_c_void_p] * 9 + [_c_int] * 10 + [_c_void_p] * 3 + [_c_float] * 2 + [_c_int] * 5
+                             + [_c_void_p, _c_i64, _c_void_p]),
+    'lvg_sres_layer_backward': (_c_int, [_c_void_p] * 13 + [_c_int] * 10 + [_c_void_p] * 3 + [_c_float] * 2 + [_c_int] * 5
+                                + [_c_void_p, _c_i64, _c_void_p]),
     'lvg_sres_dblock_conv1_workspace': (_c_i64, [_c_int] * 6),
     'lvg_sres_dblock_conv1': (_c_int, [_c_void_p] * 3 + [_c_int] + [_c_void_p] * 3 + [_c_int] * 7 + [_c_float] * 3 + [_c_void_p, _c_i64, _c_void_p]),
     'lvg_sres_dblock_conv1_backward_workspace': (_c_i64, [_c_int] * 6),
@@ -208,7 +213,7 @@ _ws = {}
 
 def _workspace(device, need):
     """The convolution engine's workspace on ``device``: one buffer of at least ``need`` bytes (and 4 MiB), grown on
-    demand and shared by every ConvNdPlugin and SresDblockPlugin call."""
+    demand and shared by every ConvNdPlugin and SresDblockPlugin call and the SresCondPlugin layer calls."""
     if need < 0:
         raise RuntimeError('convnd: configuration outside the tensor-core kernel envelope')
     buf = _ws.get(device)
@@ -977,6 +982,88 @@ class SresCondPlugin:
                 _DTYPE_CODE[x.dtype] if x is not None else _DTYPE_CODE[dtype], _DTYPE_CODE[dtype], n, t, c, c_lr, window, t_lr, h_lr, w_lr,
                 strides, ph, pw, float(gain_h), float(gain_w))
         return z, ms
+
+    # ---- the layer's modulated convolution with z built in its re-tiling pass (lvg_sres_layer_*)
+
+    def layer_workspace(self, n, t, c, c_lr, window, t_lr, h_lr, w_lr, dtype, plan_h, plan_w, cout, kh, kw, pad_h, pad_w):
+        """Workspace bytes of lvg_sres_layer_fprop / _backward, or -1 where the kernels do not take the call."""
+        return int(self._lib.lvg_sres_layer_workspace(_DTYPE_CODE.get(dtype, -1), n, t, c, c_lr, window, t_lr, h_lr, w_lr,
+                                                      self._plan(plan_h), self._plan(plan_w), cout, kh, kw, pad_h, pad_w))
+
+    def _layer_args(self, x, lr, f_h, f_w, plan_h, plan_w, window, dtype, w, a, d, padding):
+        """Checked arguments shared by layer_fprop and layer_backward."""
+        if not lr.is_cuda or lr.dtype != torch.float32 or lr.ndim != 5:
+            raise RuntimeError('sres_layer: lr must be a 5-D float32 CUDA tensor')
+        n, c_lr, t_lr, h_lr, w_lr = lr.shape
+        t = t_lr - window + 1
+        h, wd = int(plan_h[0]), int(plan_w[0])
+        c = 0 if x is None else x.shape[1]
+        if x is not None and (x.dtype not in (torch.float16, torch.float32) or x.device != lr.device
+                              or tuple(x.shape) != (n * t, c, h, wd)):
+            raise RuntimeError(f'sres_layer: x must be a float16 / float32 [{n * t}, C, {h}, {wd}] tensor on the device of lr')
+        cin = c + c_lr * window
+        if w.dtype != dtype or w.ndim != 4 or w.shape[1] != cin or w.device != lr.device:
+            raise RuntimeError(f'sres_layer: w must be a {dtype} [Cout, {cin}, kh, kw] tensor on the device of lr')
+        cout, kh, kw = int(w.shape[0]), int(w.shape[2]), int(w.shape[3])
+        if a is not None and (a.dtype != torch.float32 or a.numel() != n * t * cin) or d is not None and (d.dtype != torch.float32 or
+                                                                                                    d.numel() != n * t * cout):
+            raise RuntimeError('sres_layer: a must be float32 [N T, Cin], d float32 [N T, Cout] or None')
+        for f, q in ((f_h, plan_h), (f_w, plan_w)):
+            k = int(q[9])
+            if (k == 0) != (f is None) or f is not None and (f.dtype != torch.float32 or f.numel() != k or f.device != lr.device):
+                raise RuntimeError(f'sres_layer: a filter of {k} float32 taps on the device of lr (None for an identity axis)')
+        ph, pw = self._plan(plan_h), self._plan(plan_w)
+        dims = (n, t, c, c_lr, window, t_lr, h_lr, w_lr)
+        conv = (cout, kh, kw, int(padding[0]), int(padding[1]))
+        need = int(self._lib.lvg_sres_layer_workspace(_DTYPE_CODE[dtype], *dims, ph, pw, *conv))
+        if need < 0:
+            raise RuntimeError(f'sres_layer: no kernel for {list(lr.shape)}, window {window}, C {c}, w {list(w.shape)}, '
+                               f'padding {list(padding)}')
+        return dict(x=None if x is None else x.contiguous(), f_h=None if f_h is None else f_h.contiguous(),
+                    f_w=None if f_w is None else f_w.contiguous(), w=w.contiguous(), a=None if a is None else a.contiguous(),
+                    d=None if d is None else d.contiguous(), dims=dims, conv=conv, ph=ph, pw=pw, need=need,
+                    strides=(_c_i64 * 5)(*lr.stride()), out=(n * t, cout, h + 2 * conv[3] - kh + 1, wd + 2 * conv[4] - kw + 1))
+
+    def layer_fprop(self, x, lr, f_h, f_w, plan_h, plan_w, gain_h, gain_w, window, dtype, w, a, d, padding, want_sumsq):
+        """(y = d * conv(a * z, w) [N T, Cout, Ho, Wo] in ``dtype``, mean square of the fp32 z (0-dim) or None) with
+        z = cat(x, cond(lr)).to(dtype) as ``forward`` builds it, never stored. a [N T, Cin], d [N T, Cout] or None: fp32.
+        a None: (None, mean square) from the same pass without the convolution."""
+        q = self._layer_args(x, lr, f_h, f_w, plan_h, plan_w, window, dtype, w, a, d, padding)
+        if a is None and not want_sumsq:
+            raise RuntimeError('sres_layer_fprop: a call without a computes the mean square alone')
+        y = torch.empty(q['out'], dtype=dtype, device=lr.device) if a is not None else None
+        ms = torch.empty([], dtype=torch.float32, device=lr.device) if want_sumsq else None
+        ws = _workspace(lr.device, q['need'])
+        xt = q['x']
+        _launch('sres_layer_fprop', self._lib.lvg_sres_layer_fprop, lr, _ptr(xt), _ptr(lr), _ptr(q['f_h']), _ptr(q['f_w']), _ptr(q['w']),
+                _ptr(q['a']), _ptr(q['d']), _ptr(y), _ptr(ms), _DTYPE_CODE[xt.dtype] if xt is not None else _DTYPE_CODE[dtype],
+                _DTYPE_CODE[dtype], *q['dims'], q['strides'], q['ph'], q['pw'], float(gain_h), float(gain_w), *q['conv'], _ptr(ws),
+                ws.numel())
+        return y, ms
+
+    def layer_backward(self, x, lr, f_h, f_w, plan_h, plan_w, gain_h, gain_w, window, dtype, w, a, d, y, dy, padding, want_dx=True,
+                       want_dw=True):
+        """Gradients of ``layer_fprop``'s y in one call: (dx in x's dtype or None, dw or None, da [N T, Cin], sum_hw dy * y
+        [N T, Cout] or None when d is None)."""
+        q = self._layer_args(x, lr, f_h, f_w, plan_h, plan_w, window, dtype, w, a, d, padding)
+        dy = dy.contiguous()
+        if dy.dtype != dtype or tuple(dy.shape) != q['out'] or dy.device != lr.device:
+            raise RuntimeError(f'sres_layer_backward: dy must be a {dtype} tensor of shape {list(q["out"])}')
+        xt = q['x']
+        dx = torch.empty_like(xt) if (want_dx and xt is not None) else None
+        dw = torch.empty_like(q['w']) if want_dw else None
+        da = torch.empty(q['a'].shape, dtype=torch.float32, device=lr.device)
+        dyy = None
+        if d is not None:
+            y = y.contiguous()
+            dyy = torch.empty(q['d'].shape, dtype=torch.float32, device=lr.device)
+        ws = _workspace(lr.device, q['need'])
+        _launch('sres_layer_backward', self._lib.lvg_sres_layer_backward, lr, _ptr(xt), _ptr(lr), _ptr(q['f_h']), _ptr(q['f_w']),
+                _ptr(q['w']), _ptr(q['a']), _ptr(q['d']), _ptr(y) if d is not None else None, _ptr(dy), _ptr(dx), _ptr(dw), _ptr(da),
+                _ptr(dyy), _DTYPE_CODE[xt.dtype] if xt is not None else _DTYPE_CODE[dtype], _DTYPE_CODE[dtype], *q['dims'],
+                q['strides'], q['ph'], q['pw'], float(gain_h), float(gain_w), *q['conv'], _ptr(ws), ws.numel())
+        return dx, dw, da, dyy
+
 
 class SresDblockPlugin:
     """The two native layers of a super-res discriminator block (DESIGN.md 7i): ``conv1`` (the 4-tap FIR in the

@@ -31,15 +31,22 @@ def find_classes(targets, name, accept=None, roots=None):
     return found
 
 
-def wrap(cls, method, attr, make):
-    """Replace ``cls.<method>`` by ``make(current)``, unless a wrapper carrying ``attr`` is in the chain below it already.
-    The new wrapper keeps ``current`` as ``wrapper.<attr>`` and ``wrapper.__wrapped__``. Returns the wrapper carrying
-    ``attr``."""
-    fn = getattr(cls, method)
+def find(fn, attr):
+    """The wrapper carrying ``attr`` in the chain that starts at ``fn``, or None."""
     while fn is not None:
         if hasattr(fn, attr):
             return fn
         fn = getattr(fn, '__wrapped__', None)
+    return None
+
+
+def wrap(cls, method, attr, make):
+    """Replace ``cls.<method>`` by ``make(current)``, unless a wrapper carrying ``attr`` is in the chain below it already.
+    The new wrapper keeps ``current`` as ``wrapper.<attr>`` and ``wrapper.__wrapped__``. Returns the wrapper carrying
+    ``attr``."""
+    found = find(getattr(cls, method), attr)
+    if found is not None:
+        return found
     current = getattr(cls, method)
     wrapper = make(current)
     setattr(wrapper, attr, current)

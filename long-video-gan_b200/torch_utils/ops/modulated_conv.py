@@ -69,25 +69,33 @@ class _ModulatedConv(torch.autograd.Function):
     def backward(ctx, dy):
         x, w, a, d, y = ctx.saved_tensors
         padding = ctx.padding
-        nd = x.ndim - 2
         want_dw = ctx.needs_input_grad[1] and not conv_nd._weights_off()
         if not torch.is_grad_enabled():
             dx, dw, da, dyy = _plugin().modconv_backward(x, w, a, d, y, dy, padding, want_dw=want_dw)
             dd = dyy / d if (d is not None and ctx.needs_input_grad[3]) else None
             return (dx if ctx.needs_input_grad[0] else None), dw, (da if ctx.needs_input_grad[2] else None), dd, None
         # differentiable composition (double backward through the generator)
-        dyd = dy if d is None else dy * _bc(d, nd).to(dy.dtype)
-        dx = dw = da = dd = None
-        if ctx.needs_input_grad[0] or ctx.needs_input_grad[2]:
-            dxp = conv_nd._ConvNdDgrad.apply(dyd, w, x.shape, padding, 1, 1)
-            dx = dxp * _bc(a, nd).to(dxp.dtype)
-            da = _spatial_dot(dxp, x, nd)
-        if want_dw:
-            dw = conv_nd._ConvNdWgrad.apply(dyd, x * _bc(a, nd).to(x.dtype), w.shape, padding, 1, 1)
-        if d is not None and ctx.needs_input_grad[3]:
-            z = conv_nd._ConvNd.apply(x * _bc(a, nd).to(x.dtype), w, padding, 1, 1)
-            dd = _spatial_dot(dy, z, nd)
+        dx, dw, da, dd = backward_graph(x, w, a, d, dy, padding, ctx.needs_input_grad[0] or ctx.needs_input_grad[2], want_dw,
+                                        d is not None and ctx.needs_input_grad[3])
         return dx, dw, da, dd, None
+
+
+def backward_graph(x, w, a, d, dy, padding, want_dx_da, want_dw, want_dd):
+    """(dx, dw, da, dd) of y = d * conv(a * x, w) recorded from the differentiable conv_nd Functions and torch ops, so that
+    gradients of any order work (the create_graph=True backward pass); None where not wanted."""
+    nd = x.ndim - 2
+    dyd = dy if d is None else dy * _bc(d, nd).to(dy.dtype)
+    dx = dw = da = dd = None
+    if want_dx_da:
+        dxp = conv_nd._ConvNdDgrad.apply(dyd, w, x.shape, padding, 1, 1)
+        dx = dxp * _bc(a, nd).to(dxp.dtype)
+        da = _spatial_dot(dxp, x, nd)
+    if want_dw:
+        dw = conv_nd._ConvNdWgrad.apply(dyd, x * _bc(a, nd).to(x.dtype), w.shape, padding, 1, 1)
+    if want_dd:
+        z = conv_nd._ConvNd.apply(x * _bc(a, nd).to(x.dtype), w, padding, 1, 1)
+        dd = _spatial_dot(dy, z, nd)
+    return dx, dw, da, dd
 
 
 def modulated_conv(x, w, a, d, padding):
@@ -104,24 +112,41 @@ def _pad_tuple(padding, nd):
 
 # ---------------------------------------------------------------------------------------------------- super-res
 
+def _demodulated(w, s, demodulate):
+    if demodulate:
+        w = w * w.square().mean([1, 2, 3], keepdim=True).rsqrt()
+        s = s * s.square().mean().rsqrt()
+    return w, s
+
+
+def factors2d(w, s, gain, demodulate):
+    """(a [N, Cin, 1], d [N, Cout, 1] or None) of modulated_conv2d from the normalised w and s and the expanded gain."""
+    a = s if gain is None else s * gain
+    d = None
+    if demodulate:
+        d = (s.square() @ w.square().sum(dim=[2, 3]).t() + 1e-8).rsqrt()            # [N, Cout]
+    return a[..., None], None if d is None else d[..., None]
+
+
+def factors(w, s, demodulate=True, input_gain=None):
+    """(w~ (fp32), a, d) of ``modulated_conv2d(x, w, s, demodulate, input_gain=input_gain)``: the convolution it runs is
+    d * conv(a * x, w~.to(x.dtype)) (the same torch ops, so the same autograd graph)."""
+    w, s = _demodulated(w, s, demodulate)
+    gain = None if input_gain is None else input_gain.expand(s.shape[0], s.shape[1])
+    return (w,) + factors2d(w, s, gain, demodulate)
+
 def modulated_conv2d(x, w, s, demodulate=True, padding=0, input_gain=None):
     """generator_sres.modulated_conv2d: x [N, Cin, H, W], w [Cout, Cin, kh, kw], s [N, Cin], input_gain [], [Cin] or
     [N, Cin]; the weight is cast to x's dtype for the convolution."""
     batch_size = int(x.shape[0])
     out_channels, in_channels, kh, kw = w.shape
     assert tuple(x.shape[:2]) == (batch_size, in_channels) and tuple(s.shape) == (batch_size, in_channels)
-    if demodulate:
-        w = w * w.square().mean([1, 2, 3], keepdim=True).rsqrt()
-        s = s * s.square().mean().rsqrt()
+    w, s = _demodulated(w, s, demodulate)
     gain = None if input_gain is None else input_gain.expand(batch_size, in_channels)
     pad = _pad_tuple(padding, 2)
     wx = w.to(x.dtype)
     if _native(x, wx, pad):
-        a = s if gain is None else s * gain
-        d = None
-        if demodulate:
-            d = (s.square() @ w.square().sum(dim=[2, 3]).t() + 1e-8).rsqrt()            # [N, Cout]
-        return modulated_conv(x, wx, a[..., None], None if d is None else d[..., None], pad)
+        return modulated_conv(x, wx, *factors2d(w, s, gain, demodulate), pad)
     # the reference's formulation: per-sample weights, one grouped convolution
     wn = w.unsqueeze(0) * s[:, None, :, None, None]
     if demodulate:

@@ -216,34 +216,54 @@ def applies(G, cond, lr_plans=None):
     return rejection(G, cond, lr_plans) is None
 
 
-def layer_forward(L, g, x_prev, lr, plan, w, force_fp32=False, update_emas=False):
-    """SynthesisLayer.forward with its input ``cat((x_prev, cond), 1).to(dtype)`` from ``cond_concat`` and the magnitude
-    statistic from the same pass. ``g``: the globals of the model module (its ``misc``, ``distributed``,
-    ``modulated_conv2d`` and ``filtered_lrelu``, whatever they are patched to)."""
+def track_magnitude(L, distributed, magnitude_cur):
+    """SynthesisLayer.forward's magnitude EMA update from the layer input's mean square ``magnitude_cur``."""
+    with torch.autograd.profiler.record_function('update_magnitude_ema'):
+        if distributed.get_world_size() > 1:
+            torch.distributed.all_reduce(magnitude_cur)
+            magnitude_cur = magnitude_cur / distributed.get_world_size()
+        L.magnitude_ema.copy_(magnitude_cur.lerp(L.magnitude_ema, L.magnitude_ema_beta))
+
+
+def layer_styles(L, w):
+    """SynthesisLayer.forward's styles (the affine layer, ToRGB's weight gain)."""
+    styles = L.affine(w)
+    if L.is_torgb:
+        weight_gain = 1 / np.sqrt(L.in_channels * (L.conv_kernel ** 2))
+        styles = styles * weight_gain
+    return styles
+
+
+def conv_step(L, g, x_prev, lr, plan, w, dtype, update_emas):
+    """The step of SynthesisLayer.forward from the layer's input to its modulated convolution's output: the input
+    ``cat((x_prev, cond), 1).to(dtype)`` from ``cond_concat`` with the magnitude statistic from the same pass, the
+    magnitude EMA, the styles and ``modulated_conv2d`` (whatever the model module's global is patched to)."""
     misc, distributed = g['misc'], g['distributed']
-    dtype = torch.float16 if (L.use_fp16 and not force_fp32 and lr.device.type == 'cuda') else torch.float32
     x, magnitude_cur = cond_concat(x_prev, lr, plan, dtype, update_emas)
     misc.assert_shape(x, [None, L.in_channels, int(L.in_size[1]), int(L.in_size[0])])
     misc.assert_shape(w, [x.shape[0], L.w_dim])
 
     # Track input magnitude.
     if update_emas:
-        with torch.autograd.profiler.record_function('update_magnitude_ema'):
-            if distributed.get_world_size() > 1:
-                torch.distributed.all_reduce(magnitude_cur)
-                magnitude_cur = magnitude_cur / distributed.get_world_size()
-            L.magnitude_ema.copy_(magnitude_cur.lerp(L.magnitude_ema, L.magnitude_ema_beta))
+        track_magnitude(L, distributed, magnitude_cur)
     input_gain = L.magnitude_ema.rsqrt()
 
     # Execute affine layer.
-    styles = L.affine(w)
-    if L.is_torgb:
-        weight_gain = 1 / np.sqrt(L.in_channels * (L.conv_kernel ** 2))
-        styles = styles * weight_gain
+    styles = layer_styles(L, w)
 
     # Execute modulated conv2d.
-    x = g['modulated_conv2d'](x=x, w=L.weight, s=styles, padding=L.conv_kernel - 1, demodulate=(not L.is_torgb),
-                              input_gain=input_gain)
+    return g['modulated_conv2d'](x=x, w=L.weight, s=styles, padding=L.conv_kernel - 1, demodulate=(not L.is_torgb),
+                                 input_gain=input_gain)
+
+
+def layer_forward(L, g, x_prev, lr, plan, w, force_fp32=False, update_emas=False, step=conv_step):
+    """SynthesisLayer.forward with its input ``cat((x_prev, cond), 1).to(dtype)`` from ``cond_concat`` and the magnitude
+    statistic from the same pass. ``g``: the globals of the model module (its ``misc``, ``distributed``,
+    ``modulated_conv2d`` and ``filtered_lrelu``, whatever they are patched to). ``step``: the part from the input to the
+    modulated convolution's output (``conv_step``; torch_utils/ops/sres_layer.py replaces it by one fused op)."""
+    misc = g['misc']
+    dtype = torch.float16 if (L.use_fp16 and not force_fp32 and lr.device.type == 'cuda') else torch.float32
+    x = step(L, g, x_prev, lr, plan, w, dtype, update_emas)
 
     # Execute bias, filtered leaky ReLU, and clamping.
     gain = 1 if L.is_torgb else np.sqrt(2)
@@ -292,8 +312,11 @@ def generator_forward(G, g, z, cond, truncation_psi=1, truncation_cutoff=None, u
 
 def _forward(orig):
     g = _install.reference_function(orig).__globals__
+    fused = _install.find(orig, 'lvg_sres_layer')          # sres_layer.install's wrapper below this one
 
     def forward(self, z, cond, truncation_psi=1, truncation_cutoff=None, update_emas=False, **synthesis_kwargs):
+        if fused is not None and fused.takes(self, cond):
+            return orig(self, z, cond, truncation_psi, truncation_cutoff, update_emas, **synthesis_kwargs)
         lr_plans = plans(self, cond.size(3), cond.size(4)) if isinstance(cond, torch.Tensor) and cond.ndim == 5 else None
         if lr_plans is None or not applies(self, cond, lr_plans):
             return orig(self, z, cond, truncation_psi, truncation_cutoff, update_emas, **synthesis_kwargs)
@@ -310,8 +333,9 @@ def install(*targets):
     """Make ``Generator.forward`` of generator_sres run ``generator_forward``. ``targets``: the module
     ``model.generator_sres`` or instances holding a ``Generator`` with ``prep_cond``, ``synthesis`` and ``resamples``,
     found by ``_install.find_classes``. Calls outside ``applies`` (CPU tensors, a low-res video that is not fp32 or needs a
-    gradient, other resamplers, longer filters, shapes the kernel rejects) run the original method. Idempotent; the
-    original stays reachable as ``.forward.lvg_sres_cond``. Returns the patched classes."""
+    gradient, other resamplers, longer filters, shapes the kernel rejects) run the original method, and so do calls that a
+    ``sres_layer.install`` wrapper installed below this one takes. Idempotent; the original stays reachable as
+    ``.forward.lvg_sres_cond``. Returns the patched classes."""
     classes = _install.find_classes(targets, 'Generator', _is_generator)
     for cls in classes:
         _install.wrap(cls, 'forward', 'lvg_sres_cond', _forward)
