@@ -28,15 +28,20 @@
 //
 // Roles (384 threads): warp 0 = TMA producer (one lane), warpgroups 1-2 = wgmma consumers, each with its 64 accumulator rows
 // in registers and its own epilogue ([bias, lrelu, gain, clamp] -> NC(T)HW global). Stages hand over through full/empty mbarriers.
+//
+// Host side (conv_engine.cuh): a call is a ConvShape; fprop_job / dgrad_job derive the forward kernel's job from it,
+// plan_igemm tiles a job (host arithmetic only: lvg_convnd_plan reports it) and run_igemm re-tiles and launches; run_wgrad
+// runs the weight gradient; backward_dgrad / backward_wgrad run both gradients of a call, sharing one re-tiling of dy where
+// the tiles agree. Every workspace is carved from a rooms struct whose total the size queries return. The fused ops that
+// drive the engine live in modconv.cu, sres_layer.cu and sres_dblock.cu.
 
 #include <algorithm>
 #include <cuda.h>
 #include <stdlib.h>
-#include <cuda_bf16.h>
 
 #include "common.cuh"
 #include "wgmma.cuh"
-#include "sres_cond.cuh"
+#include "conv_engine.cuh"
 
 namespace lvg {
 // conv_pointwise.cu: streaming fp32 kernels for 1x1x1 convolutions with few channels (HBM-bound; the engine would re-tile and pad)
@@ -46,6 +51,7 @@ int pw_conv(const float* x, const float* w, float* y, int n, int cin, int cout, 
 bool pw_tc_supported(int dtype, int groups, int cin, int cout, int kt, int kh, int kw, int pad_t, int pad_h, int pad_w, int stride, int64_t P);
 int pw_tc_conv(const void* x, const void* w, void* y, int dtype, int n, int ck, int cm, int64_t P, int64_t w_sm, int64_t w_sk, void* workspace,
                int64_t workspace_bytes, cudaStream_t s, const void* res = nullptr, float rscale = 1.f);
+int64_t pw_tc_workspace(int dtype, int ck, int cm);
 }
 
 namespace lvg {
@@ -94,8 +100,6 @@ struct IgemmParams {
 
 // ------------------------------------------------------------------------------------------------ re-tiling passes
 
-__device__ __forceinline__ unsigned short bf16_bits(float v) { return __bfloat16_as_ushort(__float2bfloat16_rn(v)); }
-__device__ __forceinline__ float bf16_val(unsigned short b) { return __uint_as_float((uint32_t)b << 16); }
 
 // NC(T)HW -> X8. One thread = one pixel of one channel block: 8 strided reads (coalesced across the warp), one or two
 // 16-byte writes. SPLIT: fp32 in, bf16 hi blocks [0, cblk) and lo blocks [cblk, 2 cblk) out.
@@ -180,80 +184,6 @@ int pack_act(const void* x, void* x8, int split, int64_t inst, int c, int cblk, 
     return LVG_OK;
 }
 
-// upfirdn2d(x, f, padding = [2, 2, 2, 2]) (up 1, down 1) with a rank-1 4 x 4 filter f = outer(fy, fx), written straight
-// into X8 of the filtered (h + 1) x (w + 1) image: the FIR of conv2d_resample's down-sampling 3x3 path fused into the
-// re-tiling, so the filtered image never exists in NCHW. One CTA = one 8-channel block of one sample and a 32 x 8 tile of
-// filtered pixels: the (8 + 3) x (32 + 3) input window of the 8 channels goes to shared memory once (zeros outside the
-// image and past the last channel), a pass along y and one along x (fp32, taps in order) leave 8 values per thread, and
-// the thread writes its pixel of the block as one 16-byte store (SPLIT: the bf16 hi and lo halves, one store each).
-// gx / gy: the taps oriented for correlation (mirrored unless flip, as upfirdn2d orients them).
-constexpr int kFirTX = 32, kFirTY = 8, kFirPitch = kFirTX + 4;
-
-template <class TIn, bool SPLIT>
-__global__ void __launch_bounds__(256) conv_pack_fir4_kernel(const TIn* __restrict__ x, uint4* __restrict__ y, int c, int cblk, int h, int w,
-                                                              const float* __restrict__ fx, const float* __restrict__ fy, int flip)
-{
-    __shared__ float s_in[8][kFirTY + 3][kFirPitch];
-    __shared__ float s_mid[8][kFirTY][kFirPitch];
-    const int ho = h + 1, wo = w + 1;
-    const int ox0 = blockIdx.x * kFirTX, oy0 = blockIdx.y * kFirTY;
-    const int blk = (int)(blockIdx.z % cblk);
-    const int64_t in = blockIdx.z / cblk;
-    const int c0 = blk * 8;
-    float gx[4], gy[4];
-#pragma unroll
-    for (int k = 0; k < 4; k++) {
-        gx[k] = __ldg(fx + (flip ? k : 3 - k));
-        gy[k] = __ldg(fy + (flip ? k : 3 - k));
-    }
-    const TIn* xs = x + ((int64_t)in * c + c0) * h * w;
-    for (int i = threadIdx.x; i < 8 * (kFirTY + 3) * (kFirTX + 3); i += 256) {
-        const int col = i % (kFirTX + 3), r = (i / (kFirTX + 3)) % (kFirTY + 3), ch = i / ((kFirTX + 3) * (kFirTY + 3));
-        const int iy = oy0 + r - 2, ix = ox0 + col - 2;
-        float v = 0.f;
-        if (c0 + ch < c && iy >= 0 && iy < h && ix >= 0 && ix < w) {
-            if constexpr (SPLIT) v = __ldg(reinterpret_cast<const float*>(xs) + ((int64_t)ch * h + iy) * w + ix);
-            else v = __half2float(__ldg(reinterpret_cast<const __half*>(xs) + ((int64_t)ch * h + iy) * w + ix));
-        }
-        s_in[ch][r][col] = v;
-    }
-    __syncthreads();
-    for (int i = threadIdx.x; i < 8 * kFirTY * (kFirTX + 3); i += 256) {
-        const int col = i % (kFirTX + 3), r = (i / (kFirTX + 3)) % kFirTY, ch = i / ((kFirTX + 3) * kFirTY);
-        float v = 0.f;
-#pragma unroll
-        for (int k = 0; k < 4; k++) v = fmaf(gy[k], s_in[ch][r + k][col], v);
-        s_mid[ch][r][col] = v;
-    }
-    __syncthreads();
-    const int tx = threadIdx.x % kFirTX, ty = threadIdx.x / kFirTX;
-    const int oy = oy0 + ty, ox = ox0 + tx;
-    if (oy >= ho || ox >= wo) return;
-    float v[8];
-#pragma unroll
-    for (int ch = 0; ch < 8; ch++) {
-        float a = 0.f;
-#pragma unroll
-        for (int k = 0; k < 4; k++) a = fmaf(gx[k], s_mid[ch][ty][tx + k], a);
-        v[ch] = a;
-    }
-    const int64_t plane = (int64_t)ho * wo, off = (int64_t)oy * wo + ox;
-    if constexpr (!SPLIT) {
-        alignas(16) __half o[8];
-#pragma unroll
-        for (int ch = 0; ch < 8; ch++) o[ch] = __float2half_rn(v[ch]);
-        y[(in * cblk + blk) * plane + off] = *reinterpret_cast<const uint4*>(o);
-    } else {
-        alignas(16) unsigned short hi[8], lo[8];
-#pragma unroll
-        for (int ch = 0; ch < 8; ch++) {
-            hi[ch] = bf16_bits(v[ch]);
-            lo[ch] = bf16_bits(v[ch] - bf16_val(hi[ch]));
-        }
-        y[(in * 2 * cblk + blk) * plane + off] = *reinterpret_cast<const uint4*>(hi);
-        y[(in * 2 * cblk + cblk + blk) * plane + off] = *reinterpret_cast<const uint4*>(lo);
-    }
-}
 
 // weights -> tile images.  Element (m, k, tap) of the logical A matrix of group g sits at
 //   w[g * gstride + m * sm + k * sk + (flip ? taps-1-tap : tap)]
@@ -611,78 +541,41 @@ int encode_map(CUtensorMap* tm, void* base, int w, int h, int t, int64_t blocks,
     return LVG_OK;
 }
 
-inline int round_up(int a, int b) { return (a + b - 1) / b * b; }
-
 inline int env_flag(const char* name, int dflt)
 {
     const char* e = getenv(name);
     return e ? atoi(e) : dflt;
 }
 
-struct Geometry {
-    int cpad, cblk, nblk, nimg, kc, mt;
-    int m64, a_img;              // 64-row mode, bytes of one weight image
-    int64_t act_bytes, w_bytes;
-};
-
-// K-side geometry for `ck` contraction channels and `cm` output channels per group
-Geometry geometry(int split, int64_t inst, int groups, int ck, int cm, int64_t thw, int taps)
+bool nd_supported(int dtype, int kt, int kh, int kw)
 {
-    Geometry g;
-    g.cpad = round_up(ck, 16);
-    g.cblk = g.cpad / 8;
-    g.nblk = split ? 2 * g.cblk : g.cblk;
-    g.nimg = split ? 2 : 1;
-    g.kc = g.cpad / 16;
-    g.mt = (cm + kBM - 1) / kBM;
-    // at most 64 rows: 64-row weight images (half the A bytes per stage, no all-zero MMA rows)
-    g.m64 = cm <= 64 && env_flag("LVG_CONV_M64", 1) ? 1 : 0;
-    g.a_img = g.m64 ? kATile / 2 : kATile;
-    g.act_bytes = inst * g.nblk * thw * 16;
-    g.w_bytes = (int64_t)groups * g.mt * g.kc * taps * g.nimg * g.a_img;
-    return g;
+    return (dtype == LVG_F16 || dtype == LVG_F32) && kt >= 1 && kh >= 1 && kw >= 1 && kh * kw <= 9 && kt <= 7;
 }
 
-// shared driver of fprop and dgrad: `x` has `ck` channels per group, `y` gets `cm`; logical A[m][k][tap] = w[g*gs + m*sm + k*sk + tap']
-// `dil` > 1: x is given as an xin_h x xin_w image that is placed on every dil-th pixel of the h x wd grid (input gradient of
-// a strided convolution); `ostride` > 1: only every ostride-th output row / column is stored (strided forward convolution).
-// lvg_convnd_plan: run_igemm stops after its tile selection (pure host arithmetic, no CUDA call) and hands the parameters out
-thread_local IgemmParams* g_plan_only = nullptr;
-
-int run_igemm(const void* x, const void* w, void* y, int dtype, int n, int groups, int ck, int cm, int t, int h, int wd, int kt, int kh,
-              int kw, int pad_t, int pad_h, int pad_w, int64_t w_gs, int64_t w_sm, int64_t w_sk, int flip, const float* bias, int act,
-              float alpha, float gain, float clamp, int xin_h, int xin_w, int dil, int ostride, const unsigned char* x8_pre, void* workspace,
-              int64_t workspace_bytes, cudaStream_t s, const float* in_scale = nullptr, const float* out_scale = nullptr)
+Geometry job_geometry(const IgemmJob& j)
 {
-    // `in_scale` [n][ck][t] multiplies x while it is re-tiled (not with x8_pre: the caller re-tiled it), `out_scale`
-    // [n][cm][to] the accumulators in the epilogue (groups == 1: instance = sample)
-    // `x8_pre` != nullptr: x is already re-tiled there (lvg_convnd_backward shares dy8 with the weight gradient); the workspace
-    // then only holds the packed weights
-    const int split = dtype == LVG_F32 ? 1 : 0;
-    const int taps = kt * kh * kw;
-    const int64_t inst = (int64_t)n * groups;
-    const int64_t thw = (int64_t)t * h * wd;
-    const Geometry g = geometry(split, inst, groups, ck, cm, thw, taps);
-    const bool plan_only = g_plan_only != nullptr;
-    LVG_REQUIRE(plan_only || (workspace && workspace_bytes >= (x8_pre ? 0 : g.act_bytes) + g.w_bytes + 256), "convnd: workspace too small");
-    LVG_REQUIRE(plan_only || aligned16(workspace), "convnd: workspace must be 16-byte aligned");
+    return geometry(j.dtype == LVG_F32, (int64_t)j.n * j.groups, j.groups, j.ck, j.cm, (int64_t)j.t * j.h * j.wd, j.kt * j.kh * j.kw);
+}
+
+IgemmRooms igemm_rooms_of(const Geometry& g, bool x8_pre) { return {round256(g.w_bytes), x8_pre ? 0 : g.act_bytes}; }
+
+// The tiling of a job: host arithmetic only (no CUDA call, no pointer dereferenced). lvg_convnd_plan hands it out.
+int plan_igemm(const IgemmJob& j, IgemmParams& p)
+{
+    const int kt = j.kt, kh = j.kh, kw = j.kw, ostride = j.ostride;
+    const int64_t inst = (int64_t)j.n * j.groups;
+    const Geometry g = job_geometry(j);
     LVG_REQUIRE(inst * g.nblk < (1ll << 31), "convnd: too many channel blocks for a tensor map");
-    EncodeTiledFn enc = plan_only ? nullptr : encode_fn();
-    LVG_REQUIRE(plan_only || enc != nullptr, "convnd: cuTensorMapEncodeTiled is not available from this driver");
 
-    unsigned char* wp = reinterpret_cast<unsigned char*>(workspace);
-    unsigned char* x8 = x8_pre ? const_cast<unsigned char*>(x8_pre) : wp + ((g.w_bytes + 127) / 128) * 128;
-
-    IgemmParams p;
     memset(&p, 0, sizeof(p));
-    p.wp = wp; p.y = y; p.bias = bias; p.act = act; p.alpha = alpha; p.gain = gain; p.clamp = clamp; p.out_scale = out_scale;
-    p.out_f32 = split; p.bf16 = split;
-    p.wgroups = groups; p.cout = cm; p.mt = g.mt; p.kc = g.kc; p.nblk = g.nblk;
+    p.y = j.y; p.bias = j.bias; p.act = j.act; p.alpha = j.alpha; p.gain = j.gain; p.clamp = j.clamp; p.out_scale = j.out_scale;
+    p.out_f32 = p.bf16 = j.dtype == LVG_F32 ? 1 : 0;
+    p.wgroups = j.groups; p.cout = j.cm; p.mt = g.mt; p.kc = g.kc; p.nblk = g.nblk;
     p.nimg = g.nimg; p.lo_blk = g.cblk;
     p.m64 = g.m64; p.a_img = g.a_img;
-    p.to = t + 2 * pad_t - kt + 1; p.ho = h + 2 * pad_h - kh + 1; p.wo = wd + 2 * pad_w - kw + 1;
+    p.to = j.t + 2 * j.pad_t - kt + 1; p.ho = j.h + 2 * j.pad_h - kh + 1; p.wo = j.wd + 2 * j.pad_w - kw + 1;
     LVG_REQUIRE(p.to >= 1 && p.ho >= 1 && p.wo >= 1, "convnd: empty output");
-    p.kt = kt; p.kh = kh; p.kw = kw; p.pad_t = pad_t; p.pad_h = pad_h; p.pad_w = pad_w;
+    p.kt = kt; p.kh = kh; p.kw = kw; p.pad_t = j.pad_t; p.pad_h = j.pad_h; p.pad_w = j.pad_w;
     // tile: whole rows (and, for small frames, several frames) up to 256 accumulator columns (the register accumulator of a
     // consumer warpgroup: 128 fp32 registers per thread); wide images are cut into column tiles. LVG_CONV_COLS lowers it.
     const char* cb_env = getenv("LVG_CONV_COLS");
@@ -753,21 +646,92 @@ int run_igemm(const void* x, const void* w, void* y, int dtype, int n, int group
     {
         const int period = kt * ((g.kc + p.ks - 1) / p.ks);
         p.a_resident = 0;
-        if (groups == 1 && g.mt == 1 && period <= p.stages && env_flag("LVG_CONV_RESIDENT_W", 1)) {
+        if (j.groups == 1 && g.mt == 1 && period <= p.stages && env_flag("LVG_CONV_RESIDENT_W", 1)) {
             p.stages = p.stages / period * period;
             p.a_resident = 1;
         }
     }
     p.y_cs = (int64_t)p.to * p.hos * p.wos;
     p.total_tiles = (int64_t)p.tiles_x * p.tiles_y * p.tiles_t * g.mt * inst;
+    return LVG_OK;
+}
 
-    if (plan_only) { *g_plan_only = p; return LVG_OK; }
+}  // namespace
+
+bool ConvShape::tileable() const { return nd_supported(dtype, kt, kh, kw) && n >= 1 && groups >= 1; }
+bool ConvShape::fprop_ok() const { return tileable() && pad_t >= 0 && pad_h >= 0 && pad_w >= 0 && stride >= 1 && stride <= 4; }
+bool ConvShape::dgrad_ok() const { return fprop_ok() && pad_t <= kt - 1 && pad_h <= kh - 1 && pad_w <= kw - 1; }
+bool ConvShape::wgrad_ok() const { return fprop_ok() && kw <= 3 && !empty() && wo() <= 4 * (128 - kw + 1); }
+
+Geometry geometry(int split, int64_t inst, int groups, int ck, int cm, int64_t thw, int taps)
+{
+    Geometry g;
+    g.cpad = round_up(ck, 16);
+    g.cblk = g.cpad / 8;
+    g.nblk = split ? 2 * g.cblk : g.cblk;
+    g.nimg = split ? 2 : 1;
+    g.kc = g.cpad / 16;
+    g.mt = (cm + kBM - 1) / kBM;
+    // at most 64 rows: 64-row weight images (half the A bytes per stage, no all-zero MMA rows)
+    g.m64 = cm <= 64 && env_flag("LVG_CONV_M64", 1) ? 1 : 0;
+    g.a_img = g.m64 ? kATile / 2 : kATile;
+    g.act_bytes = inst * g.nblk * thw * 16;
+    g.w_bytes = (int64_t)groups * g.mt * g.kc * taps * g.nimg * g.a_img;
+    return g;
+}
+
+IgemmJob fprop_job(const ConvShape& s, const void* x, const void* w, void* y)
+{
+    IgemmJob j = {};
+    j.x = x; j.xin_h = s.h; j.xin_w = s.wd; j.dil = 1;
+    j.dtype = s.dtype; j.n = s.n; j.groups = s.groups; j.ck = s.cin; j.cm = s.cout;
+    j.t = s.t; j.h = s.h; j.wd = s.wd; j.kt = s.kt; j.kh = s.kh; j.kw = s.kw; j.pad_t = s.pad_t; j.pad_h = s.pad_h; j.pad_w = s.pad_w;
+    j.w = w; j.gs = (int64_t)s.cout * s.cin * s.taps(); j.sm = (int64_t)s.cin * s.taps(); j.sk = s.taps(); j.flip = 0;
+    j.y = y; j.gain = 1.f; j.clamp = -1.f;
+    j.ostride = s.stride;
+    return j;
+}
+
+// The input gradient as a forward convolution: dy (to x ho x wo, cout channels; for a strided convolution dy is spread
+// over every stride-th pixel of that grid) with the channel-transposed, mirrored weights, padding k - 1 - pad.
+IgemmJob dgrad_job(const ConvShape& s, const void* dy, const void* w, void* dx)
+{
+    IgemmJob j = {};
+    j.x = dy; j.xin_h = s.hos(); j.xin_w = s.wos(); j.dil = s.stride;
+    j.dtype = s.dtype; j.n = s.n; j.groups = s.groups; j.ck = s.cout; j.cm = s.cin;
+    j.t = s.to(); j.h = s.ho(); j.wd = s.wo(); j.kt = s.kt; j.kh = s.kh; j.kw = s.kw;
+    j.pad_t = s.kt - 1 - s.pad_t; j.pad_h = s.kh - 1 - s.pad_h; j.pad_w = s.kw - 1 - s.pad_w;
+    j.w = w; j.gs = (int64_t)s.cout * s.cin * s.taps(); j.sm = s.taps(); j.sk = (int64_t)s.cin * s.taps(); j.flip = 1;
+    j.y = dx; j.gain = 1.f; j.clamp = -1.f;
+    j.ostride = 1;
+    return j;
+}
+
+IgemmRooms igemm_rooms(const IgemmJob& j) { return igemm_rooms_of(job_geometry(j), j.x8_pre != nullptr); }
+
+// plan, re-tile the operands (x unless pre-tiled, the weights always) into the workspace, launch
+int run_igemm(const IgemmJob& j, void* workspace, int64_t workspace_bytes, cudaStream_t s)
+{
+    IgemmParams p;
+    const int prc = plan_igemm(j, p);
+    if (prc) return prc;
+    const int split = j.dtype == LVG_F32 ? 1 : 0;
+    const int taps = j.kt * j.kh * j.kw;
+    const int64_t inst = (int64_t)j.n * j.groups;
+    const Geometry g = job_geometry(j);
+    const IgemmRooms r = igemm_rooms_of(g, j.x8_pre != nullptr);
+    LVG_REQUIRE(workspace && workspace_bytes >= r.total(), "convnd: workspace too small");
+    LVG_REQUIRE(aligned16(workspace), "convnd: workspace must be 16-byte aligned");
+    LVG_REQUIRE(encode_fn() != nullptr, "convnd: cuTensorMapEncodeTiled is not available from this driver");
+    unsigned char* wp = reinterpret_cast<unsigned char*>(workspace);
+    unsigned char* x8 = j.x8_pre ? const_cast<unsigned char*>(j.x8_pre) : wp + r.wp;
+    p.wp = wp;
 
     // re-tile the operands
     {
-        const int rc = x8_pre ? LVG_OK : pack_act(x, x8, split, inst, ck, g.cblk, t, xin_h, xin_w, h, wd, dil, s, in_scale);
+        const int rc = j.x8_pre ? LVG_OK : pack_act(j.x, x8, split, inst, j.ck, g.cblk, j.t, j.xin_h, j.xin_w, j.h, j.wd, j.dil, s, j.in_scale);
         if (rc) return rc;
-        const int64_t wblocks = (int64_t)groups * g.mt * g.kc;
+        const int64_t wblocks = (int64_t)j.groups * g.mt * g.kc;
         LVG_REQUIRE(wblocks < (1ll << 31), "convnd: too many weight tiles");
         // rows of m per pass: <= ~64 KB of staging (16 * rows * taps elements either way)
         const int es = split ? 4 : 2;
@@ -775,7 +739,7 @@ int run_igemm(const void* x, const void* w, void* y, int dtype, int n, int group
         int rpp = (int)((64 * 1024) / (16 * taps * es + 16)) / 8 * 8;
         if (rpp > img_rows) rpp = img_rows;
         if (rpp < 8) rpp = 8;
-        const bool mrows = w_sk < w_sm;
+        const bool mrows = j.sk < j.sm;
         const int run_el = mrows ? 16 * taps : rpp * taps;
         const int pitch = ((run_el * es + 2 + 3) / 4) | 1;
         const int max_runs = mrows ? rpp : 16;
@@ -791,10 +755,12 @@ int run_igemm(const void* x, const void* w, void* y, int dtype, int n, int group
         const dim3 wgrid((unsigned)wblocks, (unsigned)chunks);
         if (split) {
             LVG_CUDA(cudaFuncSetAttribute(conv_pack_w_kernel<float, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsm));
-            conv_pack_w_kernel<float, true><<<wgrid, 256, wsm, s>>>((const float*)w, wp, cm, ck, g.cpad, taps, w_gs, w_sm, w_sk, flip, g.mt, g.kc, rpp, rows_per_cta, img_rows);
+            conv_pack_w_kernel<float, true><<<wgrid, 256, wsm, s>>>((const float*)j.w, wp, j.cm, j.ck, g.cpad, taps, j.gs, j.sm, j.sk, j.flip, g.mt,
+                                                                    g.kc, rpp, rows_per_cta, img_rows);
         } else {
             LVG_CUDA(cudaFuncSetAttribute(conv_pack_w_kernel<__half, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsm));
-            conv_pack_w_kernel<__half, false><<<wgrid, 256, wsm, s>>>((const __half*)w, wp, cm, ck, g.cpad, taps, w_gs, w_sm, w_sk, flip, g.mt, g.kc, rpp, rows_per_cta, img_rows);
+            conv_pack_w_kernel<__half, false><<<wgrid, 256, wsm, s>>>((const __half*)j.w, wp, j.cm, j.ck, g.cpad, taps, j.gs, j.sm, j.sk, j.flip,
+                                                                      g.mt, g.kc, rpp, rows_per_cta, img_rows);
         }
         LVG_LAUNCH_CHECK();
     }
@@ -802,7 +768,8 @@ int run_igemm(const void* x, const void* w, void* y, int dtype, int n, int group
     // tensor map over X8 as 8-byte elements: (2 W, H, T, instance * block)
     CUtensorMap tm;
     {
-        const int rc = encode_map(&tm, x8, wd, h, t, inst * g.nblk, wd, (int64_t)h * wd, thw, p.wtb, p.thb, p.tt, 2);
+        const int rc = encode_map(&tm, x8, j.wd, j.h, j.t, inst * g.nblk, j.wd, (int64_t)j.h * j.wd, (int64_t)j.t * j.h * j.wd, p.wtb, p.thb,
+                                  p.tt, 2);
         if (rc) return rc;
     }
     const size_t smem = (size_t)p.stages * p.stage_bytes + 128;
@@ -816,7 +783,7 @@ int run_igemm(const void* x, const void* w, void* y, int dtype, int n, int group
         {LVG_IGEMM_WIDTHS(false, false), LVG_IGEMM_WIDTHS(true, false)}, {LVG_IGEMM_WIDTHS(false, true), LVG_IGEMM_WIDTHS(true, true)}};
 #undef LVG_IGEMM_WIDTHS
     LVG_REQUIRE(p.ncw % 16 == 0 && p.ncw >= 16 && p.ncw <= 16 * kWidths, "convnd: MMA width %d", p.ncw);
-    void (*kern)(const CUtensorMap, const IgemmParams) = kerns[out_scale != nullptr][split][p.ncw / 16 - 1];
+    void (*kern)(const CUtensorMap, const IgemmParams) = kerns[j.out_scale != nullptr][split][p.ncw / 16 - 1];
     LVG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const char* cta_env = getenv("LVG_CONV_CTAS");          // experiments: fewer persistent CTAs than SMs
     const int max_ctas = cta_env ? atoi(cta_env) : num_sms();
@@ -826,12 +793,6 @@ int run_igemm(const void* x, const void* w, void* y, int dtype, int n, int group
     return LVG_OK;
 }
 
-bool nd_supported(int dtype, int kt, int kh, int kw)
-{
-    return (dtype == LVG_F16 || dtype == LVG_F32) && kt >= 1 && kh >= 1 && kw >= 1 && kh * kw <= 9 && kt <= 7;
-}
-
-}  // namespace
 }  // namespace lvg
 
 using namespace lvg;
@@ -839,16 +800,11 @@ using namespace lvg;
 extern "C" int64_t lvg_convnd_workspace(int dtype, int n, int groups, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw,
                                         int pad_t, int pad_h, int pad_w)
 {
-    if (!nd_supported(dtype, kt, kh, kw) || n < 1 || groups < 1) return -1;
-    const int split = dtype == LVG_F32;
-    const int taps = kt * kh * kw;
-    const int64_t inst = (int64_t)n * groups;
-    const int to = t + 2 * pad_t - kt + 1, ho = h + 2 * pad_h - kh + 1, wo = wd + 2 * pad_w - kw + 1;
-    if (to < 1 || ho < 1 || wo < 1) return -1;
-    const Geometry a = geometry(split, inst, groups, cin, cout, (int64_t)t * h * wd, taps);        // fprop
-    const Geometry b = geometry(split, inst, groups, cout, cin, (int64_t)to * ho * wo, taps);      // dgrad
-    const int64_t fa = a.act_bytes + a.w_bytes, fb = b.act_bytes + b.w_bytes;
-    return (fa > fb ? fa : fb) + 1024;
+    const ConvShape sh = {dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, 1};
+    if (!sh.tileable() || sh.empty()) return -1;
+    // the engine's forward and input gradient, and the pointwise wgmma kernels (which pack their weights here) in both roles
+    return std::max(std::max(igemm_rooms(fprop_job(sh, nullptr, nullptr, nullptr)).total(), igemm_rooms(dgrad_job(sh, nullptr, nullptr, nullptr)).total()),
+                    std::max(pw_tc_workspace(dtype, cin, cout), pw_tc_workspace(dtype, cout, cin)));
 }
 
 extern "C" int lvg_convnd_fprop(const void* x, const void* w, void* y, int dtype, int n, int groups, int cin, int cout, int t, int h, int wd,
@@ -861,14 +817,14 @@ extern "C" int lvg_convnd_fprop(const void* x, const void* w, void* y, int dtype
     if (route == 1) return pw_conv((const float*)x, (const float*)w, (float*)y, n, cin, cout, (int64_t)t * h * wd, cin, 1, (cudaStream_t)stream);
     if (route == 2 && aligned16(x) && aligned16(y))
         return pw_tc_conv(x, w, y, dtype, n, cin, cout, (int64_t)t * h * wd, cin, 1, workspace, workspace_bytes, (cudaStream_t)stream);
-    if (!nd_supported(dtype, kt, kh, kw) || n < 1 || pad_t < 0 || pad_h < 0 || pad_w < 0 || stride < 1 || stride > 4) {
+    const ConvShape sh = {dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, stride};
+    if (!sh.fprop_ok()) {
         set_error("convnd_fprop: outside the tensor-core kernel's envelope");
         return LVG_UNSUPPORTED;
     }
-    const int taps = kt * kh * kw;
-    return run_igemm(x, w, y, dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, (int64_t)cout * cin * taps,
-                     (int64_t)cin * taps, taps, 0, bias, act, alpha, gain, clamp, h, wd, 1, stride, nullptr, workspace, workspace_bytes,
-                     (cudaStream_t)stream);
+    IgemmJob j = fprop_job(sh, x, w, y);
+    j.bias = bias; j.act = act; j.alpha = alpha; j.gain = gain; j.clamp = clamp;
+    return run_igemm(j, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int lvg_convnd_dgrad(const void* dy, const void* w, void* dx, int dtype, int n, int groups, int cin, int cout, int t, int h, int wd,
@@ -880,20 +836,14 @@ extern "C" int lvg_convnd_dgrad(const void* dy, const void* w, void* dx, int dty
     if (route == 1) return pw_conv((const float*)dy, (const float*)w, (float*)dx, n, cout, cin, (int64_t)t * h * wd, 1, cin, (cudaStream_t)stream);
     if (route == 2 && aligned16(dy) && aligned16(dx))
         return pw_tc_conv(dy, w, dx, dtype, n, cout, cin, (int64_t)t * h * wd, 1, cin, workspace, workspace_bytes, (cudaStream_t)stream);
-    if (!nd_supported(dtype, kt, kh, kw) || n < 1 || pad_t < 0 || pad_h < 0 || pad_w < 0 || pad_t > kt - 1 || pad_h > kh - 1 || pad_w > kw - 1 ||
-        stride < 1 || stride > 4) {
+    const ConvShape sh = {dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, stride};
+    if (!sh.dgrad_ok()) {
         set_error("convnd_dgrad: outside the tensor-core kernel's envelope");
         return LVG_UNSUPPORTED;
     }
-    // dx = correlation of dy (to x ho x wo, cout channels; for a strided convolution: dy spread over every stride-th pixel of
-    // that grid) with the channel-transposed, mirrored weights, padding k-1-pad
-    const int taps = kt * kh * kw;
-    const int to = t + 2 * pad_t - kt + 1, ho = h + 2 * pad_h - kh + 1, wo = wd + 2 * pad_w - kw + 1;
-    const int hos = (ho - 1) / stride + 1, wos = (wo - 1) / stride + 1;
-    return run_igemm(dy, w, dx, dtype, n, groups, cout, cin, to, ho, wo, kt, kh, kw, kt - 1 - pad_t, kh - 1 - pad_h, kw - 1 - pad_w,
-                     (int64_t)cout * cin * taps, taps, (int64_t)cin * taps, 1, nullptr, 0, 0.f, 1.f, -1.f, hos, wos, stride, 1, nullptr, workspace,
-                     workspace_bytes, (cudaStream_t)stream);
+    return run_igemm(dgrad_job(sh, dy, w, dx), workspace, workspace_bytes, (cudaStream_t)stream);
 }
+
 
 // =================================================================================================
 // Weight gradient:  dW[g][co][ci][kt][ky][kx] = sum over samples and output pixels of dy[co][pix] * x[ci][pix + tap]
@@ -1073,25 +1023,19 @@ __global__ void __launch_bounds__(256) conv_wgrad_reduce_kernel(const float* __r
     }
 }
 
-struct WgradPlan {
-    int split, cpad_a, cpad_b, nt, ntiles, mt, nsplit;
-    int ablk, khc, mrows;
-    int nseg, seg_w[4], seg_x0[4], ps, rh, stages;
-    int a_stage, b_stage, stage_bytes, tail_bytes;
-    size_t smem;
-    int64_t a_bytes, b_bytes, part_bytes, dw_elems;
-};
-
 // channel padding of the dy8 operand of the weight gradient. cout < 128: only the channel blocks that exist (the same
 // tensor the input gradient reads, so one re-tiling pass serves both; the remaining rows of the 128-row MMA read whatever
 // follows in shared memory and are never stored -- rows of D depend on the same rows of A only). Otherwise whole m-tiles.
 inline int wgrad_cpad_a(int cout) { return (cout < kBM && env_flag("LVG_WGRAD_COMPACT", 1)) ? round_up(cout, 16) : round_up(cout, kBM); }
 
-WgradPlan wgrad_plan(int dtype, int n, int groups, int cin, int cout, int t, int h, int wd, int to, int ho, int wo, int kt, int kh, int kw,
-                     bool fold = true)
+}  // namespace
+
+WgradPlan wgrad_plan(const ConvShape& s, bool fold)
 {
+    const int cin = s.cin, cout = s.cout, kh = s.kh, kw = s.kw;
+    const int to = s.to(), ho = s.ho(), wo = s.wo();
     WgradPlan q;
-    q.split = dtype == LVG_F32;
+    q.split = s.split();
     q.cpad_a = wgrad_cpad_a(cout);
     q.ablk = q.cpad_a < kBM ? q.cpad_a / 8 : 16;
     // rows of the accumulator: with at most 64 output channels one consumer warpgroup (M = 64) does all the work
@@ -1124,10 +1068,10 @@ WgradPlan wgrad_plan(int dtype, int n, int groups, int cin, int cout, int t, int
     q.nt = round_up((q.cpad_b + q.ntiles - 1) / q.ntiles, 32);          // the MMAs take the input channels 32 at a time
     q.cpad_b = q.nt * q.ntiles;
     q.mt = (q.cpad_a + kBM - 1) / kBM;
-    const int64_t inst = (int64_t)n * groups;
+    const int64_t inst = s.inst();
     q.a_bytes = inst * nop * (q.cpad_a / 8) * (int64_t)to * ho * wo * 16;
-    q.b_bytes = inst * nop * (q.cpad_b / 8) * (int64_t)t * h * wd * 16;
-    q.dw_elems = (int64_t)groups * cout * cin * kt * kh * kw;
+    q.b_bytes = inst * nop * (q.cpad_b / 8) * s.thw() * 16;
+    q.dw_elems = (int64_t)s.groups * cout * cin * s.taps();
     // rows per stage: about 80 KB of operands per stage
     q.rh = 1;
     while (q.rh < ho && q.rh < 255 - q.khc && stage_of(q.rh + 1, q.nt) <= 80 * 1024) q.rh++;
@@ -1149,13 +1093,13 @@ WgradPlan wgrad_plan(int dtype, int n, int groups, int cin, int cout, int t, int
     q.smem = (size_t)q.stages * q.stage_bytes + q.tail_bytes + 128;
     // tall folded kernels (7 or 8 tap rows) over wide rows in split precision: even one-row stages of NT = 32 overflow shared
     // memory with the x tile's kh - 1 halo rows -- one CTA per tap row instead
-    if (q.khc > 1 && q.smem > 227 * 1024) return wgrad_plan(dtype, n, groups, cin, cout, t, h, wd, to, ho, wo, kt, kh, kw, false);
+    if (q.khc > 1 && q.smem > 227 * 1024) return wgrad_plan(s, false);
     // Split the pixel range over `nsplit` CTAs per output tile. One CTA per SM is resident, so the kernel runs in waves of
     // num_sms CTAs: choose the split that minimises waves x (stages per CTA + a fixed per-CTA cost of ~4 stages: clearing
     // shared memory, the register -> global epilogue) -- e.g. with 132 SMs and 3 output tiles: 44 splits = 132 CTAs = one
     // wave instead of 64 splits = 192 CTAs = two waves. Partial sums are capped at 256 MB.
-    const int64_t ctas = (int64_t)q.ntiles * (kh / q.khc) * kt * q.mt * groups;
-    const int64_t stages = (int64_t)n * to * q.nseg * ((ho + q.rh - 1) / q.rh);
+    const int64_t ctas = (int64_t)q.ntiles * (kh / q.khc) * s.kt * q.mt * s.groups;
+    const int64_t stages = (int64_t)s.n * to * q.nseg * ((ho + q.rh - 1) / q.rh);
     const int sms = num_sms();
     int64_t cap = 160;
     if (cap > stages) cap = stages;
@@ -1175,6 +1119,8 @@ WgradPlan wgrad_plan(int dtype, int n, int groups, int cin, int cout, int t, int
     q.part_bytes = q.nsplit > 1 ? q.nsplit * q.dw_elems * 4 : 0;
     return q;
 }
+
+namespace {
 
 // The (taps per CTA, NT) pairs wgrad_plan can return: NT a multiple of 32 with taps * NT <= 256 (kw <= 3, and kh * kw <= 8
 // when the tap rows are folded), NT <= 128 with split operands. nullptr for anything else.
@@ -1212,37 +1158,41 @@ WgradKernel wgrad_kernel_of(int taps, int nt)
 }
 WgradKernel wgrad_kernel(int split, int taps, int nt) { return split ? wgrad_kernel_of<true>(taps, nt) : wgrad_kernel_of<false>(taps, nt); }
 
-// the weight-gradient launch; `dy8_pre` != nullptr: dy is already re-tiled (the tensor the input gradient of the same call read)
-int run_wgrad(const void* x, const void* dy, void* dw, int dtype, int n, int groups, int cin, int cout, int t, int h, int wd, int kt, int kh,
-              int kw, int pad_t, int pad_h, int pad_w, int stride, const unsigned char* dy8_pre, void* workspace, int64_t workspace_bytes,
-              cudaStream_t s, const float* x_scale = nullptr, const float* dy_scale = nullptr, const unsigned char* x8_pre = nullptr)
+// the tiles of dy and x agree (cout < 128 or a multiple of 128: every layer of the networks), so one re-tiling of dy can
+// serve the input gradient and the weight gradient
+bool dy8_tiles_agree(const ConvShape& s) { return wgrad_cpad_a(s.cout) == round_up(s.cout, 16); }
+
+}  // namespace
+
+WgradRooms wgrad_rooms(const WgradPlan& q, bool dy8_pre) { return {dy8_pre ? 0 : round256(q.a_bytes), round256(q.b_bytes), q.part_bytes}; }
+
+int run_wgrad(const ConvShape& sh, const void* x, const void* dy, void* dw, const WgradInputs& in, void* workspace, int64_t workspace_bytes,
+              cudaStream_t s)
 {
-    // `x8_pre` != nullptr: x is already re-tiled there, with cpad_b / 8 blocks (conv_pack_fir4_kernel: the filtered image of
-    // a super-res discriminator block); x is not read
-    const int to = t + 2 * pad_t - kt + 1, ho = h + 2 * pad_h - kh + 1, wo = wd + 2 * pad_w - kw + 1;
-    const WgradPlan q = wgrad_plan(dtype, n, groups, cin, cout, t, h, wd, to, ho, wo, kt, kh, kw);
-    const int64_t a_room = dy8_pre ? 0 : ((q.a_bytes + 255) / 256) * 256;
-    LVG_REQUIRE(workspace && workspace_bytes >= a_room + q.b_bytes + q.part_bytes + 768, "convnd_wgrad: workspace too small");
+    const int to = sh.to(), ho = sh.ho(), wo = sh.wo();
+    const WgradPlan q = wgrad_plan(sh);
+    const WgradRooms r = wgrad_rooms(q, in.dy8_pre != nullptr);
+    LVG_REQUIRE(workspace && workspace_bytes >= r.total(), "convnd_wgrad: workspace too small");
     LVG_REQUIRE(aligned16(workspace), "convnd_wgrad: workspace must be 16-byte aligned");
-    LVG_REQUIRE(groups <= 65535 && q.mt <= 65535, "convnd_wgrad: too many groups / channel tiles");
-    const int64_t inst = (int64_t)n * groups;
-    unsigned char* x8 = x8_pre ? const_cast<unsigned char*>(x8_pre) : reinterpret_cast<unsigned char*>(workspace) + a_room;
-    unsigned char* dy8 = dy8_pre ? const_cast<unsigned char*>(dy8_pre) : reinterpret_cast<unsigned char*>(workspace);
-    float* part = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(workspace) + a_room + ((q.b_bytes + 255) / 256) * 256);
-    const int64_t thw_a = (int64_t)to * ho * wo, thw_b = (int64_t)t * h * wd;
+    LVG_REQUIRE(sh.groups <= 65535 && q.mt <= 65535, "convnd_wgrad: too many groups / channel tiles");
+    const int64_t inst = sh.inst();
+    unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
+    unsigned char* dy8 = in.dy8_pre ? const_cast<unsigned char*>(in.dy8_pre) : ws;
+    unsigned char* x8 = in.x8_pre ? const_cast<unsigned char*>(in.x8_pre) : ws + r.dy8;
+    float* part = reinterpret_cast<float*>(ws + r.dy8 + r.x8);
+    const int64_t thw_a = (int64_t)to * ho * wo, thw_b = sh.thw();
     {
         // dy of a strided convolution is spread over every stride-th pixel of the stride-1 output grid (zeros between)
-        int rc = dy8_pre ? LVG_OK : pack_act(dy, dy8, q.split, inst, cout, q.cpad_a / 8, to, (ho - 1) / stride + 1, (wo - 1) / stride + 1, ho, wo, stride, s,
-                                             dy_scale);
+        int rc = in.dy8_pre ? LVG_OK : pack_act(dy, dy8, q.split, inst, sh.cout, q.cpad_a / 8, to, sh.hos(), sh.wos(), ho, wo, sh.stride, s, in.dy_scale);
         if (rc) return rc;
-        rc = x8_pre ? LVG_OK : pack_act(x, x8, q.split, inst, cin, q.cpad_b / 8, t, h, wd, h, wd, 1, s, x_scale);   // x_scale [n][cin][t]: x is modulated
+        rc = in.x8_pre ? LVG_OK : pack_act(x, x8, q.split, inst, sh.cin, q.cpad_b / 8, sh.t, sh.h, sh.wd, sh.h, sh.wd, 1, s, in.x_scale);
         if (rc) return rc;
     }
     WgradV2Params p;
     memset(&p, 0, sizeof(p));
     p.out_f32 = q.split; p.bf16 = q.split; p.split = q.split;
-    p.n = n; p.groups = groups; p.cin = cin; p.cout = cout; p.to = to; p.ho = ho;
-    p.kt = kt; p.kh = kh; p.kw = kw; p.pad_t = pad_t; p.pad_h = pad_h; p.pad_w = pad_w;
+    p.n = sh.n; p.groups = sh.groups; p.cin = sh.cin; p.cout = sh.cout; p.to = to; p.ho = ho;
+    p.kt = sh.kt; p.kh = sh.kh; p.kw = sh.kw; p.pad_t = sh.pad_t; p.pad_h = sh.pad_h; p.pad_w = sh.pad_w;
     p.nt = q.nt;
     p.nblk_a = (q.split ? 2 : 1) * (q.cpad_a / 8); p.nblk_b = (q.split ? 2 : 1) * (q.cpad_b / 8);
     p.lo_a = q.cpad_a / 8; p.lo_b = q.cpad_b / 8;
@@ -1265,13 +1215,14 @@ int run_wgrad(const void* x, const void* dy, void* dw, int dtype, int n, int gro
         if (rc) return rc;
     }
     {
-        const int rc = encode_map(&maps.b, x8, wd, h, t, inst * p.nblk_b, wd, (int64_t)h * wd, thw_b, p.ps[0], p.rh + q.khc - 1, 1, q.nt / 8);
+        const int rc = encode_map(&maps.b, x8, sh.wd, sh.h, sh.t, inst * p.nblk_b, sh.wd, (int64_t)sh.h * sh.wd, thw_b, p.ps[0], p.rh + q.khc - 1, 1,
+                                  q.nt / 8);
         if (rc) return rc;
     }
-    void (*const kern)(const WgradMaps, const WgradV2Params) = wgrad_kernel(q.split, q.khc * kw, q.nt);
-    LVG_REQUIRE(kern != nullptr, "convnd_wgrad: no kernel for %d taps x %d columns (split %d)", q.khc * kw, q.nt, q.split);
+    void (*const kern)(const WgradMaps, const WgradV2Params) = wgrad_kernel(q.split, q.khc * sh.kw, q.nt);
+    LVG_REQUIRE(kern != nullptr, "convnd_wgrad: no kernel for %d taps x %d columns (split %d)", q.khc * sh.kw, q.nt, q.split);
     LVG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    dim3 grid((unsigned)(q.ntiles * kt * (kh / q.khc) * q.nsplit), (unsigned)q.mt, (unsigned)groups);
+    dim3 grid((unsigned)(q.ntiles * sh.kt * (sh.kh / q.khc) * q.nsplit), (unsigned)q.mt, (unsigned)sh.groups);
     kern<<<grid, kIgemmThreads, smem, s>>>(maps, p);
     LVG_LAUNCH_CHECK();
     if (q.nsplit > 1) {
@@ -1285,23 +1236,62 @@ int run_wgrad(const void* x, const void* dy, void* dw, int dtype, int n, int gro
     return LVG_OK;
 }
 
-bool wgrad_in_envelope(int dtype, int n, int groups, int t, int h, int wd, int kt, int kh, int kw, int pad_t, int pad_h, int pad_w, int stride)
+// ---- both gradients of one call. dy (times a factor d, for modulated convolutions) is re-tiled ONCE when the tiles of the
+// two gradients agree: the input gradient (forward kernel on dy) and the weight gradient (dy as the M-side operand) read
+// the same channel-block tensor. LVG_CONV_SHARED_DY8=0 re-tiles it for each gradient.
+bool shares_dy8(const ConvShape& s) { return env_flag("LVG_CONV_SHARED_DY8", 1) && dy8_tiles_agree(s); }
+
+BackwardRooms backward_rooms(const ConvShape& s, bool shared)
 {
-    const int to = t + 2 * pad_t - kt + 1, ho = h + 2 * pad_h - kh + 1, wo = wd + 2 * pad_w - kw + 1;
-    return nd_supported(dtype, kt, kh, kw) && n >= 1 && groups >= 1 && kw <= 3 && pad_t >= 0 && pad_h >= 0 && pad_w >= 0 && to >= 1 && ho >= 1 &&
-           wo >= 1 && wo <= 4 * (128 - kw + 1) && stride >= 1 && stride <= 4;
+    const Geometry gd = job_geometry(dgrad_job(s, nullptr, nullptr, nullptr));
+    const WgradRooms wr = wgrad_rooms(wgrad_plan(s), shared);
+    return {shared ? round256(gd.act_bytes) : 0, std::max(igemm_rooms_of(gd, shared).total(), wr.total()), wr.dy8};
 }
 
-}  // namespace
+int64_t backward_workspace(const ConvShape& s)
+{
+    const int64_t sep = backward_rooms(s, false).total();
+    return dy8_tiles_agree(s) ? std::max(sep, backward_rooms(s, true).total()) : sep;
+}
+
+int backward_dgrad(const ConvShape& s, const void* dy, const float* d, const void* w, void* dx, void* workspace, int64_t workspace_bytes,
+                   cudaStream_t st, Backward& b)
+{
+    const bool shared = shares_dy8(s);
+    const BackwardRooms r = backward_rooms(s, shared);
+    LVG_REQUIRE(workspace && aligned16(workspace) && workspace_bytes >= r.total(), "convnd backward: workspace too small or misaligned");
+    unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
+    b.dy8 = shared ? ws : nullptr;
+    b.rest = ws + r.dy8;
+    b.rest_bytes = workspace_bytes - r.dy8;
+    b.x8 = b.rest + r.x8;
+    IgemmJob j = dgrad_job(s, dy, w, dx);
+    if (shared) {
+        const int rc = pack_act(dy, ws, s.split(), s.inst(), s.cout, job_geometry(j).cblk, s.to(), s.hos(), s.wos(), s.ho(), s.wo(), s.stride, st, d);
+        if (rc) return rc;
+        j.x8_pre = ws;
+    } else {
+        j.in_scale = d;
+    }
+    // (stream order: the weight gradient's re-tiling of x overwrites the packed weights only after the input gradient read them)
+    return run_igemm(j, b.rest, b.rest_bytes, st);
+}
+
+int backward_wgrad(const ConvShape& s, const Backward& b, const void* x, const void* dy, const float* d, void* dw, const float* x_scale,
+                   const unsigned char* x8_pre, cudaStream_t st)
+{
+    const WgradInputs in = {b.dy8, x8_pre, x_scale, b.dy8 ? nullptr : d};
+    return run_wgrad(s, x, dy, dw, in, b.rest, b.rest_bytes, st);
+}
+
 }  // namespace lvg
 
 extern "C" int64_t lvg_convnd_wgrad_workspace(int dtype, int n, int groups, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw,
                                               int pad_t, int pad_h, int pad_w)
 {
-    if (!wgrad_in_envelope(dtype, n, groups, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, 1)) return -1;
-    const int to = t + 2 * pad_t - kt + 1, ho = h + 2 * pad_h - kh + 1, wo = wd + 2 * pad_w - kw + 1;
-    const WgradPlan q = wgrad_plan(dtype, n, groups, cin, cout, t, h, wd, to, ho, wo, kt, kh, kw);
-    return q.a_bytes + q.b_bytes + q.part_bytes + 1024;
+    const ConvShape sh = {dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, 1};
+    if (!sh.wgrad_ok()) return -1;
+    return wgrad_rooms(wgrad_plan(sh), false).total();
 }
 
 extern "C" int lvg_convnd_wgrad(const void* x, const void* dy, void* dw, int dtype, int n, int groups, int cin, int cout, int t, int h, int wd,
@@ -1309,12 +1299,12 @@ extern "C" int lvg_convnd_wgrad(const void* x, const void* dy, void* dw, int dty
                                 void* stream)
 {
     LVG_REQUIRE(x && dy && dw, "convnd_wgrad: x, dy, dw must not be NULL");
-    if (!wgrad_in_envelope(dtype, n, groups, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, stride)) {
+    const ConvShape sh = {dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, stride};
+    if (!sh.wgrad_ok()) {
         set_error("convnd_wgrad: outside the tensor-core kernel's envelope");
         return LVG_UNSUPPORTED;
     }
-    return run_wgrad(x, dy, dw, dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, stride, nullptr, workspace, workspace_bytes,
-                     (cudaStream_t)stream);
+    return run_wgrad(sh, x, dy, dw, WgradInputs{}, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 // which kernels a call takes (host arithmetic only): mode 0 forward (`epilogue` != 0: with a bias / activation / gain /
@@ -1324,17 +1314,14 @@ extern "C" int lvg_convnd_wgrad(const void* x, const void* dy, void* dw, int dty
 extern "C" int lvg_convnd_route(int mode, int dtype, int n, int groups, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw, int pad_t,
                                 int pad_h, int pad_w, int stride, int epilogue)
 {
+    const ConvShape sh = {dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, stride};
     if (mode < 0 || mode > 2 || n < 1 || groups < 1) return LVG_UNSUPPORTED;
-    if (mode == 2) return wgrad_in_envelope(dtype, n, groups, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, stride) ? 0 : LVG_UNSUPPORTED;
-    const int64_t P = (int64_t)t * h * wd;
+    if (mode == 2) return sh.wgrad_ok() ? 0 : LVG_UNSUPPORTED;
     if (mode == 1 || !epilogue) {
-        if (pw_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, P)) return 1;
-        if (pw_tc_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, P)) return 2;
+        if (pw_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, sh.thw())) return 1;
+        if (pw_tc_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, sh.thw())) return 2;
     }
-    if (!nd_supported(dtype, kt, kh, kw) || pad_t < 0 || pad_h < 0 || pad_w < 0 || stride < 1 || stride > 4 ||
-        (mode == 1 && (pad_t > kt - 1 || pad_h > kh - 1 || pad_w > kw - 1)))
-        return LVG_UNSUPPORTED;
-    return 0;
+    return (mode == 0 ? sh.fprop_ok() : sh.dgrad_ok()) ? 0 : LVG_UNSUPPORTED;
 }
 
 // the tiling lvg_convnd_fprop (mode 0) / lvg_convnd_dgrad (mode 1) would launch with, as ints (host arithmetic only;
@@ -1344,31 +1331,16 @@ extern "C" int lvg_convnd_plan(int mode, int dtype, int n, int groups, int cin, 
 {
     LVG_REQUIRE(out && out_len >= 48, "convnd_plan: out must hold 48 ints");
     LVG_REQUIRE(mode == 0 || mode == 1, "convnd_plan: mode 0 (forward) or 1 (input gradient)");
-    const int taps = kt * kh * kw;
-    if (!nd_supported(dtype, kt, kh, kw) || n < 1 || groups < 1 || pad_t < 0 || pad_h < 0 || pad_w < 0 || stride < 1 || stride > 4 ||
-        (mode == 1 && (pad_t > kt - 1 || pad_h > kh - 1 || pad_w > kw - 1))) {
+    const ConvShape sh = {dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, stride};
+    if (!(mode == 0 ? sh.fprop_ok() : sh.dgrad_ok())) {
         set_error("convnd_plan: outside the tensor-core kernel's envelope");
         return LVG_UNSUPPORTED;
     }
     for (int i = 0; i < out_len; i++) out[i] = 0;
-    if (pw_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, (int64_t)t * h * wd)) { out[47] = 1; return LVG_OK; }
+    if (pw_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, sh.thw())) { out[47] = 1; return LVG_OK; }
+    if (mode == 1 && sh.empty()) { set_error("convnd_plan: empty output"); return LVG_UNSUPPORTED; }
     IgemmParams p;
-    memset(&p, 0, sizeof(p));
-    void* dummy = reinterpret_cast<void*>(256);          // never dereferenced in plan-only mode
-    g_plan_only = &p;
-    int rc;
-    if (mode == 0) {
-        rc = run_igemm(dummy, dummy, dummy, dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, (int64_t)cout * cin * taps,
-                       (int64_t)cin * taps, taps, 0, nullptr, 0, 0.f, 1.f, -1.f, h, wd, 1, stride, nullptr, nullptr, 0, nullptr);
-    } else {
-        const int to = t + 2 * pad_t - kt + 1, ho = h + 2 * pad_h - kh + 1, wo = wd + 2 * pad_w - kw + 1;
-        if (to < 1 || ho < 1 || wo < 1) { g_plan_only = nullptr; set_error("convnd_plan: empty output"); return LVG_UNSUPPORTED; }
-        const int hos = (ho - 1) / stride + 1, wos = (wo - 1) / stride + 1;
-        rc = run_igemm(dummy, dummy, dummy, dtype, n, groups, cout, cin, to, ho, wo, kt, kh, kw, kt - 1 - pad_t, kh - 1 - pad_h, kw - 1 - pad_w,
-                       (int64_t)cout * cin * taps, taps, (int64_t)cin * taps, 1, nullptr, 0, 0.f, 1.f, -1.f, hos, wos, stride, 1, nullptr, nullptr, 0,
-                       nullptr);
-    }
-    g_plan_only = nullptr;
+    const int rc = plan_igemm(mode == 0 ? fprop_job(sh, nullptr, nullptr, nullptr) : dgrad_job(sh, nullptr, nullptr, nullptr), p);
     if (rc) return rc;
     const int v[48] = {p.wgroups, p.cout, p.mt, p.kc, p.nblk, p.nimg, p.lo_blk, p.to, p.ho, p.wo, p.kt, p.kh, p.kw, p.pad_t, p.pad_h, p.pad_w,
                        p.tt, p.th, p.wt, p.wtb, p.thb, p.frame_px, p.ncols, p.tiles_x, p.tiles_y, p.tiles_t,
@@ -1383,12 +1355,12 @@ extern "C" int lvg_convnd_wgrad_plan(int dtype, int n, int groups, int cin, int 
                                      int pad_h, int pad_w, int* out, int out_len)
 {
     LVG_REQUIRE(out && out_len >= 32, "convnd_wgrad_plan: out must hold 32 ints");
-    if (!wgrad_in_envelope(dtype, n, groups, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, 1)) {
+    const ConvShape sh = {dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, 1};
+    if (!sh.wgrad_ok()) {
         set_error("convnd_wgrad_plan: outside the tensor-core kernel's envelope");
         return LVG_UNSUPPORTED;
     }
-    const int to = t + 2 * pad_t - kt + 1, ho = h + 2 * pad_h - kh + 1, wo = wd + 2 * pad_w - kw + 1;
-    const WgradPlan q = wgrad_plan(dtype, n, groups, cin, cout, t, h, wd, to, ho, wo, kt, kh, kw);
+    const WgradPlan q = wgrad_plan(sh);
     const int v[32] = {q.split, q.cpad_a, q.cpad_b, q.nt, q.ntiles, q.mt, q.nsplit, q.ablk, q.khc, q.nseg, q.ps, q.rh, q.stages, q.a_stage, q.b_stage,
                        q.stage_bytes, q.tail_bytes, (int)q.smem, q.seg_w[0], q.seg_w[1], q.seg_w[2], q.seg_w[3], q.seg_x0[0], q.seg_x0[1], q.seg_x0[2],
                        q.seg_x0[3], 0, q.mrows, 0, 0, 0, 0};
@@ -1396,32 +1368,13 @@ extern "C" int lvg_convnd_wgrad_plan(int dtype, int n, int groups, int cin, int 
     return LVG_OK;
 }
 
-// ---- both gradients of one convolution call. dy is re-tiled ONCE: the input gradient (forward kernel on dy) and the weight
-// gradient (dy as the M-side operand) read the same channel-block tensor whenever their paddings agree (cout < 128 or a
-// multiple of 128: every layer of the networks); otherwise, and for the streaming 1x1x1 kernels, the two entry points above run
-// one after the other. Workspace layout of the shared case: [dy8][packed weights of the input gradient][x8][partial sums].
-namespace lvg {
-namespace {
-bool backward_shares_dy8(int dtype, int n, int groups, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw, int pad_t, int pad_h,
-                         int pad_w, int stride)
-{
-    const int64_t P = (int64_t)t * h * wd;
-    if (!env_flag("LVG_CONV_SHARED_DY8", 1)) return false;
-    if (pw_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, P)) return false;
-    if (pw_tc_supported(dtype, groups, cin, cout, kt, kh, kw, pad_t, pad_h, pad_w, stride, P)) return false;     // reads dy as it is
-    return wgrad_cpad_a(cout) == round_up(cout, 16);
-}
-}  // namespace
-}  // namespace lvg
-
 extern "C" int64_t lvg_convnd_backward_workspace(int dtype, int n, int groups, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw,
                                                  int pad_t, int pad_h, int pad_w)
 {
-    const int64_t a = lvg_convnd_workspace(dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w);
-    const int64_t b = lvg_convnd_wgrad_workspace(dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w);
-    if (a < 0 || b < 0) return -1;
-    // (the shared layout never needs more than the two separate ones together)
-    return a + b + 1024;
+    const ConvShape sh = {dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, 1};
+    if (!sh.wgrad_ok()) return -1;
+    // the engine's backward, or lvg_convnd_dgrad on a pointwise route followed by lvg_convnd_wgrad
+    return std::max(backward_workspace(sh), pw_tc_workspace(dtype, cout, cin));
 }
 
 extern "C" int lvg_convnd_backward(const void* x, const void* dy, const void* w, void* dx, void* dw, int dtype, int n, int groups, int cin, int cout,
@@ -1430,9 +1383,9 @@ extern "C" int lvg_convnd_backward(const void* x, const void* dy, const void* w,
 {
     LVG_REQUIRE(x && dy && w && dx && dw, "convnd_backward: x, dy, w, dx, dw must not be NULL");
     LVG_REQUIRE(workspace && aligned16(workspace), "convnd_backward: workspace must be 16-byte aligned and not NULL");
-    const bool tc_ok = wgrad_in_envelope(dtype, n, groups, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, stride) && pad_t <= kt - 1 && pad_h <= kh - 1 &&
-                       pad_w <= kw - 1;
-    if (!tc_ok || !backward_shares_dy8(dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, stride)) {
+    const ConvShape sh = {dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, stride};
+    // the pointwise kernels read dy as it is: the two entry points one after the other
+    if (!sh.wgrad_ok() || !sh.dgrad_ok() || lvg_convnd_route(1, dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, stride, 0) != 0) {
         const int rc = lvg_convnd_dgrad(dy, w, dx, dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, stride, workspace,
                                         workspace_bytes, stream);
         if (rc) return rc;
@@ -1440,690 +1393,8 @@ extern "C" int lvg_convnd_backward(const void* x, const void* dy, const void* w,
                                 stream);
     }
     cudaStream_t s = (cudaStream_t)stream;
-    const int split = dtype == LVG_F32 ? 1 : 0;
-    const int taps = kt * kh * kw;
-    const int to = t + 2 * pad_t - kt + 1, ho = h + 2 * pad_h - kh + 1, wo = wd + 2 * pad_w - kw + 1;
-    const int hos = (ho - 1) / stride + 1, wos = (wo - 1) / stride + 1;
-    const int64_t inst = (int64_t)n * groups;
-    const Geometry gd = geometry(split, inst, groups, cout, cin, (int64_t)to * ho * wo, taps);      // the input gradient's operands
-    const int64_t dy8_room = ((gd.act_bytes + 255) / 256) * 256;
-    const int64_t wp_room = ((gd.w_bytes + 255) / 256) * 256 + 256;
-    LVG_REQUIRE(workspace_bytes >= dy8_room + wp_room, "convnd_backward: workspace too small");
-    unsigned char* dy8 = reinterpret_cast<unsigned char*>(workspace);
-    unsigned char* rest = dy8 + dy8_room;
-    int rc = pack_act(dy, dy8, split, inst, cout, gd.cblk, to, hos, wos, ho, wo, stride, s);
+    Backward b;
+    const int rc = backward_dgrad(sh, dy, nullptr, w, dx, workspace, workspace_bytes, s, b);
     if (rc) return rc;
-    rc = run_igemm(dy, w, dx, dtype, n, groups, cout, cin, to, ho, wo, kt, kh, kw, kt - 1 - pad_t, kh - 1 - pad_h, kw - 1 - pad_w,
-                   (int64_t)cout * cin * taps, taps, (int64_t)cin * taps, 1, nullptr, 0, 0.f, 1.f, -1.f, hos, wos, stride, 1, dy8, rest, wp_room, s);
-    if (rc) return rc;
-    // (stream order: the weight gradient's re-tiling of x overwrites the packed weights only after the input gradient read them)
-    return run_wgrad(x, dy, dw, dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, stride, dy8, rest,
-                     workspace_bytes - dy8_room, s);
-}
-
-// ---- conv1 of a super-res discriminator block (conv2d_resample with down = 2, a 3x3 kernel and padding 1): the 4-tap FIR
-// with padding 2 runs inside the re-tiling pass (conv_pack_fir4_kernel), the stride-2 convolution and its bias_act epilogue
-// on the engine as lvg_convnd_fprop runs them. Workspace: [packed weights][X8 of the filtered image].
-extern "C" int64_t lvg_sres_dblock_conv1_workspace(int dtype, int n, int cin, int cout, int h, int wd)
-{
-    if ((dtype != LVG_F16 && dtype != LVG_F32) || n < 1 || cin < 1 || cout < 1 || h < 2 || wd < 2) return -1;
-    const int hf = h + 1, wf = wd + 1;
-    const Geometry g = geometry(dtype == LVG_F32, n, 1, cin, cout, (int64_t)hf * wf, 9);
-    if ((int64_t)n * g.cblk > 65535 || (int64_t)n * g.nblk >= (1ll << 31) || wf - 2 > 4 * (128 - 2)) return -1;
-    return ((g.w_bytes + 256 + 255) / 256) * 256 + g.act_bytes + 256;
-}
-
-extern "C" int lvg_sres_dblock_conv1(const void* x, const float* fx, const float* fy, int flip, const void* w, const float* bias, void* y, int dtype,
-                                     int n, int cin, int cout, int h, int wd, int act, float alpha, float gain, float clamp, void* workspace,
-                                     int64_t workspace_bytes, void* stream)
-{
-    LVG_REQUIRE(x && fx && fy && w && y, "sres_dblock_conv1: x, fx, fy, w, y must not be NULL");
-    const int64_t need = lvg_sres_dblock_conv1_workspace(dtype, n, cin, cout, h, wd);
-    if (need < 0) {
-        set_error("sres_dblock_conv1: outside the kernels' envelope");
-        return LVG_UNSUPPORTED;
-    }
-    LVG_REQUIRE(workspace && aligned16(workspace) && workspace_bytes >= need, "sres_dblock_conv1: workspace too small or misaligned");
-    cudaStream_t s = (cudaStream_t)stream;
-    const int split = dtype == LVG_F32;
-    const int hf = h + 1, wf = wd + 1;
-    const Geometry g = geometry(split, n, 1, cin, cout, (int64_t)hf * wf, 9);
-    const int64_t wp_room = ((g.w_bytes + 256 + 255) / 256) * 256;
-    unsigned char* x8 = reinterpret_cast<unsigned char*>(workspace) + wp_room;
-    {
-        const dim3 grid((unsigned)((wf + kFirTX - 1) / kFirTX), (unsigned)((hf + kFirTY - 1) / kFirTY), (unsigned)(n * g.cblk));
-        if (split) conv_pack_fir4_kernel<float, true><<<grid, 256, 0, s>>>((const float*)x, (uint4*)x8, cin, g.cblk, h, wd, fx, fy, flip);
-        else conv_pack_fir4_kernel<__half, false><<<grid, 256, 0, s>>>((const __half*)x, (uint4*)x8, cin, g.cblk, h, wd, fx, fy, flip);
-        LVG_LAUNCH_CHECK();
-    }
-    return run_igemm(x8, w, y, dtype, n, 1, cin, cout, 1, hf, wf, 1, 3, 3, 0, 0, 0, (int64_t)cout * cin * 9, (int64_t)cin * 9, 9, 0, bias, act, alpha,
-                     gain, clamp, hf, wf, 1, 2, x8, workspace, wp_room, s);
-}
-
-// ---- conv1's backward: dhf = the input gradient of the strided convolution (the filtered image's gradient, (h + 1) x (wd + 1),
-// lvg_convnd_dgrad), and dw from the weight-gradient kernel with its B operand re-tiled straight from x by
-// conv_pack_fir4_kernel (the filtered image is recomputed into X8, never into NCHW). Workspace: [X8 of the filtered image]
-// [the larger of the two kernels' workspaces].
-namespace lvg {
-namespace {
-int64_t conv1_bwd_x8_bytes(int dtype, int n, int cin, int cout, int h, int wd)
-{
-    const WgradPlan q = wgrad_plan(dtype, n, 1, cin, cout, 1, h + 1, wd + 1, 1, h - 1, wd - 1, 1, 3, 3);
-    return ((q.b_bytes + 255) / 256) * 256;
-}
-}  // namespace
-}  // namespace lvg
-
-extern "C" int64_t lvg_sres_dblock_conv1_backward_workspace(int dtype, int n, int cin, int cout, int h, int wd)
-{
-    if (lvg_sres_dblock_conv1_workspace(dtype, n, cin, cout, h, wd) < 0) return -1;
-    if (!wgrad_in_envelope(dtype, n, 1, 1, h + 1, wd + 1, 1, 3, 3, 0, 0, 0, 2)) return -1;
-    const int64_t a = lvg_convnd_workspace(dtype, n, 1, cin, cout, 1, h + 1, wd + 1, 1, 3, 3, 0, 0, 0);
-    const int64_t b = lvg_convnd_wgrad_workspace(dtype, n, 1, cin, cout, 1, h + 1, wd + 1, 1, 3, 3, 0, 0, 0);
-    if (a < 0 || b < 0) return -1;
-    return conv1_bwd_x8_bytes(dtype, n, cin, cout, h, wd) + (a > b ? a : b) + 1024;
-}
-
-extern "C" int lvg_sres_dblock_conv1_backward(const void* x, const float* fx, const float* fy, int flip, const void* dy, const void* w, void* dhf,
-                                              void* dw, int dtype, int n, int cin, int cout, int h, int wd, void* workspace, int64_t workspace_bytes,
-                                              void* stream)
-{
-    LVG_REQUIRE(x && fx && fy && dy && w && (dhf || dw), "sres_dblock_conv1_backward: x, fx, fy, dy, w and dhf or dw must not be NULL");
-    const int64_t need = lvg_sres_dblock_conv1_backward_workspace(dtype, n, cin, cout, h, wd);
-    if (need < 0) {
-        set_error("sres_dblock_conv1_backward: outside the kernels' envelope");
-        return LVG_UNSUPPORTED;
-    }
-    LVG_REQUIRE(workspace && aligned16(workspace) && workspace_bytes >= need, "sres_dblock_conv1_backward: workspace too small or misaligned");
-    cudaStream_t s = (cudaStream_t)stream;
-    const int hf = h + 1, wf = wd + 1;
-    const int64_t x8_room = conv1_bwd_x8_bytes(dtype, n, cin, cout, h, wd);
-    unsigned char* x8 = reinterpret_cast<unsigned char*>(workspace);
-    unsigned char* rest = x8 + x8_room;
-    const int64_t rest_bytes = workspace_bytes - x8_room;
-    if (dhf) {
-        const int rc = lvg_convnd_dgrad(dy, w, dhf, dtype, n, 1, cin, cout, 1, hf, wf, 1, 3, 3, 0, 0, 0, 2, rest, rest_bytes, stream);
-        if (rc) return rc;
-    }
-    if (!dw) return LVG_OK;
-    const WgradPlan q = wgrad_plan(dtype, n, 1, cin, cout, 1, hf, wf, 1, hf - 2, wf - 2, 1, 3, 3);
-    const int cblk = q.cpad_b / 8;
-    LVG_REQUIRE((int64_t)n * cblk <= 65535, "sres_dblock_conv1_backward: too many channel blocks");
-    {
-        const dim3 grid((unsigned)((wf + kFirTX - 1) / kFirTX), (unsigned)((hf + kFirTY - 1) / kFirTY), (unsigned)(n * cblk));
-        if (q.split) conv_pack_fir4_kernel<float, true><<<grid, 256, 0, s>>>((const float*)x, (uint4*)x8, cin, cblk, h, wd, fx, fy, flip);
-        else conv_pack_fir4_kernel<__half, false><<<grid, 256, 0, s>>>((const __half*)x, (uint4*)x8, cin, cblk, h, wd, fx, fy, flip);
-        LVG_LAUNCH_CHECK();
-    }
-    return run_wgrad(nullptr, dy, dw, dtype, n, 1, cin, cout, 1, hf, wf, 1, 3, 3, 0, 0, 0, 2, nullptr, rest, rest_bytes, s, nullptr, nullptr, x8);
-}
-
-// =================================================================================================
-// Modulated convolution  y = d (.) conv(a (.) x, w)  with one weight tensor shared by every sample (groups = 1, stride 1):
-// a [n][cin][t] scales x while it is re-tiled (conv_pack_act_kernel), d [n][cout][to] the accumulators in the epilogue
-// (conv_igemm_kernel). The per-sample weights of the reference's grouped formulation (generator_sres.py:44-60) and the
-// modulated activation copies (generator_lres.py:117-123) are never formed.
-// Backward: dy is re-tiled with the factor d for both gradients; dgrad writes dx' = conv^T(d dy, w) into dx, and one
-// streaming pass (modconv_rowdot_kernel) turns it into dx = a dx' while it sums da = sum_hw dx' x. The gradient of d comes
-// from sum_hw dy y (= d sum_hw dy conv(a x, w)), a second pass of the same kernel; the caller divides by d.
-
-namespace lvg {
-namespace {
-
-__device__ __forceinline__ float to_f32(float v) { return v; }
-__device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
-__device__ __forceinline__ void from_f32(float& o, float v) { o = v; }
-__device__ __forceinline__ void from_f32(__half& o, float v) { o = __float2half_rn(v); }
-
-// r[row] = sum_i u[row][i] * v[row][i] over rows of `len` contiguous elements (fp32 accumulation); scale != nullptr:
-// u[row][i] *= scale[row] in place (after it was read). One CTA per row; VEC elements per 16-byte load when rows are aligned.
-template <class T, int VEC>
-__global__ void __launch_bounds__(256) modconv_rowdot_kernel(T* __restrict__ u, const T* __restrict__ v, const float* __restrict__ scale,
-                                                             float* __restrict__ r, int64_t rows, int64_t len)
-{
-    __shared__ float red[8];
-    for (int64_t row = blockIdx.x; row < rows; row += gridDim.x) {
-        T* ur = u + row * len;
-        const T* vr = v + row * len;
-        const float sc = scale != nullptr ? __ldg(scale + row) : 1.f;
-        float acc = 0.f;
-        for (int64_t i = (int64_t)threadIdx.x * VEC; i < len; i += 256 * VEC) {
-            alignas(16) T ue[VEC], ve[VEC];
-            if constexpr (VEC > 1) {
-                *reinterpret_cast<uint4*>(ue) = *reinterpret_cast<const uint4*>(ur + i);
-                *reinterpret_cast<uint4*>(ve) = __ldg(reinterpret_cast<const uint4*>(vr + i));
-            } else {
-                ue[0] = ur[i];
-                ve[0] = vr[i];
-            }
-#pragma unroll
-            for (int j = 0; j < VEC; j++) {
-                const float uf = to_f32(ue[j]);
-                acc += uf * to_f32(ve[j]);
-                from_f32(ue[j], uf * sc);
-            }
-            if (scale != nullptr) {
-                if constexpr (VEC > 1) *reinterpret_cast<uint4*>(ur + i) = *reinterpret_cast<const uint4*>(ue);
-                else ur[i] = ue[0];
-            }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-        if (threadIdx.x % 32 == 0) red[threadIdx.x / 32] = acc;
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            float s = 0.f;
-            for (int k = 0; k < 8; k++) s += red[k];
-            if (r != nullptr) r[row] = s;
-        }
-        __syncthreads();
-    }
-}
-
-int modconv_rowdot(void* u, const void* v, const float* scale, float* r, int dtype, int64_t rows, int64_t len, cudaStream_t s)
-{
-    int64_t blocks = rows;
-    const int64_t cap = (int64_t)num_sms() * 8;
-    if (blocks > cap) blocks = cap;
-    if (blocks < 1) return LVG_OK;
-    const int es = dtype == LVG_F32 ? 4 : 2;
-    const bool vec = aligned16(u) && aligned16(v) && (len * es) % 16 == 0;
-    if (dtype == LVG_F32) {
-        if (vec) modconv_rowdot_kernel<float, 4><<<(unsigned)blocks, 256, 0, s>>>((float*)u, (const float*)v, scale, r, rows, len);
-        else modconv_rowdot_kernel<float, 1><<<(unsigned)blocks, 256, 0, s>>>((float*)u, (const float*)v, scale, r, rows, len);
-    } else {
-        if (vec) modconv_rowdot_kernel<__half, 8><<<(unsigned)blocks, 256, 0, s>>>((__half*)u, (const __half*)v, scale, r, rows, len);
-        else modconv_rowdot_kernel<__half, 1><<<(unsigned)blocks, 256, 0, s>>>((__half*)u, (const __half*)v, scale, r, rows, len);
-    }
-    LVG_LAUNCH_CHECK();
-    return LVG_OK;
-}
-
-// forward and backward run on the engine alone (never the streaming 1x1x1 kernels, which take no factors)
-bool modconv_in_envelope(int dtype, int n, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw, int pad_t, int pad_h, int pad_w)
-{
-    return cin >= 1 && cout >= 1 && pad_t <= kt - 1 && pad_h <= kh - 1 && pad_w <= kw - 1 &&
-           wgrad_in_envelope(dtype, n, 1, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, 1);
-}
-
-inline int64_t round256(int64_t b) { return (b + 255) / 256 * 256; }
-
-}  // namespace
-}  // namespace lvg
-
-extern "C" int64_t lvg_modconv_workspace(int dtype, int n, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw, int pad_t, int pad_h,
-                                         int pad_w)
-{
-    if (!modconv_in_envelope(dtype, n, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w)) return -1;
-    const int split = dtype == LVG_F32;
-    const int taps = kt * kh * kw;
-    const int to = t + 2 * pad_t - kt + 1, ho = h + 2 * pad_h - kh + 1, wo = wd + 2 * pad_w - kw + 1;
-    const Geometry gf = geometry(split, n, 1, cin, cout, (int64_t)t * h * wd, taps);          // forward
-    const Geometry gd = geometry(split, n, 1, cout, cin, (int64_t)to * ho * wo, taps);        // input gradient
-    const WgradPlan q = wgrad_plan(dtype, n, 1, cin, cout, t, h, wd, to, ho, wo, kt, kh, kw);
-    const int64_t sep = std::max(std::max(gf.act_bytes + gf.w_bytes, gd.act_bytes + gd.w_bytes), q.a_bytes + q.b_bytes + q.part_bytes);
-    const int64_t shared = round256(gd.act_bytes) + std::max(round256(gd.w_bytes) + 256, round256(q.b_bytes) + q.part_bytes + 768);
-    return std::max(sep, shared) + 1024;
-}
-
-extern "C" int lvg_modconv_fprop(const void* x, const void* w, const float* a, const float* d, void* y, int dtype, int n, int cin, int cout, int t,
-                                 int h, int wd, int kt, int kh, int kw, int pad_t, int pad_h, int pad_w, void* workspace, int64_t workspace_bytes,
-                                 void* stream)
-{
-    LVG_REQUIRE(x && w && a && y, "modconv_fprop: x, w, a, y must not be NULL");
-    if (!modconv_in_envelope(dtype, n, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w)) {
-        set_error("modconv_fprop: outside the tensor-core kernel's envelope");
-        return LVG_UNSUPPORTED;
-    }
-    const int taps = kt * kh * kw;
-    return run_igemm(x, w, y, dtype, n, 1, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, (int64_t)cout * cin * taps, (int64_t)cin * taps,
-                     taps, 0, nullptr, 0, 0.f, 1.f, -1.f, h, wd, 1, 1, nullptr, workspace, workspace_bytes, (cudaStream_t)stream, a, d);
-}
-
-extern "C" int lvg_modconv_backward(const void* x, const void* w, const float* a, const float* d, const void* y, const void* dy, void* dx, void* dw,
-                                    float* da, float* dyy, int dtype, int n, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw,
-                                    int pad_t, int pad_h, int pad_w, void* workspace, int64_t workspace_bytes, void* stream)
-{
-    LVG_REQUIRE(x && w && a && dy && dx, "modconv_backward: x, w, a, dy, dx must not be NULL");
-    LVG_REQUIRE(!dyy || (y && d), "modconv_backward: sum(dy * y) needs y and d");
-    LVG_REQUIRE(workspace && aligned16(workspace), "modconv_backward: workspace must be 16-byte aligned and not NULL");
-    if (!modconv_in_envelope(dtype, n, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w)) {
-        set_error("modconv_backward: outside the tensor-core kernel's envelope");
-        return LVG_UNSUPPORTED;
-    }
-    cudaStream_t s = (cudaStream_t)stream;
-    const int split = dtype == LVG_F32 ? 1 : 0;
-    const int taps = kt * kh * kw;
-    const int to = t + 2 * pad_t - kt + 1, ho = h + 2 * pad_h - kh + 1, wo = wd + 2 * pad_w - kw + 1;
-    int rc;
-    if (dyy) {
-        rc = modconv_rowdot(const_cast<void*>(dy), y, nullptr, dyy, dtype, (int64_t)n * cout * to, (int64_t)ho * wo, s);
-        if (rc) return rc;
-    }
-    const Geometry gd = geometry(split, n, 1, cout, cin, (int64_t)to * ho * wo, taps);
-    const int64_t w_gs = (int64_t)cout * cin * taps;
-    if (wgrad_cpad_a(cout) == round_up(cout, 16)) {
-        // one re-tiling of d dy serves both gradients (layout as lvg_convnd_backward: [dy8][dgrad weights | x8, partial sums])
-        const int64_t dy8_room = round256(gd.act_bytes);
-        const int64_t wp_room = round256(gd.w_bytes) + 256;
-        LVG_REQUIRE(workspace_bytes >= dy8_room + wp_room, "modconv_backward: workspace too small");
-        unsigned char* dy8 = reinterpret_cast<unsigned char*>(workspace);
-        unsigned char* rest = dy8 + dy8_room;
-        rc = pack_act(dy, dy8, split, n, cout, gd.cblk, to, ho, wo, ho, wo, 1, s, d);
-        if (rc) return rc;
-        rc = run_igemm(dy, w, dx, dtype, n, 1, cout, cin, to, ho, wo, kt, kh, kw, kt - 1 - pad_t, kh - 1 - pad_h, kw - 1 - pad_w, w_gs, taps,
-                       (int64_t)cin * taps, 1, nullptr, 0, 0.f, 1.f, -1.f, ho, wo, 1, 1, dy8, rest, wp_room, s);
-        if (rc) return rc;
-        rc = modconv_rowdot(dx, x, a, da, dtype, (int64_t)n * cin * t, (int64_t)h * wd, s);
-        if (rc) return rc;
-        return dw ? run_wgrad(x, dy, dw, dtype, n, 1, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, 1, dy8, rest, workspace_bytes - dy8_room, s, a)
-                  : LVG_OK;
-    }
-    // output channels that are neither < 128 nor a multiple of 128: the two gradients tile d dy differently, each re-tiles it
-    rc = run_igemm(dy, w, dx, dtype, n, 1, cout, cin, to, ho, wo, kt, kh, kw, kt - 1 - pad_t, kh - 1 - pad_h, kw - 1 - pad_w, w_gs, taps,
-                   (int64_t)cin * taps, 1, nullptr, 0, 0.f, 1.f, -1.f, ho, wo, 1, 1, nullptr, workspace, workspace_bytes, s, d);
-    if (rc) return rc;
-    rc = modconv_rowdot(dx, x, a, da, dtype, (int64_t)n * cin * t, (int64_t)h * wd, s);
-    if (rc) return rc;
-    return dw ? run_wgrad(x, dy, dw, dtype, n, 1, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, 1, nullptr, workspace, workspace_bytes, s, a, d)
-              : LVG_OK;
-}
-
-// =================================================================================================
-// Super-res generator layer  y = d (.) conv(a (.) z, w)  with z = cat(x_prev, cond(lr)) never formed (DESIGN.md 7j): the
-// re-tiling pass (conv_pack_cond_kernel) reads x_prev and evaluates the layer's conditioning from the low-res video by its
-// plan (sres_cond.cuh: the tap tables and both passes of sres_cond_kernel, in the same order), rounds each value to the
-// layer's dtype as lvg_sres_cond does, multiplies it by a and writes X8 as conv_pack_act_kernel does from z: bit for bit
-// the modulated convolution of lvg_sres_cond's z. Channel c < C of a sample is x_prev's channel c, channel C + k window + s
-// the conditioning of low-res channel k at frame t + s; a block of 8 channels may hold both.
-// Backward: dgrad of d dy into all Cin channels (workspace), one streaming pass that dots each row with dtype(x_prev) or
-// the conditioning (materialised for its c_lr window channels only, by lvg_sres_cond) for da and writes dx_prev =
-// x_dtype(dtype(a dx')) for the x_prev channels, and the weight gradient from X8 rebuilt by the same re-tiling pass.
-
-namespace lvg {
-namespace {
-
-constexpr int kCondPackRows = 8;              // output rows per re-tiling CTA (shared memory: 8 channels x rows x low-res row)
-constexpr int kCondPackSmem = 48 * 1024;
-
-struct CondPackParams {
-    const void* x;                            // x_prev [np][c][h][w] (TX), unused when c == 0
-    const float* lr;
-    uint4* y;                                 // X8 [np][nblk][h][w], or nullptr (SQ: only the sums of squares)
-    const float* a;                           // [np][cin]
-    double* part;                             // one sum of squares per CTA (SQ)
-    int64_t s_n, s_c, s_t, s_h, s_w;          // element strides of lr
-    int t, c, cin, window, cblk;
-    int rows, row_tiles;
-    sres::Axis ah, aw;
-};
-
-template <class TX, bool SPLIT, bool SQ>
-__global__ void __launch_bounds__(256) conv_pack_cond_kernel(const CondPackParams p)
-{
-    extern __shared__ __align__(16) unsigned char smem[];
-    const int64_t b = blockIdx.x;
-    const int tile = (int)(b % p.row_tiles);
-    const int blk = (int)((b / p.row_tiles) % p.cblk);
-    const int64_t np = b / p.row_tiles / p.cblk;
-    const int n = (int)(np / p.t), t = (int)(np % p.t);
-    const int c0 = blk * 8;
-    const int r0 = tile * p.rows;
-    const int rows = min(p.rows, p.ah.out - r0);
-    const int wout = p.aw.out, wl = p.aw.len;
-    const int nth = p.ah.nt, ntw = p.aw.nt;
-    // channels j < k0 of the block come from x_prev, k0 <= j < k1 from the conditioning, the rest are padding
-    const int k0 = min(max(p.c - c0, 0), 8), k1 = min(max(p.cin - c0, 0), 8);
-
-    float* inter = reinterpret_cast<float*>(smem);                       // [8][p.rows][wl]
-    float* wh = inter + 8 * p.rows * wl;                                 // [p.rows][nth]
-    float* ww = wh + p.rows * nth;                                       // [wout][ntw]
-    int* sh = reinterpret_cast<int*>(ww + wout * ntw);                   // [p.rows][nth]
-    int* sw = sh + p.rows * nth;                                         // [wout][ntw]
-    if (k0 < k1) {                                                       // uniform over the CTA
-        for (int r = threadIdx.x; r < rows; r += 256) sres::axis_taps(p.ah, r0 + r, sh + r * nth, wh + r * nth);
-        for (int i = threadIdx.x; i < wout; i += 256) sres::axis_taps(p.aw, i, sw + i * ntw, ww + i * ntw);
-        __syncthreads();
-        const int plane = rows * wl;
-        for (int idx = threadIdx.x; idx < (k1 - k0) * plane; idx += 256) {
-            const int j = k0 + idx / plane, r = (idx % plane) / wl, x = idx % wl;
-            const int ch = c0 + j - p.c, k = ch / p.window, s = ch % p.window;
-            const float* __restrict__ L = p.lr + n * p.s_n + k * p.s_c + (int64_t)(t + s) * p.s_t;
-            inter[(j * p.rows + r) * wl + x] = sres::vertical_tap_sum(L, p.s_h, p.s_w, x, wh + r * nth, sh + r * nth, nth);
-        }
-        __syncthreads();
-    }
-
-    const int64_t hw = (int64_t)p.ah.out * wout;
-    const TX* __restrict__ xs = reinterpret_cast<const TX*>(p.x) + (np * p.c + c0) * hw;
-    const float* __restrict__ as = p.a + np * p.cin + c0;
-    const int nblk = SPLIT ? 2 * p.cblk : p.cblk;
-    uint4* __restrict__ yo = p.y + (np * nblk + blk) * hw;
-    float sq = 0.f;
-    const bool store = p.y != nullptr;                                 // nullptr: the statistic alone
-    for (int idx = threadIdx.x; idx < rows * wout; idx += 256) {
-        const int r = idx / wout, i = idx - r * wout;
-        const int64_t pix = (int64_t)(r0 + r) * wout + i;
-        float v[8];
-#pragma unroll
-        for (int j = 0; j < 8; j++) {
-            float f = 0.f;
-            if (j < k0) f = to_acc(__ldg(xs + j * hw + pix));
-            else if (j < k1) f = sres::horizontal_tap_sum(inter + (j * p.rows + r) * wl, ww + i * ntw, sw + i * ntw, ntw);
-            if (SQ) sq += f * f;
-            // the layer input z in the layer's dtype (lvg_sres_cond's rounding), then conv_pack_act_kernel's scaling
-            if constexpr (!SPLIT) f = __half2float(__float2half_rn(f));
-            v[j] = f;
-        }
-        if (!store) continue;
-        if constexpr (!SPLIT) {
-            alignas(16) unsigned short o[8];
-#pragma unroll
-            for (int j = 0; j < 8; j++) o[j] = j < k1 ? __half_as_ushort(__float2half_rn(v[j] * __ldg(as + j))) : (unsigned short)0;
-            yo[pix] = *reinterpret_cast<const uint4*>(o);
-        } else {
-            alignas(16) unsigned short hi[8], lo[8];
-#pragma unroll
-            for (int j = 0; j < 8; j++) {
-                const float f = j < k1 ? v[j] * __ldg(as + j) : 0.f;
-                hi[j] = bf16_bits(f);
-                lo[j] = bf16_bits(f - bf16_val(hi[j]));
-            }
-            yo[pix] = *reinterpret_cast<const uint4*>(hi);
-            yo[(int64_t)p.cblk * hw + pix] = *reinterpret_cast<const uint4*>(lo);
-        }
-    }
-    if (SQ) {
-        __shared__ float swarp[8];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
-        if ((threadIdx.x & 31) == 0) swarp[threadIdx.x >> 5] = sq;
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            double s = 0.0;
-            for (int k = 0; k < 8; k++) s += (double)swarp[k];
-            p.part[blockIdx.x] = s;
-        }
-    }
-}
-
-// mean of the squares: the per-CTA partials summed by one CTA in a fixed order
-__global__ void __launch_bounds__(256) conv_pack_cond_fold_kernel(const double* __restrict__ part, int64_t nparts, double count,
-                                                                  float* __restrict__ mean_sq)
-{
-    __shared__ double s[256];
-    double acc = 0.0;
-    for (int64_t k = threadIdx.x; k < nparts; k += 256) acc += part[k];
-    s[threadIdx.x] = acc;
-    __syncthreads();
-    for (int w = 128; w > 0; w >>= 1) {
-        if (threadIdx.x < w) s[threadIdx.x] += s[threadIdx.x + w];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *mean_sq = (float)(s[0] / count);
-}
-
-template <class T> __device__ __forceinline__ T round_to(float v);
-template <> __device__ __forceinline__ float round_to<float>(float v) { return v; }
-template <> __device__ __forceinline__ __half round_to<__half>(float v) { return __float2half_rn(v); }
-
-// modconv_rowdot_kernel over the rows (sample, channel) of dx' [np][cin][len] (the layer's dtype T) against the layer input
-// z without z: rows c < C read dtype(x_prev) (TX), the others the conditioning [np][cin - C][len] (T). da[row] = sum dx' z
-// in modconv_rowdot_kernel's order; dx (NULL = not wanted) gets x_dtype(dtype(a dx')) for the x_prev rows.
-template <class T, class TX, int VEC>
-__global__ void __launch_bounds__(256) sres_layer_rowdot_kernel(const T* __restrict__ u, const TX* __restrict__ x, const T* __restrict__ cond,
-                                                                const float* __restrict__ a, float* __restrict__ da, TX* __restrict__ dx,
-                                                                int64_t rows, int cin, int c, int64_t len)
-{
-    __shared__ float red[8];
-    for (int64_t row = blockIdx.x; row < rows; row += gridDim.x) {
-        const int64_t np = row / cin;
-        const int ch = (int)(row % cin);
-        const bool from_x = ch < c;
-        const T* ur = u + row * len;
-        const TX* xr = x + (np * c + ch) * len;
-        const T* cr = cond + (np * (cin - c) + (ch - c)) * len;
-        TX* dr = dx + (np * c + ch) * len;
-        const float sc = __ldg(a + row);
-        float acc = 0.f;
-        for (int64_t i = (int64_t)threadIdx.x * VEC; i < len; i += 256 * VEC) {
-            alignas(16) T ue[VEC];
-            if constexpr (VEC > 1) *reinterpret_cast<uint4*>(ue) = __ldg(reinterpret_cast<const uint4*>(ur + i));
-            else ue[0] = ur[i];
-#pragma unroll
-            for (int j = 0; j < VEC; j++) {
-                const float uf = to_f32(ue[j]);
-                const float vf = from_x ? to_f32(round_to<T>(to_f32(__ldg(xr + i + j)))) : to_f32(__ldg(cr + i + j));
-                acc += uf * vf;
-                if (from_x && dx != nullptr) from_f32(dr[i + j], to_f32(round_to<T>(uf * sc)));
-            }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-        if (threadIdx.x % 32 == 0) red[threadIdx.x / 32] = acc;
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            float s = 0.f;
-            for (int k = 0; k < 8; k++) s += red[k];
-            da[row] = s;
-        }
-        __syncthreads();
-    }
-}
-
-// one call of the layer op: the conditioning's shape and plan (as lvg_sres_cond takes them) and the convolution's
-struct SresLayer {
-    int n, t, c, c_lr, window, t_lr, h_lr, w_lr, cin, cout, kh, kw, pad_h, pad_w, dtype;
-    int64_t np, hw;
-    sres::Axis ah, aw;
-    int rows, row_tiles, smem;
-};
-
-bool sres_layer_plan(int dtype, int n, int t, int c, int c_lr, int window, int t_lr, int h_lr, int w_lr, const int* plan_h, const int* plan_w,
-                     int cout, int kh, int kw, int pad_h, int pad_w, SresLayer& L)
-{
-    if (n < 1 || t < 1 || c < 0 || c_lr < 1 || window < 1 || h_lr < 1 || w_lr < 1 || !plan_h || !plan_w) return false;
-    if ((int64_t)t + window - 1 > t_lr || (int64_t)c + (int64_t)c_lr * window > (1 << 20)) return false;
-    if (!sres::read_axis(plan_h, h_lr, L.ah) || !sres::read_axis(plan_w, w_lr, L.aw)) return false;
-    L.n = n; L.t = t; L.c = c; L.c_lr = c_lr; L.window = window; L.t_lr = t_lr; L.h_lr = h_lr; L.w_lr = w_lr;
-    L.cin = c + c_lr * window; L.cout = cout; L.kh = kh; L.kw = kw; L.pad_h = pad_h; L.pad_w = pad_w; L.dtype = dtype;
-    L.np = (int64_t)n * t;
-    L.hw = (int64_t)L.ah.out * L.aw.out;
-    if ((L.np * std::max(L.cin, cout) * L.hw) >> 40) return false;
-    if (!modconv_in_envelope(dtype, (int)std::min<int64_t>(L.np, 1 << 30), L.cin, cout, 1, L.ah.out, L.aw.out, 1, kh, kw, 0, pad_h, pad_w))
-        return false;
-    if (L.np > (1 << 24)) return false;
-    // the conditioning (and its per-call statistic) through lvg_sres_cond must take the same call
-    if (lvg_sres_cond_workspace(n, t, 0, c_lr, window, t_lr, h_lr, w_lr, dtype, plan_h, plan_w) < 0) return false;
-    for (L.rows = std::min(kCondPackRows, L.ah.out); L.rows >= 1; L.rows--) {
-        L.smem = (int)((8ll * L.rows * w_lr + 2ll * L.rows * L.ah.nt + 2ll * L.aw.out * L.aw.nt) * 4);
-        if (L.smem <= kCondPackSmem) break;
-    }
-    if (L.rows < 1) return false;
-    L.row_tiles = (L.ah.out + L.rows - 1) / L.rows;
-    return true;
-}
-
-int64_t sres_layer_pack_ctas(const SresLayer& L, int cblk) { return L.np * cblk * L.row_tiles; }
-
-int sres_layer_pack(const SresLayer& L, const void* x, int x_dtype, const float* lr, const int64_t* st, const float* f_h, float gain_h,
-                    const float* f_w, float gain_w, const float* a, void* x8, int cblk, double* part, cudaStream_t s)
-{
-    CondPackParams p;
-    memset(&p, 0, sizeof(p));
-    p.x = x; p.lr = lr; p.y = (uint4*)x8; p.a = a; p.part = part;
-    p.s_n = st[0]; p.s_c = st[1]; p.s_t = st[2]; p.s_h = st[3]; p.s_w = st[4];
-    p.t = L.t; p.c = L.c; p.cin = L.cin; p.window = L.window; p.cblk = cblk;
-    p.rows = L.rows; p.row_tiles = L.row_tiles;
-    p.ah = L.ah; p.aw = L.aw;
-    p.ah.f = f_h; p.ah.gain = gain_h;
-    p.aw.f = f_w; p.aw.gain = gain_w;
-    const int64_t ctas = sres_layer_pack_ctas(L, cblk);
-    LVG_REQUIRE(ctas < (1ll << 31), "sres_layer: too many re-tiling CTAs");
-    const bool split = L.dtype == LVG_F32, xf32 = x_dtype == LVG_F32, sq = part != nullptr;
-    void (*const kerns[2][2][2])(const CondPackParams) = {
-        {{conv_pack_cond_kernel<__half, false, false>, conv_pack_cond_kernel<__half, false, true>},
-         {conv_pack_cond_kernel<__half, true, false>, conv_pack_cond_kernel<__half, true, true>}},
-        {{conv_pack_cond_kernel<float, false, false>, conv_pack_cond_kernel<float, false, true>},
-         {conv_pack_cond_kernel<float, true, false>, conv_pack_cond_kernel<float, true, true>}}};
-    void (*kern)(const CondPackParams) = kerns[xf32][split][sq];
-    kern<<<(unsigned)ctas, 256, L.smem, s>>>(p);
-    LVG_LAUNCH_CHECK();
-    return LVG_OK;
-}
-
-// workspace of the forward: [X8][packed weights][statistic partials]
-struct SresLayerFwdRooms { int64_t x8, wp, part; };
-SresLayerFwdRooms sres_layer_fwd_rooms(const SresLayer& L)
-{
-    const Geometry g = geometry(L.dtype == LVG_F32, L.np, 1, L.cin, L.cout, L.hw, L.kh * L.kw);
-    return {round256(g.act_bytes), round256(g.w_bytes) + 256, round256(sres_layer_pack_ctas(L, g.cblk) * (int64_t)sizeof(double))};
-}
-
-// workspace of the backward: [d dy re-tiled (shared by both gradients) | -][dx' over all Cin][conditioning][rest: the
-// dgrad weights, then the weight gradient's X8 and partial sums]
-struct SresLayerBwdRooms { bool shared; int64_t dy8, dxp, cond, rest, wp; };
-SresLayerBwdRooms sres_layer_bwd_rooms(const SresLayer& L)
-{
-    const int es = L.dtype == LVG_F32 ? 4 : 2;
-    const int ho = L.ah.out + 2 * L.pad_h - L.kh + 1, wo = L.aw.out + 2 * L.pad_w - L.kw + 1;
-    const Geometry gd = geometry(L.dtype == LVG_F32, L.np, 1, L.cout, L.cin, (int64_t)ho * wo, L.kh * L.kw);
-    const WgradPlan q = wgrad_plan(L.dtype, (int)L.np, 1, L.cin, L.cout, 1, L.ah.out, L.aw.out, 1, ho, wo, 1, L.kh, L.kw);
-    SresLayerBwdRooms r;
-    r.shared = wgrad_cpad_a(L.cout) == round_up(L.cout, 16);
-    r.dy8 = r.shared ? round256(gd.act_bytes) : 0;
-    r.dxp = round256(L.np * L.cin * L.hw * es);
-    r.cond = round256(L.np * (L.cin - L.c) * L.hw * es);
-    r.wp = round256(gd.w_bytes) + 256;
-    const int64_t wg = (r.shared ? 0 : round256(q.a_bytes)) + round256(q.b_bytes) + q.part_bytes + 768;
-    const int64_t dg = r.shared ? r.wp : round256(gd.w_bytes) + gd.act_bytes + 256;
-    r.rest = std::max(wg, dg);
-    return r;
-}
-
-}  // namespace
-}  // namespace lvg
-
-extern "C" int64_t lvg_sres_layer_workspace(int dtype, int n, int t, int c, int c_lr, int window, int t_lr, int h_lr, int w_lr,
-                                            const int* plan_h, const int* plan_w, int cout, int kh, int kw, int pad_h, int pad_w)
-{
-    SresLayer L;
-    if (!sres_layer_plan(dtype, n, t, c, c_lr, window, t_lr, h_lr, w_lr, plan_h, plan_w, cout, kh, kw, pad_h, pad_w, L)) return -1;
-    const SresLayerFwdRooms f = sres_layer_fwd_rooms(L);
-    const SresLayerBwdRooms b = sres_layer_bwd_rooms(L);
-    return std::max(f.x8 + f.wp + f.part, b.dy8 + b.dxp + b.cond + b.rest) + 1024;
-}
-
-extern "C" int lvg_sres_layer_fprop(const void* x, const float* lr, const float* f_h, const float* f_w, const void* w, const float* a,
-                                    const float* d, void* y, float* mean_sq, int x_dtype, int dtype, int n, int t, int c, int c_lr,
-                                    int window, int t_lr, int h_lr, int w_lr, const int64_t* lr_strides, const int* plan_h,
-                                    const int* plan_w, float gain_h, float gain_w, int cout, int kh, int kw, int pad_h, int pad_w,
-                                    void* workspace, int64_t workspace_bytes, void* stream)
-{
-    SresLayer L;
-    if (!sres_layer_plan(dtype, n, t, c, c_lr, window, t_lr, h_lr, w_lr, plan_h, plan_w, cout, kh, kw, pad_h, pad_w, L)) {
-        set_error("sres_layer_fprop: shape, plan or convolution outside the kernels' envelope");
-        return LVG_UNSUPPORTED;
-    }
-    LVG_REQUIRE(x_dtype == LVG_F32 || x_dtype == LVG_F16, "sres_layer_fprop: x_prev is fp32 or fp16");
-    LVG_REQUIRE(lr && lr_strides && (c == 0 || x) && (y ? w && a : mean_sq != nullptr),
-                "sres_layer_fprop: lr, lr_strides, x when c > 0, and w, a, y or (y NULL) mean_sq must not be NULL");
-    LVG_REQUIRE((L.ah.ntaps == 0 || f_h) && (L.aw.ntaps == 0 || f_w), "sres_layer_fprop: a filtered axis needs its filter");
-    LVG_REQUIRE(c == 0 || ((uintptr_t)x % (x_dtype == LVG_F32 ? 4 : 2)) == 0, "sres_layer_fprop: x is not aligned to its element");
-    const SresLayerFwdRooms r = sres_layer_fwd_rooms(L);
-    LVG_REQUIRE(workspace && aligned16(workspace) && workspace_bytes >= r.x8 + r.wp + r.part, "sres_layer_fprop: workspace too small or misaligned");
-    cudaStream_t s = (cudaStream_t)stream;
-    unsigned char* x8 = reinterpret_cast<unsigned char*>(workspace);
-    unsigned char* wp = x8 + r.x8;
-    double* part = mean_sq ? reinterpret_cast<double*>(wp + r.wp) : nullptr;
-    const Geometry g = geometry(dtype == LVG_F32, L.np, 1, L.cin, cout, L.hw, kh * kw);
-    int rc = sres_layer_pack(L, x, x_dtype, lr, lr_strides, f_h, gain_h, f_w, gain_w, a, y ? x8 : nullptr, g.cblk, part, s);
-    if (rc) return rc;
-    if (mean_sq) {
-        conv_pack_cond_fold_kernel<<<1, 256, 0, s>>>(part, sres_layer_pack_ctas(L, g.cblk), (double)L.np * L.cin * (double)L.hw, mean_sq);
-        LVG_LAUNCH_CHECK();
-    }
-    if (!y) return LVG_OK;
-    const int taps = kh * kw;
-    return run_igemm(x8, w, y, dtype, (int)L.np, 1, L.cin, cout, 1, L.ah.out, L.aw.out, 1, kh, kw, 0, pad_h, pad_w, (int64_t)cout * L.cin * taps,
-                     (int64_t)L.cin * taps, taps, 0, nullptr, 0, 0.f, 1.f, -1.f, L.ah.out, L.aw.out, 1, 1, x8, wp, r.wp, s, nullptr, d);
-}
-
-extern "C" int lvg_sres_layer_backward(const void* x, const float* lr, const float* f_h, const float* f_w, const void* w, const float* a,
-                                       const float* d, const void* y, const void* dy, void* dx, void* dw, float* da, float* dyy,
-                                       int x_dtype, int dtype, int n, int t, int c, int c_lr, int window, int t_lr, int h_lr, int w_lr,
-                                       const int64_t* lr_strides, const int* plan_h, const int* plan_w, float gain_h, float gain_w,
-                                       int cout, int kh, int kw, int pad_h, int pad_w, void* workspace, int64_t workspace_bytes,
-                                       void* stream)
-{
-    SresLayer L;
-    if (!sres_layer_plan(dtype, n, t, c, c_lr, window, t_lr, h_lr, w_lr, plan_h, plan_w, cout, kh, kw, pad_h, pad_w, L)) {
-        set_error("sres_layer_backward: shape, plan or convolution outside the kernels' envelope");
-        return LVG_UNSUPPORTED;
-    }
-    LVG_REQUIRE(x_dtype == LVG_F32 || x_dtype == LVG_F16, "sres_layer_backward: x_prev is fp32 or fp16");
-    LVG_REQUIRE(lr && w && a && dy && da && lr_strides && (c == 0 || x), "sres_layer_backward: lr, w, a, dy, da, lr_strides (and x when c > 0) must not be NULL");
-    LVG_REQUIRE(!dyy || (y && d), "sres_layer_backward: sum(dy * y) needs y and d");
-    LVG_REQUIRE((L.ah.ntaps == 0 || f_h) && (L.aw.ntaps == 0 || f_w), "sres_layer_backward: a filtered axis needs its filter");
-    LVG_REQUIRE(c == 0 || ((uintptr_t)x % (x_dtype == LVG_F32 ? 4 : 2)) == 0, "sres_layer_backward: x is not aligned to its element");
-    const SresLayerBwdRooms r = sres_layer_bwd_rooms(L);
-    LVG_REQUIRE(workspace && aligned16(workspace) && workspace_bytes >= r.dy8 + r.dxp + r.cond + r.rest,
-                "sres_layer_backward: workspace too small or misaligned");
-    cudaStream_t s = (cudaStream_t)stream;
-    const int split = dtype == LVG_F32 ? 1 : 0;
-    const int taps = kh * kw;
-    const int h = L.ah.out, wd = L.aw.out, np = (int)L.np;
-    const int ho = h + 2 * pad_h - kh + 1, wo = wd + 2 * pad_w - kw + 1;
-    unsigned char* dy8 = reinterpret_cast<unsigned char*>(workspace);
-    unsigned char* dxp = dy8 + r.dy8;
-    unsigned char* cond = dxp + r.dxp;
-    unsigned char* rest = cond + r.cond;
-    const int64_t rest_bytes = workspace_bytes - (r.dy8 + r.dxp + r.cond);
-    int rc;
-    if (dyy) {
-        rc = modconv_rowdot(const_cast<void*>(dy), y, nullptr, dyy, dtype, (int64_t)np * cout, (int64_t)ho * wo, s);
-        if (rc) return rc;
-    }
-    // dx' = conv^T(d dy, w) over all Cin channels, as lvg_modconv_backward computes it
-    const Geometry gd = geometry(split, np, 1, cout, L.cin, (int64_t)ho * wo, taps);
-    const int64_t w_gs = (int64_t)cout * L.cin * taps;
-    if (r.shared) {
-        rc = pack_act(dy, dy8, split, np, cout, gd.cblk, 1, ho, wo, ho, wo, 1, s, d);
-        if (rc) return rc;
-        rc = run_igemm(dy, w, dxp, dtype, np, 1, cout, L.cin, 1, ho, wo, 1, kh, kw, 0, kh - 1 - pad_h, kw - 1 - pad_w, w_gs, taps,
-                       (int64_t)L.cin * taps, 1, nullptr, 0, 0.f, 1.f, -1.f, ho, wo, 1, 1, dy8, rest, r.wp, s);
-    } else {
-        rc = run_igemm(dy, w, dxp, dtype, np, 1, cout, L.cin, 1, ho, wo, 1, kh, kw, 0, kh - 1 - pad_h, kw - 1 - pad_w, w_gs, taps,
-                       (int64_t)L.cin * taps, 1, nullptr, 0, 0.f, 1.f, -1.f, ho, wo, 1, 1, nullptr, rest, rest_bytes, s, d);
-    }
-    if (rc) return rc;
-    // the conditioning channels of z, as lvg_sres_cond writes them
-    rc = lvg_sres_cond(nullptr, lr, f_h, f_w, cond, nullptr, nullptr, 0, dtype, dtype, n, t, 0, c_lr, window, t_lr, h_lr, w_lr, lr_strides,
-                       plan_h, plan_w, gain_h, gain_w, stream);
-    if (rc) return rc;
-    {
-        const int64_t rows = (int64_t)np * L.cin, len = L.hw;
-        const int64_t blocks = std::min<int64_t>(rows, (int64_t)num_sms() * 8);
-        const bool vec = (len * (split ? 4 : 2)) % 16 == 0;
-#define LVG_SRES_ROWDOT(T, TX, V)                                                                                                  \
-    sres_layer_rowdot_kernel<T, TX, V><<<(unsigned)blocks, 256, 0, s>>>((const T*)dxp, (const TX*)x, (const T*)cond, a, da, (TX*)dx, rows, \
-                                                                         L.cin, c, len)
-        if (split) {
-            if (x_dtype == LVG_F32) { if (vec) LVG_SRES_ROWDOT(float, float, 4); else LVG_SRES_ROWDOT(float, float, 1); }
-            else { if (vec) LVG_SRES_ROWDOT(float, __half, 4); else LVG_SRES_ROWDOT(float, __half, 1); }
-        } else {
-            if (x_dtype == LVG_F32) { if (vec) LVG_SRES_ROWDOT(__half, float, 8); else LVG_SRES_ROWDOT(__half, float, 1); }
-            else { if (vec) LVG_SRES_ROWDOT(__half, __half, 8); else LVG_SRES_ROWDOT(__half, __half, 1); }
-        }
-#undef LVG_SRES_ROWDOT
-        LVG_LAUNCH_CHECK();
-    }
-    if (!dw) return LVG_OK;
-    // dw from X8 of a z rebuilt by the re-tiling pass, in the slot run_wgrad would re-tile x into
-    const WgradPlan q = wgrad_plan(dtype, np, 1, L.cin, cout, 1, h, wd, 1, ho, wo, 1, kh, kw);
-    unsigned char* x8 = r.shared ? rest : rest + round256(q.a_bytes);
-    rc = sres_layer_pack(L, x, x_dtype, lr, lr_strides, f_h, gain_h, f_w, gain_w, a, x8, q.cpad_b / 8, nullptr, s);
-    if (rc) return rc;
-    return run_wgrad(nullptr, dy, dw, dtype, np, 1, L.cin, cout, 1, h, wd, 1, kh, kw, 0, pad_h, pad_w, 1, r.shared ? dy8 : nullptr, rest,
-                     rest_bytes, s, nullptr, r.shared ? nullptr : d, x8);
+    return backward_wgrad(sh, b, x, dy, nullptr, dw, nullptr, nullptr, s);
 }

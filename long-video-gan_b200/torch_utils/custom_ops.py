@@ -538,7 +538,7 @@ class ConvNdPlugin:
         """The shapes the engine plans and runs in every direction (forward, input gradient, weight gradient): fp16 / fp32,
         1-D / 2-D / 3-D, kh * kw <= 9 with kw <= 3, kt <= 7, 0 <= padding <= k - 1, dilation 1, the same stride 1-4 on H and W
         (1 on T and on 1-D tensors), and a stride-1 output width the weight gradient's at most 4 column segments of
-        128 - (kw - 1) pixels cover (wgrad_in_envelope in csrc/conv_igemm.cu)."""
+        128 - (kw - 1) pixels cover (ConvShape::wgrad_ok in csrc/conv_igemm.cu)."""
         if not (dtype in (torch.float16, torch.float32) and len(x_shape) == len(w_shape) and len(x_shape) in (3, 4, 5)):
             return False
         nd = len(x_shape) - 2

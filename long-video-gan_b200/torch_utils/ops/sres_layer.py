@@ -6,7 +6,7 @@ to re-tile it. ``sres_layer`` computes
 
   y = d * conv(a * z, w)        with z never formed
 
-on the convolution engine (csrc/conv_igemm.cu: lvg_sres_layer_fprop / _backward): the re-tiling pass reads x_prev and
+on the convolution engine (csrc/sres_layer.cu: lvg_sres_layer_fprop / _backward): the re-tiling pass reads x_prev and
 evaluates the conditioning from the low-res video by the layer's plan with the same sums as sres_cond's kernel
 (csrc/sres_cond.cuh), so y and every gradient are bit for bit those of ``modulated_conv(cond_concat(...))``. The autograd
 Function saves x_prev, lr, the plan, w, a, d and y, not z; the first-order backward pass is one native call (dx_prev in

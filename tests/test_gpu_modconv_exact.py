@@ -1,5 +1,5 @@
 """Bit-exact checks of the fused modulated convolution y = d * conv(a * x, w) (lvg_modconv_fprop / lvg_modconv_backward,
-csrc/conv_igemm.cu) over its envelope, and of the two wrappers of torch_utils/ops/modulated_conv.py.
+csrc/modconv.cu) over its envelope, and of the two wrappers of torch_utils/ops/modulated_conv.py.
 
 The operands are those of tests/test_gpu_conv_exact.py (sparse small integers; for the fp32 split path also dyadic values
 whose bf16 lo half is not zero) and power-of-two factors a in 2^{-1,0,1}, d in 2^{-2..0}: a * x splits into bf16 halves
@@ -296,12 +296,14 @@ def test_modconv_exact(plug, case, dtype, dyad):
     check_case(plug, case, dtype, dyad)
 
 
-# ---- tiling invariance on a subset: shared / separate backward layout, 64- / 128-row mode, a multi-frame 3-D case
+# ---- tiling invariance on a subset: shared / separate backward layout, 64- / 128-row mode, a multi-frame 3-D case; the
+# engine's switches and LVG_CONV_SHARED_DY8=0, which re-tiles d dy for each gradient where the backward would share it
 KNOB_CASES = [c for c in CASES if c[2] == (0, 1, 1) and c[3].get('width') in ((0, 64), (1, 64), (0, 80))] + \
              [c for c in CASES if c[3].get('multiframe') and c[0][0] == 3]
+MODCONV_KNOBS = KNOBS + [('LVG_CONV_SHARED_DY8', '0')]
 
 
-@pytest.mark.parametrize('knob,value', KNOBS, ids=[f'{k}={v}' for k, v in KNOBS])
+@pytest.mark.parametrize('knob,value', MODCONV_KNOBS, ids=[f'{k}={v}' for k, v in MODCONV_KNOBS])
 @pytest.mark.parametrize('dtype,dyad', [MODES[0], MODES[2]], ids=[MODE_IDS[0], MODE_IDS[2]])
 def test_modconv_tiling_knobs_exact(plug, monkeypatch, knob, value, dtype, dyad):
     monkeypatch.setenv(knob, value)

@@ -1,4 +1,4 @@
-"""The super-res discriminator block op (torch_utils/ops/sres_dblock.py, csrc/conv_igemm.cu conv_pack_fir4_kernel, the
+"""The super-res discriminator block op (torch_utils/ops/sres_dblock.py, csrc/sres_dblock.cu conv_pack_fir4_kernel, the
 residual epilogue of csrc/conv_pw_tc.cu) on the GPU: exact arithmetic of both native layers in fp32 and fp16, guard bands,
 every block shape of the default discriminator at batch 8 against float64 and the composition, CUDA-graph capture, kernel
 names, and the whole installed reference discriminator (tests/sres_dblock_run.py) against the original."""

@@ -1,4 +1,4 @@
-"""The fused super-res layer op (torch_utils/ops/sres_layer.py, lvg_sres_layer_* in csrc/conv_igemm.cu) on the GPU.
+"""The fused super-res layer op (torch_utils/ops/sres_layer.py, lvg_sres_layer_* in csrc/sres_layer.cu) on the GPU.
 
 Per layer, for all 15 layers of the default generator (hr 144 x 256, lr 36 x 64) at N T = 64 and for a layer whose x_prev
 channel count is not a multiple of 8, with fp32 and fp16 x_prev: the output and the gradients of x_prev, w, a and d bit
