@@ -468,6 +468,35 @@ int lvg_sres_layer_backward(const void* x, const float* lr, const float* f_h, co
                             void* stream);
 
 /*
+ * The super-res generator's ToRGB layer in one pass over its input (DESIGN.md 7k), on the CUDA cores:
+ *   y = dtype(clamp(dtype(u) + b, +-clamp)),  u = sum_c w[o][c] r(a[c] z[c])  per pixel, o < cout = 3
+ * with z = cat(x, cond(lr)).to(dtype) as lvg_sres_cond defines it, never stored, and r() the rounding of the convolution
+ * engine's re-tiling pass (fp16 layers: fp16(a z); fp32 layers: a z in fp32); products accumulated in fp32. x, lr, f_h,
+ * f_w, x_dtype, n, t, c, c_lr, window, t_lr, h_lr, w_lr, lr_strides, plan_h, plan_w, gain_h, gain_w: as lvg_sres_cond
+ * (dtype = its z_dtype, the layer's). w [cout][cin] and b [cout] in dtype, cin = c + c_lr window; a fp32 [n t][cin];
+ * y [n t][cout][h_out][w_out] (dtype). clamp >= 0 (infinity: none). mask (NULL = not wanted): [n t][h_out][w_out] bytes,
+ * bit o set where output o was clamped (|dtype(u) + b| > clamp), which the backward needs. One kernel launch.
+ * lvg_sres_torgb_backward, from the forward's mask and dy (dtype, y's shape): dy' = dy where not clamped, else 0;
+ * dx' = dtype(w^T dy') per pixel; dx (NULL = not wanted) = x_dtype(dtype(a dx')) for the x channels; da [n t][cin] (fp32) =
+ * sum over pixels of dx' z; dw [cout][cin] = dtype(sum over samples and pixels of dy' r(a z)) and db [cout] =
+ * dtype(sum dy') (dtype; NULL = not wanted). Per-CTA partial sums in `workspace` (lvg_sres_torgb_workspace bytes), folded
+ * by two more kernels in a fixed order: bitwise reproducible, no atomics. The forward needs no workspace. The size query
+ * returns -1 for anything the kernels do not take (cout != 3, more than 1024 input channels, a conditioning
+ * lvg_sres_cond_workspace rejects, an output wider than 2048 pixels); such calls return LVG_UNSUPPORTED.
+ */
+int64_t lvg_sres_torgb_workspace(int dtype, int n, int t, int c, int c_lr, int window, int t_lr, int h_lr, int w_lr,
+                                 const int* plan_h, const int* plan_w, int cout);
+int lvg_sres_torgb_fprop(const void* x, const float* lr, const float* f_h, const float* f_w, const void* w, const float* a,
+                         const void* b, void* y, unsigned char* mask, int x_dtype, int dtype, int n, int t, int c, int c_lr,
+                         int window, int t_lr, int h_lr, int w_lr, const int64_t* lr_strides, const int* plan_h,
+                         const int* plan_w, float gain_h, float gain_w, int cout, float clamp, void* stream);
+int lvg_sres_torgb_backward(const void* x, const float* lr, const float* f_h, const float* f_w, const void* w, const float* a,
+                            const unsigned char* mask, const void* dy, void* dx, void* dw, float* da, void* db, int x_dtype,
+                            int dtype, int n, int t, int c, int c_lr, int window, int t_lr, int h_lr, int w_lr,
+                            const int64_t* lr_strides, const int* plan_h, const int* plan_w, float gain_h, float gain_w,
+                            int cout, void* workspace, int64_t workspace_bytes, void* stream);
+
+/*
  * Layers of a super-res discriminator block (discriminator_sres.py DiscriminatorBlock, architecture 'resnet'; DESIGN.md 7i).
  *
  * lvg_sres_dblock_conv1: conv1, y = bias_act(conv2d(upfirdn2d(x, f, padding 2), w, stride 2), bias, act, alpha, gain,

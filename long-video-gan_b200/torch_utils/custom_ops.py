@@ -98,6 +98,10 @@ _SIGNATURES = {
                              + [_c_void_p, _c_i64, _c_void_p]),
     'lvg_sres_layer_backward': (_c_int, [_c_void_p] * 13 + [_c_int] * 10 + [_c_void_p] * 3 + [_c_float] * 2 + [_c_int] * 5
                                 + [_c_void_p, _c_i64, _c_void_p]),
+    'lvg_sres_torgb_workspace': (_c_i64, [_c_int] * 9 + [_c_void_p] * 2 + [_c_int]),
+    'lvg_sres_torgb_fprop': (_c_int, [_c_void_p] * 9 + [_c_int] * 10 + [_c_void_p] * 3 + [_c_float] * 2 + [_c_int, _c_float, _c_void_p]),
+    'lvg_sres_torgb_backward': (_c_int, [_c_void_p] * 12 + [_c_int] * 10 + [_c_void_p] * 3 + [_c_float] * 2 + [_c_int]
+                                + [_c_void_p, _c_i64, _c_void_p]),
     'lvg_sres_dblock_conv1_workspace': (_c_i64, [_c_int] * 6),
     'lvg_sres_dblock_conv1': (_c_int, [_c_void_p] * 3 + [_c_int] + [_c_void_p] * 3 + [_c_int] * 7 + [_c_float] * 3 + [_c_void_p, _c_i64, _c_void_p]),
     'lvg_sres_dblock_conv1_backward_workspace': (_c_i64, [_c_int] * 6),
@@ -1063,6 +1067,80 @@ class SresCondPlugin:
                 _ptr(dyy), _DTYPE_CODE[xt.dtype] if xt is not None else _DTYPE_CODE[dtype], _DTYPE_CODE[dtype], *q['dims'],
                 q['strides'], q['ph'], q['pw'], float(gain_h), float(gain_w), *q['conv'], _ptr(ws), ws.numel())
         return dx, dw, da, dyy
+
+    # ---- the ToRGB layer in one pass over its input (lvg_sres_torgb_*)
+
+    def torgb_workspace(self, n, t, c, c_lr, window, t_lr, h_lr, w_lr, dtype, plan_h, plan_w, cout):
+        """Workspace bytes of lvg_sres_torgb_backward, or -1 where the kernels do not take the call."""
+        return int(self._lib.lvg_sres_torgb_workspace(_DTYPE_CODE.get(dtype, -1), n, t, c, c_lr, window, t_lr, h_lr, w_lr,
+                                                      self._plan(plan_h), self._plan(plan_w), cout))
+
+    def _torgb_args(self, x, lr, f_h, f_w, plan_h, plan_w, window, dtype, w, a, b):
+        """Checked arguments shared by torgb_fprop and torgb_backward."""
+        if not lr.is_cuda or lr.dtype != torch.float32 or lr.ndim != 5:
+            raise RuntimeError('sres_torgb: lr must be a 5-D float32 CUDA tensor')
+        n, c_lr, t_lr, h_lr, w_lr = lr.shape
+        t = t_lr - window + 1
+        h, wd = int(plan_h[0]), int(plan_w[0])
+        if (x is None or x.dtype not in (torch.float16, torch.float32) or x.device != lr.device or x.ndim != 4
+                or x.shape[0] != n * t or tuple(x.shape[2:]) != (h, wd)):
+            raise RuntimeError(f'sres_torgb: x must be a float16 / float32 [{n * t}, C, {h}, {wd}] tensor on the device of lr')
+        c = x.shape[1]
+        cin = c + c_lr * window
+        if w.dtype != dtype or w.ndim != 2 or w.shape[1] != cin or w.device != lr.device:
+            raise RuntimeError(f'sres_torgb: w must be a {dtype} [Cout, {cin}] tensor on the device of lr')
+        cout = int(w.shape[0])
+        if a.dtype != torch.float32 or a.numel() != n * t * cin or a.device != lr.device:
+            raise RuntimeError(f'sres_torgb: a must be a float32 [{n * t}, {cin}] tensor on the device of lr')
+        if b.dtype != dtype or tuple(b.shape) != (cout,) or b.device != lr.device:
+            raise RuntimeError(f'sres_torgb: b must be a {dtype} [{cout}] tensor on the device of lr')
+        for f, q in ((f_h, plan_h), (f_w, plan_w)):
+            k = int(q[9])
+            if (k == 0) != (f is None) or f is not None and (f.dtype != torch.float32 or f.numel() != k or f.device != lr.device):
+                raise RuntimeError(f'sres_torgb: a filter of {k} float32 taps on the device of lr (None for an identity axis)')
+        ph, pw = self._plan(plan_h), self._plan(plan_w)
+        dims = (n, t, c, c_lr, window, t_lr, h_lr, w_lr)
+        need = int(self._lib.lvg_sres_torgb_workspace(_DTYPE_CODE[dtype], *dims, ph, pw, cout))
+        if need < 0:
+            raise RuntimeError(f'sres_torgb: no kernel for {list(lr.shape)}, window {window}, C {c}, w {list(w.shape)}')
+        return dict(x=x.contiguous(), f_h=None if f_h is None else f_h.contiguous(), f_w=None if f_w is None else f_w.contiguous(),
+                    w=w.contiguous(), a=a.contiguous(), b=b.contiguous(), dims=dims, cout=cout, ph=ph, pw=pw, need=need,
+                    strides=(_c_i64 * 5)(*lr.stride()), out=(n * t, cout, h, wd))
+
+    def torgb_fprop(self, x, lr, f_h, f_w, plan_h, plan_w, gain_h, gain_w, window, dtype, w, a, b, clamp, want_mask):
+        """(y [N T, Cout, H, W] in ``dtype``, clamp mask [N T, H, W] uint8 or None): y = dtype(clamp(dtype(w r(a z)) + b))
+        with z = cat(x, cond(lr)).to(dtype) as ``forward`` builds it, never stored. w [Cout, Cin] and b [Cout] in dtype, a
+        [N T, Cin] fp32, clamp None for no clamp."""
+        q = self._torgb_args(x, lr, f_h, f_w, plan_h, plan_w, window, dtype, w, a, b)
+        y = torch.empty(q['out'], dtype=dtype, device=lr.device)
+        mask = torch.empty([q['out'][0], q['out'][2], q['out'][3]], dtype=torch.uint8, device=lr.device) if want_mask else None
+        xt = q['x']
+        _launch('sres_torgb_fprop', self._lib.lvg_sres_torgb_fprop, lr, _ptr(xt), _ptr(lr), _ptr(q['f_h']), _ptr(q['f_w']), _ptr(q['w']),
+                _ptr(q['a']), _ptr(q['b']), _ptr(y), _ptr(mask), _DTYPE_CODE[xt.dtype], _DTYPE_CODE[dtype], *q['dims'], q['strides'],
+                q['ph'], q['pw'], float(gain_h), float(gain_w), q['cout'], float('inf') if clamp is None else float(clamp))
+        return y, mask
+
+    def torgb_backward(self, x, lr, f_h, f_w, plan_h, plan_w, gain_h, gain_w, window, dtype, w, a, b, mask, dy, want_dx=True,
+                       want_dw=True, want_db=True):
+        """Gradients of ``torgb_fprop``'s y in one call: (dx in x's dtype or None, dw [Cout, Cin] in dtype or None, da
+        [N T, Cin] fp32, db [Cout] in dtype or None)."""
+        q = self._torgb_args(x, lr, f_h, f_w, plan_h, plan_w, window, dtype, w, a, b)
+        dy = dy.contiguous()
+        if dy.dtype != dtype or tuple(dy.shape) != q['out'] or dy.device != lr.device:
+            raise RuntimeError(f'sres_torgb_backward: dy must be a {dtype} tensor of shape {list(q["out"])}')
+        if mask is None or mask.dtype != torch.uint8 or tuple(mask.shape) != (q['out'][0],) + q['out'][2:]:
+            raise RuntimeError('sres_torgb_backward: the clamp mask of the forward call is needed')
+        xt = q['x']
+        dx = torch.empty_like(xt) if want_dx else None
+        dw = torch.empty_like(q['w']) if want_dw else None
+        da = torch.empty(q['a'].shape, dtype=torch.float32, device=lr.device)
+        db = torch.empty_like(q['b']) if want_db else None
+        ws = _workspace(lr.device, q['need'])
+        _launch('sres_torgb_backward', self._lib.lvg_sres_torgb_backward, lr, _ptr(xt), _ptr(lr), _ptr(q['f_h']), _ptr(q['f_w']),
+                _ptr(q['w']), _ptr(q['a']), _ptr(mask.contiguous()), _ptr(dy), _ptr(dx), _ptr(dw), _ptr(da), _ptr(db),
+                _DTYPE_CODE[xt.dtype], _DTYPE_CODE[dtype], *q['dims'], q['strides'], q['ph'], q['pw'], float(gain_h), float(gain_w),
+                q['cout'], _ptr(ws), ws.numel())
+        return dx, dw, da, db
 
 
 class SresDblockPlugin:

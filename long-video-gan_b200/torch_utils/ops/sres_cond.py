@@ -277,15 +277,17 @@ def layer_forward(L, g, x_prev, lr, plan, w, force_fp32=False, update_emas=False
     return x
 
 
-def synthesis_forward(S, g, ws, lr, lr_plans, **layer_kwargs):
-    """SynthesisNetwork.forward with each layer's input from ``cond_concat``."""
+def synthesis_forward(S, g, ws, lr, lr_plans, torgb=None, **layer_kwargs):
+    """SynthesisNetwork.forward with each layer's input from ``cond_concat``. ``torgb``: the forward of the ToRGB layer
+    (``layer_forward``'s arguments; torch_utils/ops/sres_torgb.py runs it as one op), None for ``layer_forward``."""
     misc = g['misc']
     misc.assert_shape(ws, [None, S.num_ws, S.w_dim])
     ws = ws.to(torch.float32).unbind(dim=1)
 
     x = S.input(ws[0].size(0)) if S.fourfeats else None
     for name, w, plan in zip(S.layer_names, ws, lr_plans):
-        x = layer_forward(getattr(S, name), g, x, lr, plan, w, **layer_kwargs)
+        L = getattr(S, name)
+        x = (torgb if (torgb is not None and L.is_torgb) else layer_forward)(L, g, x, lr, plan, w, **layer_kwargs)
     if S.output_scale != 1:
         x = x * S.output_scale
 
@@ -312,10 +314,11 @@ def generator_forward(G, g, z, cond, truncation_psi=1, truncation_cutoff=None, u
 
 def _forward(orig):
     g = _install.reference_function(orig).__globals__
-    fused = _install.find(orig, 'lvg_sres_layer')          # sres_layer.install's wrapper below this one
+    # sres_layer.install's and sres_torgb.install's wrappers below this one
+    fused = [f for f in (_install.find(orig, 'lvg_sres_layer'), _install.find(orig, 'lvg_sres_torgb')) if f is not None]
 
     def forward(self, z, cond, truncation_psi=1, truncation_cutoff=None, update_emas=False, **synthesis_kwargs):
-        if fused is not None and fused.takes(self, cond):
+        if any(f.takes(self, cond, update_emas) for f in fused):
             return orig(self, z, cond, truncation_psi, truncation_cutoff, update_emas, **synthesis_kwargs)
         lr_plans = plans(self, cond.size(3), cond.size(4)) if isinstance(cond, torch.Tensor) and cond.ndim == 5 else None
         if lr_plans is None or not applies(self, cond, lr_plans):

@@ -159,16 +159,19 @@ def rejection(G, cond, lr_plans=None):
     return why
 
 
-def _takes(G, cond):
+def _takes(G, cond, update_emas=False):
+    """The installed forward takes the call (``update_emas``: the call's flag, which this op's envelope ignores)."""
     return isinstance(cond, torch.Tensor) and cond.ndim == 5 and rejection(G, cond) is None
 
 
 def _forward(orig):
     g = _install.reference_function(orig).__globals__
+    torgb = _install.find(orig, 'lvg_sres_torgb')          # sres_torgb.install's wrapper below this one
 
     def forward(self, z, cond, truncation_psi=1, truncation_cutoff=None, update_emas=False, **synthesis_kwargs):
         lr_plans = sc.plans(self, cond.size(3), cond.size(4)) if isinstance(cond, torch.Tensor) and cond.ndim == 5 else None
-        if lr_plans is None or rejection(self, cond, lr_plans) is not None:
+        if (lr_plans is None or rejection(self, cond, lr_plans) is not None
+                or (torgb is not None and torgb.takes(self, cond, update_emas))):
             return orig(self, z, cond, truncation_psi, truncation_cutoff, update_emas, **synthesis_kwargs)
         return sc.generator_forward(self, g, z, cond, truncation_psi, truncation_cutoff, update_emas, lr_plans=lr_plans,
                                     step=conv_step, **synthesis_kwargs)
@@ -179,7 +182,9 @@ def _forward(orig):
 def install(*targets):
     """Make ``Generator.forward`` of generator_sres run ``sres_cond.generator_forward`` with every layer's input and
     modulated convolution from ``sres_layer``. ``targets`` as ``sres_cond.install``. Calls outside ``rejection`` run the
-    method this wrapper replaced. Composes with ``sres_cond.install`` and ``modulated_conv.install`` in either order.
+    method this wrapper replaced, and so do calls that an ``sres_torgb.install`` wrapper installed below this one takes
+    (it runs this op's step on the other layers). Composes with ``sres_cond.install``, ``sres_torgb.install`` and
+    ``modulated_conv.install`` in any order.
     Idempotent; the replaced method stays reachable as ``.forward.lvg_sres_layer``. Returns the patched classes."""
     classes = _install.find_classes(targets, 'Generator', sc._is_generator)
     for cls in classes:
