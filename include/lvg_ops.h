@@ -224,6 +224,15 @@ int lvg_convnd_wgrad(const void* x, const void* dy, void* dw, int dtype, int n, 
 int lvg_convnd_plan(int mode, int dtype, int n, int groups, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw,
                     int pad_t, int pad_h, int pad_w, int stride, int* out, int out_len);
 /*
+ * Introspection: the epilogue of the launch lvg_convnd_plan describes, as 4 ints -- [0] 1 when adjacent accumulator
+ * columns are stored as one 8-byte fp32 / 4-byte half2 pair (unit stride, even tile widths, output width and channel
+ * stride; the launch also needs y aligned to a pair), 0 for one store per element, -1 when the call takes the streaming
+ * 1x1x1 kernels; [1] stages of the operand ring (= lvg_convnd_plan's); [2] dynamic shared memory bytes of the launch;
+ * [3] static shared memory bytes of the column map. Host arithmetic only, same arguments as lvg_convnd_plan.
+ */
+int lvg_convnd_epilogue_plan(int mode, int dtype, int n, int groups, int cin, int cout, int t, int h, int wd, int kt, int kh,
+                             int kw, int pad_t, int pad_h, int pad_w, int stride, int* out, int out_len);
+/*
  * Introspection: the kernels a call takes -- mode 0 forward (`epilogue` != 0: with bias / act / gain / clamp), 1 input
  * gradient, 2 weight gradient -> 0 the implicit-GEMM engine, 1 the streaming SIMT kernels for few-channel fp32 1x1x1
  * layers, 2 the pointwise wgmma kernels for every other 1x1x1 forward / input gradient (stride 1, no padding, groups 1,

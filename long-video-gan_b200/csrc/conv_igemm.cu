@@ -38,6 +38,7 @@
 #include <algorithm>
 #include <cuda.h>
 #include <stdlib.h>
+#include <type_traits>
 
 #include "common.cuh"
 #include "wgmma.cuh"
@@ -66,14 +67,28 @@ constexpr int kWidths = 16;                  // conv_igemm_kernel: MMA widths 16
 constexpr int kMaxStages = 6;
 constexpr int kBSlack = 1024;                // shared memory behind an activation stage that MMAs may read
 
+// Unsigned division of n < 2^31 by a launch constant d >= 1 as a multiply-high and a shift (Granlund and Montgomery):
+// mul = ceil(2^(31 + ceil(log2 d)) / d); d = 1 takes mul = 0 and returns n.
+struct FastDiv {
+    uint32_t d, mul, shift;
+};
+inline FastDiv fast_div(int d)
+{
+    FastDiv f = {(uint32_t)d, 0u, 0u};
+    int l = 0;
+    while ((1ull << l) < (uint64_t)d) l++;
+    if (d > 1) { f.mul = (uint32_t)(((1ull << (31 + l)) + d - 1) / d); f.shift = (uint32_t)(l - 1); }
+    return f;
+}
+__device__ __forceinline__ int div_of(int n, const FastDiv& f) { return f.mul ? (int)(__umulhi((uint32_t)n, f.mul) >> f.shift) : n; }
+
 struct IgemmParams {
     const unsigned char* wp;     // packed weights [wgroups][mt][kc][taps_all][a_img]
     void* y;
     const float* bias;           // per output channel (group-local index g*cout + co), or nullptr
     int act;                     // 0 = none, 1 = (x + b) * gain clamped, 2 = lrelu(x + b, alpha) * gain clamped
     float alpha, gain, clamp;    // clamp < 0: none
-    int out_f32;
-    int bf16;                    // operands are bf16 (split fp32) instead of fp16
+    int bf16;                    // operands are bf16 (split fp32) instead of fp16; y is fp32 then, fp16 otherwise
     int wgroups, cout, mt, kc;   // kc = 16-channel steps of the packed K axis
     int nblk;                    // channel blocks per instance in X8
     int nimg;                    // operand images per k-step: 1 (fp16) or 2 (split: hi and lo halves of both operands)
@@ -87,7 +102,8 @@ struct IgemmParams {
     int ncw;                     // MMA width of a consumer: ncols, or in 64-row mode ncols / 2 rounded up to 16
     int a_img;                   // bytes of one weight image: 4096 (128 rows), 2048 (64 rows)
     int tiles_x, tiles_y, tiles_t;
-    int64_t total_tiles;         // tiles_x * tiles_y * tiles_t * mt * instances
+    int64_t total_tiles;         // tiles_x * tiles_y * tiles_t * mt * instances (< 2^31)
+    FastDiv div_x, div_y, div_t, div_mt, div_groups;     // tiles_x, tiles_y, tiles_t, mt, wgroups
     int ks;                      // k-steps per stage (> 1 only when kt == 1)
     int stages;
     int a_resident;              // the ring length is a multiple of the stages per tile and every tile of the launch uses the same weights:
@@ -95,6 +111,9 @@ struct IgemmParams {
     int a_stage, b_step, b_bytes, b_box, stage_bytes;    // bytes: A per stage, B stride per k-step / per pair of blocks, TMA payload of a pair, whole stage
     int64_t y_cs;                // output channel stride (= to*hos*wos)
     int ostride, hos, wos;       // output decimation (strided convolution): only rows / columns divisible by ostride are stored
+    int ths, wts;                // th / ostride, wt / ostride: a row / column tile's origin on the stored grid (tile origins lie on the lattice)
+    int pair_store;              // adjacent even / odd accumulator columns are adjacent output elements and y is aligned for
+                                 // one 8-byte fp32 / 4-byte half2 store per pair (plan_pairs_columns and an aligned y)
     const float* out_scale;      // per-(instance, output channel, output frame) factor [inst][cout][to] on the accumulator, or nullptr
 };
 
@@ -332,18 +351,52 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, i
                  : "memory");
 }
 
-struct TileCoord { int ox0, oy0, t0, mti, inst; };
+struct TileCoord { int ox0, oy0, t0, mti, inst, grp, ix, iy; };
 
-__device__ __forceinline__ TileCoord decode_tile(const IgemmParams& p, int64_t L)
+__device__ __forceinline__ TileCoord decode_tile(const IgemmParams& p, int L)
 {
     TileCoord c;
-    int64_t r = L;
-    c.ox0 = (int)(r % p.tiles_x) * p.wt; r /= p.tiles_x;
-    c.oy0 = (int)(r % p.tiles_y) * p.th; r /= p.tiles_y;
-    c.t0 = (int)(r % p.tiles_t) * p.tt; r /= p.tiles_t;
-    c.mti = (int)(r % p.mt);
-    c.inst = (int)(r / p.mt);
+    int q = div_of(L, p.div_x);
+    c.ix = L - q * p.tiles_x;
+    int r = div_of(q, p.div_y);
+    c.iy = q - r * p.tiles_y;
+    q = div_of(r, p.div_t);
+    c.t0 = (r - q * p.tiles_t) * p.tt;
+    c.inst = div_of(q, p.div_mt);
+    c.mti = q - c.inst * p.mt;
+    c.grp = c.inst - div_of(c.inst, p.div_groups) * p.wgroups;
+    c.ox0 = c.ix * p.wt; c.oy0 = c.iy * p.th;
     return c;
+}
+
+// Column map of the epilogue. Which output element an accumulator column holds depends on the launch only: column n is
+// (frame f, row r, col cc) of the tile, stored at f * hos * wos + (r / ostride) * wos + cc / ostride past the tile's
+// origin on the stored grid, unless it is a halo column, lies off the stride lattice or is past ncols. Each CTA builds the
+// map once; a tile then needs only its origin and its clipped extents, and the epilogue does no division.
+// The clip test is one subtraction: key = cc | r << 11 | f << 22 (10-, 10- and 8-bit fields), a tile's limit word holds
+// (extent - 1) of each axis in the same fields with the guard bits 10, 21 and 30 set; (limit - key) keeps a field's guard
+// bit exactly when key's field is within the extent (no borrow crosses a guard). Columns never stored get a key whose cc
+// field (1023) no tile accepts.
+constexpr uint32_t kKeyGuards = (1u << 10) | (1u << 21) | (1u << 30);
+constexpr uint32_t kKeyNever = 1023u;
+constexpr int kMapCols = 256;                // at most 256 accumulator columns per tile (both halves in 64-row mode)
+
+__device__ __forceinline__ uint32_t col_limit(int tl, int hl, int wl)
+{
+    return ((uint32_t)(wl - 1) | (uint32_t)(hl - 1) << 11 | (uint32_t)(tl - 1) << 22) | kKeyGuards;
+}
+__device__ __forceinline__ bool col_in_tile(uint32_t key, uint32_t limit) { return ((limit - key) & kKeyGuards) == kKeyGuards; }
+
+// [bias, lrelu, gain, clamp] as the reference applies them (act 0: the accumulator as it is)
+__device__ __forceinline__ float epilogue_value(const IgemmParams& p, float v, float bias)
+{
+    if (p.act) {
+        v += bias;
+        if (p.act == 2) v = v < 0.f ? v * p.alpha : v;
+        v *= p.gain;
+        if (p.clamp >= 0.f) v = fminf(fmaxf(v, -p.clamp), p.clamp);
+    }
+    return v;
 }
 
 // Persistent: CTA b works on tiles b, b + gridDim.x, ... (pixel tile fastest, so that concurrently running CTAs share the
@@ -357,8 +410,10 @@ __device__ __forceinline__ TileCoord decode_tile(const IgemmParams& p, int64_t L
 template <bool BF16, int NW, bool OSCALE>
 __global__ void __launch_bounds__(kIgemmThreads, 1) conv_igemm_kernel(const __grid_constant__ CUtensorMap tmx, const IgemmParams p)
 {
+    using OutT = typename std::conditional<BF16, float, __half>::type;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     __shared__ uint64_t full_bar[kMaxStages], empty_bar[kMaxStages];
+    __shared__ __align__(16) int2 col_map[kMapCols];         // accumulator column -> (offset past the tile origin, clip key)
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~(uintptr_t)127);
 
     const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
@@ -370,19 +425,26 @@ __global__ void __launch_bounds__(kIgemmThreads, 1) conv_igemm_kernel(const __gr
         for (int s = 0; s < p.stages; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
         fence_barrier_init();
     }
+    for (int n = threadIdx.x; n < (p.m64 ? 2 * NW : NW); n += kIgemmThreads) {
+        const int f = n / p.frame_px, rem = n - f * p.frame_px;
+        const int r = rem / p.wtb, cc = rem - r * p.wtb;
+        const bool st = n < p.ncols && f < p.tt && r < p.th && cc < p.wt && r % p.ostride == 0 && cc % p.ostride == 0;
+        col_map[n] = st ? make_int2((f * p.hos + r / p.ostride) * p.wos + cc / p.ostride, (int)((uint32_t)cc | (uint32_t)r << 11 | (uint32_t)f << 22))
+                        : make_int2(0, (int)kKeyNever);
+    }
     __syncthreads();
 
     if (wg == 0) {
         if (warp == 0 && elect_one()) {
-            int it = 0;
-            for (int64_t L = blockIdx.x; L < p.total_tiles; L += gridDim.x) {
+            int it = 0, s = 0;
+            uint32_t phase = 0;                               // (it / stages) & 1: the ring position kept without a division
+            for (int L = blockIdx.x; L < p.total_tiles; L += gridDim.x) {
                 const TileCoord c = decode_tile(p, L);
-                const unsigned char* wpg = p.wp + (((int64_t)(c.inst % p.wgroups) * p.mt + c.mti) * p.kc) * (int64_t)(p.kt * taps2) * (p.nimg * p.a_img);
+                const unsigned char* wpg = p.wp + (((int64_t)c.grp * p.mt + c.mti) * p.kc) * (int64_t)(p.kt * taps2) * (p.nimg * p.a_img);
                 const int blk0 = c.inst * p.nblk;
                 for (int kt = 0; kt < p.kt; kt++) {
-                    for (int kcix = 0; kcix < kchunks; kcix++, it++) {
-                        const int s = it % p.stages;
-                        if (it >= p.stages) mbar_wait(&empty_bar[s], (uint32_t)((it / p.stages - 1) & 1));
+                    for (int kcix = 0; kcix < kchunks; kcix++, it++, s = s + 1 == p.stages ? (phase ^= 1u, 0) : s + 1) {
+                        if (it >= p.stages) mbar_wait(&empty_bar[s], phase ^ 1u);
                         unsigned char* st = smem + (size_t)s * p.stage_bytes;
                         const int k0 = kcix * p.ks;
                         const int nks = min(p.ks, p.kc - k0);
@@ -410,17 +472,17 @@ __global__ void __launch_bounds__(kIgemmThreads, 1) conv_igemm_kernel(const __gr
         // 128-row images: this warpgroup's 64 rows start 1024 bytes into an image; 64-row mode: its columns start NW pixels in
         const uint32_t a_row0 = p.m64 ? 0u : (uint32_t)cw * 1024u;
         const int col0 = p.m64 ? cw * NW : 0;
-        int it = 0;
-        for (int64_t L = blockIdx.x; L < p.total_tiles; L += gridDim.x) {
+        int s = 0;
+        uint32_t phase = 0;
+        for (int L = blockIdx.x; L < p.total_tiles; L += gridDim.x) {
             const TileCoord c = decode_tile(p, L);
             float acc[NW / 2];
 #pragma unroll
             for (int i = 0; i < NW / 2; i++) acc[i] = 0.f;
             int prev = -1;
             for (int kt = 0; kt < p.kt; kt++) {
-                for (int kcix = 0; kcix < kchunks; kcix++, it++) {
-                    const int s = it % p.stages;
-                    mbar_wait(&full_bar[s], (uint32_t)((it / p.stages) & 1));
+                for (int kcix = 0; kcix < kchunks; kcix++, s = s + 1 == p.stages ? (phase ^= 1u, 0) : s + 1) {
+                    mbar_wait(&full_bar[s], phase);
                     wgmma_fence();
                     const uint32_t st = smem_u32(smem + (size_t)s * p.stage_bytes);
                     const int nks = min(p.ks, p.kc - kcix * p.ks);
@@ -452,9 +514,12 @@ __global__ void __launch_bounds__(kIgemmThreads, 1) conv_igemm_kernel(const __gr
             mbar_arrive_if(&empty_bar[prev], tid == 0);
 
             // ---- epilogue: registers -> [bias, lrelu, gain, clamp] -> NC(T)HW global. This thread holds accumulator rows
-            // r and r + 8 (conv_pack_w_kernel's row order -> channel) and column pairs col0 + 8 j + 2 (lane % 4).
+            // r and r + 8 (conv_pack_w_kernel's row order -> channel) and column pairs col0 + 8 j + 2 (lane % 4); the column
+            // map gives each column's place past the tile origin.
             const int per = m_rows_per_quadrant(p.cout - c.mti * kBM);
-            int64_t chbase[2];
+            const uint32_t limit = col_limit(min(p.tt, p.to - c.t0), min(p.th, p.ho - c.oy0), min(p.wt, p.wo - c.ox0));
+            const int64_t tile_off = ((int64_t)c.t0 * p.hos + c.iy * p.ths) * p.wos + c.ix * p.wts;
+            OutT* yrow[2];
             float bias[2];
             bool rok[2];
             const float* osc[2];
@@ -464,41 +529,46 @@ __global__ void __launch_bounds__(kIgemmThreads, 1) conv_igemm_kernel(const __gr
                 const int ch = p.m64 ? row : m_channel_of_row(cw * 64 + row, per);
                 const int co = c.mti * kBM + ch;
                 rok[h] = ch < kBM && co < p.cout;
-                bias[h] = (p.bias != nullptr && rok[h]) ? __ldg(p.bias + (int64_t)(c.inst % p.wgroups) * p.cout + co) : 0.f;
-                chbase[h] = ((int64_t)c.inst * p.cout + co) * p.y_cs;
-                osc[h] = OSCALE ? p.out_scale + ((int64_t)c.inst * p.cout + co) * p.to : nullptr;
+                bias[h] = (p.bias != nullptr && rok[h]) ? __ldg(p.bias + (int64_t)c.grp * p.cout + co) : 0.f;
+                yrow[h] = reinterpret_cast<OutT*>(p.y) + ((int64_t)c.inst * p.cout + co) * p.y_cs + tile_off;
+                osc[h] = OSCALE ? p.out_scale + ((int64_t)c.inst * p.cout + co) * p.to + c.t0 : nullptr;
             }
+            const int2* cmap = col_map + col0 + 2 * (lane % 4);
+            if (p.pair_store) {
+                // columns 2i and 2i + 1 are stored together or not at all, at adjacent addresses
 #pragma unroll
-            for (int j = 0; j < NW / 8; j++) {
-#pragma unroll
-                for (int e = 0; e < 2; e++) {
-                    // accumulator column -> (frame, row, col) of the tile
-                    const int n = col0 + j * 8 + 2 * (lane % 4) + e;
-                    const int f = n / p.frame_px, rem = n - f * p.frame_px;
-                    const int r = rem / p.wtb, cc = rem - r * p.wtb;
-                    const int ot = c.t0 + f, oy = c.oy0 + r, ox = c.ox0 + cc;
-                    bool ok = n < p.ncols && f < p.tt && r < p.th && cc < p.wt && ot < p.to && oy < p.ho && ox < p.wo;
-                    int64_t off;
-                    if (p.ostride == 1) {
-                        off = ((int64_t)ot * p.ho + oy) * p.wo + ox;
-                    } else {
-                        ok = ok && (oy % p.ostride == 0) && (ox % p.ostride == 0);
-                        off = ((int64_t)ot * p.hos + oy / p.ostride) * p.wos + ox / p.ostride;
-                    }
-                    if (!ok) continue;
+                for (int j = 0; j < NW / 8; j++) {
+                    const int2 m = cmap[j * 8];
+                    if (!col_in_tile((uint32_t)m.y, limit)) continue;
 #pragma unroll
                     for (int h = 0; h < 2; h++) {
                         if (!rok[h]) continue;
-                        float v = acc[4 * j + 2 * h + e];
-                        if constexpr (OSCALE) v *= __ldg(osc[h] + ot);
-                        if (p.act) {
-                            v += bias[h];
-                            if (p.act == 2) v = v < 0.f ? v * p.alpha : v;
-                            v *= p.gain;
-                            if (p.clamp >= 0.f) v = fminf(fmaxf(v, -p.clamp), p.clamp);
+                        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                        if constexpr (OSCALE) { const float s = __ldg(osc[h] + ((uint32_t)m.y >> 22)); v0 *= s; v1 *= s; }
+                        v0 = epilogue_value(p, v0, bias[h]);
+                        v1 = epilogue_value(p, v1, bias[h]);
+                        if constexpr (BF16) *reinterpret_cast<float2*>(yrow[h] + m.x) = make_float2(v0, v1);
+                        else *reinterpret_cast<__half2*>(yrow[h] + m.x) = __floats2half2_rn(v0, v1);
+                    }
+                }
+            } else {
+#pragma unroll
+                for (int j = 0; j < NW / 8; j++) {
+                    const int4 m = *reinterpret_cast<const int4*>(cmap + j * 8);
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        const int off = e ? m.z : m.x;
+                        const uint32_t key = (uint32_t)(e ? m.w : m.y);
+                        if (!col_in_tile(key, limit)) continue;
+#pragma unroll
+                        for (int h = 0; h < 2; h++) {
+                            if (!rok[h]) continue;
+                            float v = acc[4 * j + 2 * h + e];
+                            if constexpr (OSCALE) v *= __ldg(osc[h] + (key >> 22));
+                            v = epilogue_value(p, v, bias[h]);
+                            if constexpr (BF16) yrow[h][off] = v;
+                            else yrow[h][off] = __float2half_rn(v);
                         }
-                        if (p.out_f32) reinterpret_cast<float*>(p.y)[chbase[h] + off] = v;
-                        else reinterpret_cast<__half*>(p.y)[chbase[h] + off] = __float2half_rn(v);
                     }
                 }
             }
@@ -559,6 +629,18 @@ Geometry job_geometry(const IgemmJob& j)
 
 IgemmRooms igemm_rooms_of(const Geometry& g, bool x8_pre) { return {round256(g.w_bytes), x8_pre ? 0 : g.act_bytes}; }
 
+// Accumulator columns 2i and 2i + 1 are the same output row's elements x and x + 1 with x even, both stored or both
+// clipped, and every such pair starts at an even element offset: unit stride, even tile and box widths (so even frame
+// and row strides in the accumulator), an even output width and channel stride. With a y aligned to a pair's size the
+// epilogue stores one 8-byte fp32 / 4-byte half2 per pair.
+bool plan_pairs_columns(const IgemmParams& p)
+{
+    return p.ostride == 1 && p.wt % 2 == 0 && p.wtb % 2 == 0 && p.wo % 2 == 0 && p.y_cs % 2 == 0;
+}
+
+// dynamic shared memory of a launch: the stage ring and its 128-byte alignment
+int igemm_smem_bytes(const IgemmParams& p) { return p.stages * p.stage_bytes + 128; }
+
 // The tiling of a job: host arithmetic only (no CUDA call, no pointer dereferenced). lvg_convnd_plan hands it out.
 int plan_igemm(const IgemmJob& j, IgemmParams& p)
 {
@@ -569,7 +651,7 @@ int plan_igemm(const IgemmJob& j, IgemmParams& p)
 
     memset(&p, 0, sizeof(p));
     p.y = j.y; p.bias = j.bias; p.act = j.act; p.alpha = j.alpha; p.gain = j.gain; p.clamp = j.clamp; p.out_scale = j.out_scale;
-    p.out_f32 = p.bf16 = j.dtype == LVG_F32 ? 1 : 0;
+    p.bf16 = j.dtype == LVG_F32 ? 1 : 0;
     p.wgroups = j.groups; p.cout = j.cm; p.mt = g.mt; p.kc = g.kc; p.nblk = g.nblk;
     p.nimg = g.nimg; p.lo_blk = g.cblk;
     p.m64 = g.m64; p.a_img = g.a_img;
@@ -653,6 +735,13 @@ int plan_igemm(const IgemmJob& j, IgemmParams& p)
     }
     p.y_cs = (int64_t)p.to * p.hos * p.wos;
     p.total_tiles = (int64_t)p.tiles_x * p.tiles_y * p.tiles_t * g.mt * inst;
+    LVG_REQUIRE(p.total_tiles < (1ll << 31), "convnd: too many tiles");
+    p.div_x = fast_div(p.tiles_x); p.div_y = fast_div(p.tiles_y); p.div_t = fast_div(p.tiles_t); p.div_mt = fast_div(g.mt);
+    p.div_groups = fast_div(j.groups);
+    // the epilogue places a tile on the stored grid by its tile indices
+    LVG_REQUIRE((p.tiles_x == 1 || p.wt % ostride == 0) && (p.tiles_y == 1 || p.th % ostride == 0), "convnd: tile origins off the stride lattice");
+    p.ths = p.th / ostride; p.wts = p.wt / ostride;
+    p.pair_store = plan_pairs_columns(p) ? 1 : 0;          // run_igemm clears it for a y that is not aligned for pairs
     return LVG_OK;
 }
 
@@ -726,6 +815,7 @@ int run_igemm(const IgemmJob& j, void* workspace, int64_t workspace_bytes, cudaS
     unsigned char* wp = reinterpret_cast<unsigned char*>(workspace);
     unsigned char* x8 = j.x8_pre ? const_cast<unsigned char*>(j.x8_pre) : wp + r.wp;
     p.wp = wp;
+    if (reinterpret_cast<uintptr_t>(j.y) % (split ? 8 : 4) != 0) p.pair_store = 0;
 
     // re-tile the operands
     {
@@ -772,7 +862,7 @@ int run_igemm(const IgemmJob& j, void* workspace, int64_t workspace_bytes, cudaS
                                   p.tt, 2);
         if (rc) return rc;
     }
-    const size_t smem = (size_t)p.stages * p.stage_bytes + 128;
+    const size_t smem = (size_t)igemm_smem_bytes(p);
     // one instantiation per MMA width (the output-scaled epilogue is a separate one: the unscaled one stays as it was)
 #define LVG_IGEMM_WIDTHS(B, S)                                                                                                     \
     {conv_igemm_kernel<B, 16, S>,  conv_igemm_kernel<B, 32, S>,  conv_igemm_kernel<B, 48, S>,  conv_igemm_kernel<B, 64, S>,        \
@@ -1347,6 +1437,27 @@ extern "C" int lvg_convnd_plan(int mode, int dtype, int n, int groups, int cin, 
                        (int)p.total_tiles, p.ks, p.stages, p.a_resident, p.a_stage, p.b_step, p.b_bytes, p.b_box, p.stage_bytes, p.ostride, p.hos, p.wos,
                        p.m64, p.ncw, 0, 0, 0, 0, 0, 0, 0, 0};
     for (int i = 0; i < 48; i++) out[i] = v[i];
+    return LVG_OK;
+}
+
+// the epilogue of that launch (host arithmetic only; tests/test_conv_epilogue_host.py checks it against the tiling)
+extern "C" int lvg_convnd_epilogue_plan(int mode, int dtype, int n, int groups, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw,
+                                        int pad_t, int pad_h, int pad_w, int stride, int* out, int out_len)
+{
+    LVG_REQUIRE(out && out_len >= 4, "convnd_epilogue_plan: out must hold 4 ints");
+    int plan[48];
+    const int rc = lvg_convnd_plan(mode, dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, stride, plan, 48);
+    if (rc) return rc;
+    for (int i = 0; i < out_len; i++) out[i] = 0;
+    if (plan[47]) { out[0] = -1; return LVG_OK; }
+    const ConvShape sh = {dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, stride};
+    IgemmParams p;
+    const int prc = plan_igemm(mode == 0 ? fprop_job(sh, nullptr, nullptr, nullptr) : dgrad_job(sh, nullptr, nullptr, nullptr), p);
+    if (prc) return prc;
+    out[0] = p.pair_store;
+    out[1] = p.stages;
+    out[2] = igemm_smem_bytes(p);
+    out[3] = kMapCols * (int)sizeof(int2);
     return LVG_OK;
 }
 
