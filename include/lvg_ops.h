@@ -506,6 +506,34 @@ int lvg_sres_torgb_backward(const void* x, const float* lr, const float* f_h, co
                             int cout, void* workspace, int64_t workspace_bytes, void* stream);
 
 /*
+ * The low-res generator's ToRGB layer in one pass over its input (DESIGN.md 7l), on the CUDA cores:
+ *   y = dtype(clamp(dtype(u) + dtype(b), +-clamp)),  u = sum_c w[o][c] a[n][c][t] r(x[c])  per pixel, o < cout = 3
+ * with r() the rounding of x.type(dtype) and the products accumulated in fp32. x: dense [n][cin][t][h][wd] in x_dtype
+ * (fp16 / fp32), read in place; w fp32 [cout][cin] (the reference's weight / sqrt(cin)); a fp32 [n][cin][t] (style times
+ * the magnitude-EMA gain); b fp32 [cout]; dtype (fp16 / fp32) the layer's. clamp < 0: none (bias_act's convention).
+ * lvg_lres_torgb_fprop writes exactly one of y ([n][cout][t][h][wd], dtype) or u (same shape, fp32, before rounding,
+ * bias and clamp). With sumsq (NULL = not wanted) it also writes the sum of r(x)^2 over the whole input to sumsq[0],
+ * from per-CTA partials in `workspace` folded in a fixed order (one more launch). lvg_lres_torgb_finish then writes
+ * y = dtype(clamp(dtype(gain[0] u) + dtype(b))) with the gain read from device memory (no host synchronisation).
+ * lvg_lres_torgb_backward, from the forward's y and dy (dtype, y's shape): dy' = dy where -clamp < y < clamp, else 0;
+ * dx (NULL = not wanted) = x_dtype(a w^T dy') per pixel; da [n][cin][t] = sum over the pixels of a plane of
+ * sum_o w[o][c] dy'[o] r(x[c]); dw [cout][cin] (NULL = not wanted) = sum over planes of a times the same sums; db
+ * [cout] (NULL = not wanted) = sum dy'; all fp32. Per-CTA partial sums in `workspace` (lvg_lres_torgb_workspace bytes,
+ * which also covers the forward's sumsq), folded by two more kernels in a fixed order: bitwise reproducible, no
+ * atomics. The size query returns -1 for anything the kernels do not take (cout != 3, a kernel other than 1 x 1 x 1
+ * (kt, kh, kw), more than 512 input channels, a dtype other than fp16 / fp32); such calls return LVG_UNSUPPORTED.
+ */
+int64_t lvg_lres_torgb_workspace(int x_dtype, int dtype, int n, int cin, int t, int h, int wd, int cout, int kt, int kh, int kw);
+int lvg_lres_torgb_fprop(const void* x, const float* w, const float* a, const float* b, void* y, float* u, float* sumsq,
+                         int x_dtype, int dtype, int n, int cin, int t, int h, int wd, int cout, float clamp,
+                         void* workspace, int64_t workspace_bytes, void* stream);
+int lvg_lres_torgb_finish(const float* u, const float* gain, const float* b, void* y, int dtype, int n, int t, int h, int wd,
+                          float clamp, void* stream);
+int lvg_lres_torgb_backward(const void* x, const float* w, const float* a, const void* y, const void* dy, void* dx, float* dw,
+                            float* da, float* db, int x_dtype, int dtype, int n, int cin, int t, int h, int wd, int cout,
+                            float clamp, void* workspace, int64_t workspace_bytes, void* stream);
+
+/*
  * Layers of a super-res discriminator block (discriminator_sres.py DiscriminatorBlock, architecture 'resnet'; DESIGN.md 7i).
  *
  * lvg_sres_dblock_conv1: conv1, y = bias_act(conv2d(upfirdn2d(x, f, padding 2), w, stride 2), bias, act, alpha, gain,

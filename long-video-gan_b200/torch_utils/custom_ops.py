@@ -103,6 +103,10 @@ _SIGNATURES = {
     'lvg_sres_torgb_fprop': (_c_int, [_c_void_p] * 9 + [_c_int] * 10 + [_c_void_p] * 3 + [_c_float] * 2 + [_c_int, _c_float, _c_void_p]),
     'lvg_sres_torgb_backward': (_c_int, [_c_void_p] * 12 + [_c_int] * 10 + [_c_void_p] * 3 + [_c_float] * 2 + [_c_int]
                                 + [_c_void_p, _c_i64, _c_void_p]),
+    'lvg_lres_torgb_workspace': (_c_i64, [_c_int] * 11),
+    'lvg_lres_torgb_fprop': (_c_int, [_c_void_p] * 7 + [_c_int] * 8 + [_c_float, _c_void_p, _c_i64, _c_void_p]),
+    'lvg_lres_torgb_finish': (_c_int, [_c_void_p] * 4 + [_c_int] * 5 + [_c_float, _c_void_p]),
+    'lvg_lres_torgb_backward': (_c_int, [_c_void_p] * 9 + [_c_int] * 8 + [_c_float, _c_void_p, _c_i64, _c_void_p]),
     'lvg_sres_dblock_conv1_workspace': (_c_i64, [_c_int] * 6),
     'lvg_sres_dblock_conv1': (_c_int, [_c_void_p] * 3 + [_c_int] + [_c_void_p] * 3 + [_c_int] * 7 + [_c_float] * 3 + [_c_void_p, _c_i64, _c_void_p]),
     'lvg_sres_dblock_conv1_backward_workspace': (_c_i64, [_c_int] * 6),
@@ -218,7 +222,8 @@ _ws = {}
 
 def _workspace(device, need):
     """The convolution engine's workspace on ``device``: one buffer of at least ``need`` bytes (and 4 MiB), grown on
-    demand and shared by every ConvNdPlugin and SresDblockPlugin call and the SresCondPlugin layer calls."""
+    demand and shared by every ConvNdPlugin and SresDblockPlugin call, the SresCondPlugin layer calls and the LresTorgbPlugin calls
+    that need one."""
     if need < 0:
         raise RuntimeError('convnd: configuration outside the tensor-core kernel envelope')
     buf = _ws.get(device)
@@ -1144,6 +1149,89 @@ class SresCondPlugin:
         return dx, dw, da, db
 
 
+class LresTorgbPlugin:
+    """The low-res generator's ToRGB layer in one pass over its input (DESIGN.md 7l; no reference plugin: ToRGB.forward
+    composes MagnitudeEMA, ATen muls, F.conv3d and bias_act, generator_lres.py:618-641). x [N, Cin, T, H, W] fp16 / fp32
+    is read in its own dtype; w fp32 [3, Cin], a fp32 [N, Cin, T], b fp32 [3]; ``dtype`` is the layer's."""
+
+    def __init__(self, lib):
+        self._lib = lib
+
+    def workspace(self, x_dtype, dtype, n, cin, t, h, w, cout, kernel=(1, 1, 1)):
+        """Workspace bytes of lvg_lres_torgb_backward (and of the forward's sum of squares), or -1 where the kernels do not
+        take the call."""
+        return int(self._lib.lvg_lres_torgb_workspace(_DTYPE_CODE.get(x_dtype, -1), _DTYPE_CODE.get(dtype, -1), n, cin, t, h, w,
+                                                      cout, *(int(k) for k in kernel)))
+
+    def _args(self, x, w, a, b, dtype):
+        """Checked, dense arguments shared by every entry point, and the workspace the call needs."""
+        if not x.is_cuda or x.dtype not in (torch.float16, torch.float32) or x.ndim != 5:
+            raise RuntimeError('lres_torgb: x must be a 5-D float16 / float32 CUDA tensor')
+        n, cin, t, h, wd = x.shape
+        if w.dtype != torch.float32 or w.ndim != 2 or w.shape[1] != cin or w.device != x.device:
+            raise RuntimeError(f'lres_torgb: w must be a float32 [3, {cin}] tensor on the device of x')
+        if a.dtype != torch.float32 or tuple(a.shape) != (n, cin, t) or a.device != x.device:
+            raise RuntimeError(f'lres_torgb: a must be a float32 [{n}, {cin}, {t}] tensor on the device of x')
+        cout = int(w.shape[0])
+        if b is not None and (b.dtype != torch.float32 or tuple(b.shape) != (cout,) or b.device != x.device):
+            raise RuntimeError(f'lres_torgb: b must be a float32 [{cout}] tensor on the device of x')
+        need = self.workspace(x.dtype, dtype, n, cin, t, h, wd, cout)
+        if need < 0:
+            raise RuntimeError(f'lres_torgb: no kernel for x {list(x.shape)} ({x.dtype}), w {list(w.shape)}, layer dtype {dtype}')
+        return (x.contiguous(), w.contiguous(), a.contiguous(), None if b is None else b.contiguous(),
+                (_DTYPE_CODE[x.dtype], _DTYPE_CODE[dtype], n, cin, t, h, wd, cout), need)
+
+    def fprop(self, x, w, a, b, dtype, clamp):
+        """y [N, 3, T, H, W] in dtype: dtype(clamp(dtype(sum_c w a r(x)) + dtype(b))), clamp None for none."""
+        x, w, a, b, dims, _ = self._args(x, w, a, b, dtype)
+        y = torch.empty([dims[2], dims[7], *x.shape[2:]], dtype=dtype, device=x.device)
+        _launch('lres_torgb_fprop', self._lib.lvg_lres_torgb_fprop, x, _ptr(x), _ptr(w), _ptr(a), _ptr(b), _ptr(y), None, None,
+                *dims, -1.0 if clamp is None else float(clamp), None, 0)
+        return y
+
+    def fprop_sumsq(self, x, w, a, dtype):
+        """(u [N, 3, T, H, W] fp32 = sum_c w a r(x), sum of r(x)^2 over x as a 0-dim fp32 tensor), from one pass over x."""
+        x, w, a, _, dims, need = self._args(x, w, a, None, dtype)
+        u = torch.empty([dims[2], dims[7], *x.shape[2:]], dtype=torch.float32, device=x.device)
+        sumsq = torch.empty([], dtype=torch.float32, device=x.device)
+        ws = _workspace(x.device, need)
+        _launch('lres_torgb_fprop', self._lib.lvg_lres_torgb_fprop, x, _ptr(x), _ptr(w), _ptr(a), None, None, _ptr(u), _ptr(sumsq),
+                *dims, -1.0, _ptr(ws), ws.numel())
+        return u, sumsq
+
+    def finish(self, u, gain, b, dtype, clamp):
+        """y = dtype(clamp(dtype(gain u) + dtype(b))) from fprop_sumsq's u, gain a 0-dim fp32 tensor on the device."""
+        if not u.is_cuda or u.dtype != torch.float32 or u.ndim != 5 or u.shape[1] != 3:
+            raise RuntimeError('lres_torgb_finish: u must be a float32 [N, 3, T, H, W] CUDA tensor')
+        if gain.dtype != torch.float32 or gain.numel() != 1 or gain.device != u.device:
+            raise RuntimeError('lres_torgb_finish: gain must be one float32 value on the device of u')
+        if b.dtype != torch.float32 or tuple(b.shape) != (3,) or b.device != u.device:
+            raise RuntimeError('lres_torgb_finish: b must be a float32 [3] tensor on the device of u')
+        u, gain, b = u.contiguous(), gain.contiguous(), b.contiguous()
+        n, _, t, h, wd = u.shape
+        y = torch.empty(u.shape, dtype=dtype, device=u.device)
+        _launch('lres_torgb_finish', self._lib.lvg_lres_torgb_finish, u, _ptr(u), _ptr(gain), _ptr(b), _ptr(y), _dtype_code(y, 'lres_torgb'),
+                n, t, h, wd, -1.0 if clamp is None else float(clamp))
+        return y
+
+    def backward(self, x, w, a, y, dy, dtype, clamp, want_dx=True, want_dw=True, want_db=True):
+        """(dx in x's dtype or None, dw fp32 [3, Cin] or None, da fp32 [N, Cin, T], db fp32 [3] or None) of fprop's y."""
+        x, w, a, _, dims, need = self._args(x, w, a, None, dtype)
+        shape = (dims[2], dims[7]) + tuple(x.shape[2:])
+        for name, v in (('y', y), ('dy', dy)):
+            if v.dtype != dtype or tuple(v.shape) != shape or v.device != x.device:
+                raise RuntimeError(f'lres_torgb_backward: {name} must be a {dtype} tensor of shape {list(shape)}')
+        y, dy = y.contiguous(), dy.contiguous()
+        dx = torch.empty_like(x) if want_dx else None
+        dw = torch.empty_like(w) if want_dw else None
+        da = torch.empty_like(a)
+        db = torch.empty([dims[7]], dtype=torch.float32, device=x.device) if want_db else None
+        ws = _workspace(x.device, need)
+        _launch('lres_torgb_backward', self._lib.lvg_lres_torgb_backward, x, _ptr(x), _ptr(w), _ptr(a), _ptr(y), _ptr(dy), _ptr(dx),
+                _ptr(dw), _ptr(da), _ptr(db), *dims, -1.0 if clamp is None else float(clamp), _ptr(ws), ws.numel())
+        return dx, dw, da, db
+
+
 class SresDblockPlugin:
     """The two native layers of a super-res discriminator block (DESIGN.md 7i): ``conv1`` (the 4-tap FIR in the
     convolution's re-tiling pass, the stride-2 3x3 convolution with its bias_act epilogue) and ``skip`` (the 1x1 convolution
@@ -1224,6 +1312,7 @@ class SresDblockPlugin:
 
 
 _PLUGIN_CLASSES = {
+    'lres_torgb_plugin': LresTorgbPlugin,
     'sres_dblock_plugin': SresDblockPlugin,
     'sres_cond_plugin': SresCondPlugin,
     'dblock_tail_plugin': DblockTailPlugin,
