@@ -534,6 +534,32 @@ int lvg_lres_torgb_backward(const void* x, const float* w, const float* a, const
                             float clamp, void* workspace, int64_t workspace_bytes, void* stream);
 
 /*
+ * The first modulated convolution of the low-res generator's residual block with its bias_act (DESIGN.md 7m):
+ *   y = clamp(act(d (.) conv(a (.) x, w) + b) * gain)
+ * with x, w, a, d, the shapes and the padding as lvg_modconv_fprop (d required; the output keeps the input's frame count),
+ * b fp32 [cout] or NULL, act 1 linear / 2 lrelu with alpha, gain and clamp (< 0: none) as lvg_convnd_fprop. The
+ * pre-activation is never stored: the engine's epilogue applies d, the bias, the activation, the gain and the clamp.
+ * sumsq (NULL = not wanted): sum of the squares of y as stored (rounded to dtype) in sumsq[0], fp32, from one more pass
+ * over y (per-CTA partials over a fixed grid, folded in a fixed order: two more launches).
+ * lvg_gblock_conv0_backward, from the forward's y and dy (y's dtype and shape), with dz = G(y) dy bias_act's gradient
+ * (decided from y): dx (x's shape and dtype), dw (w's, NULL = not wanted), da [n][cin][t] as lvg_modconv_backward of dz;
+ * dd [n][cout][t] (NULL = not wanted) = sum_hw dz (z(y) - b) / d with z(y) the pre-activation recovered from y; db [cout]
+ * (NULL = not wanted) = sum dz over n, t, h, w in a fixed order; all fp32, bitwise reproducible. dz is never written: the
+ * convolution gradients re-tile dy with G(y) and d. `workspace`: lvg_gblock_conv0_workspace bytes (forward and backward),
+ * 16-byte aligned; -1 / LVG_UNSUPPORTED outside lvg_modconv_workspace's envelope or for an output frame count other than t.
+ */
+int64_t lvg_gblock_conv0_workspace(int dtype, int n, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw,
+                                   int pad_t, int pad_h, int pad_w);
+int lvg_gblock_conv0_fprop(const void* x, const void* w, const float* a, const float* d, const float* b, void* y, float* sumsq,
+                           int dtype, int n, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw, int pad_t,
+                           int pad_h, int pad_w, int act, float alpha, float gain, float clamp, void* workspace,
+                           int64_t workspace_bytes, void* stream);
+int lvg_gblock_conv0_backward(const void* x, const void* w, const float* a, const float* d, const float* b, const void* y,
+                              const void* dy, void* dx, void* dw, float* da, float* dd, float* db, int dtype, int n, int cin,
+                              int cout, int t, int h, int wd, int kt, int kh, int kw, int pad_t, int pad_h, int pad_w, int act,
+                              float alpha, float gain, float clamp, void* workspace, int64_t workspace_bytes, void* stream);
+
+/*
  * Layers of a super-res discriminator block (discriminator_sres.py DiscriminatorBlock, architecture 'resnet'; DESIGN.md 7i).
  *
  * lvg_sres_dblock_conv1: conv1, y = bias_act(conv2d(upfirdn2d(x, f, padding 2), w, stride 2), bias, act, alpha, gain,

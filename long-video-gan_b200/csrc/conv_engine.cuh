@@ -52,6 +52,15 @@ struct Geometry {
 };
 Geometry geometry(int split, int64_t inst, int groups, int ck, int cm, int64_t thw, int taps);
 
+// bias_act's gradient rule applied while a gradient dy is re-tiled: dy * G(y) with G decided from the layer's output y
+// (same layout as dy) as bias_act's grad-1 kernel decides it: slope 1 or alpha (lrelu) by the sign of y, times gain, 0 where
+// y is not inside (-clamp, clamp). act: 1 linear, 2 lrelu (the engine epilogue's codes); y == nullptr: no gate.
+struct ActGate {
+    const void* y;
+    int act;
+    float alpha, gain, clamp;
+};
+
 // One launch of the forward kernel: y = correlation of x with the weights, or the input gradient run as one.
 struct IgemmJob {
     // input operand: x (or, x8_pre != nullptr, its re-tiled X8, which the job then does not read or write), in_scale
@@ -59,6 +68,7 @@ struct IgemmJob {
     const void* x;
     const unsigned char* x8_pre;
     const float* in_scale;
+    ActGate in_gate;             // (input gradients) dy re-tiled as dy * G(y) * in_scale
     int xin_h, xin_w, dil;
     // GEMM shape and padding: ck channels in, cm out, per group
     int dtype, n, groups, ck, cm, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w;
@@ -102,6 +112,7 @@ struct WgradInputs {
     const unsigned char* x8_pre;
     const float* x_scale;
     const float* dy_scale;
+    ActGate dy_gate;             // dy re-tiled as dy * G(y) * dy_scale
 };
 
 // workspace of a weight gradient: [dy8, unless pre-tiled][x8][fp32 partial sums]
@@ -130,9 +141,11 @@ struct Backward {
     unsigned char* rest;
     int64_t rest_bytes;
     unsigned char* x8;           // where the weight gradient re-tiles x: a caller may build X8 there and pass it as x8_pre
+    ActGate gate;                // the gate dy was re-tiled with (the weight gradient applies it too when it re-tiles dy itself)
 };
+// gate != nullptr: both gradients take dy * G(y) (bias_act's gradient) in place of dy, without it being written
 int backward_dgrad(const ConvShape& s, const void* dy, const float* d, const void* w, void* dx, void* workspace, int64_t workspace_bytes,
-                   cudaStream_t st, Backward& b);
+                   cudaStream_t st, Backward& b, const ActGate* gate = nullptr);
 int backward_wgrad(const ConvShape& s, const Backward& b, const void* x, const void* dy, const float* d, void* dw, const float* x_scale,
                    const unsigned char* x8_pre, cudaStream_t st);
 

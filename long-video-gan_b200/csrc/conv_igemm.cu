@@ -126,11 +126,21 @@ struct IgemmParams {
 // the oh x ow output image, which the caller has zeroed.
 // `scale` (modulated convolutions): every element is multiplied by scale[instance][channel][frame] in fp32 before it is
 // rounded to fp16 / split into bf16 halves; nullptr = the elements are copied as they are.
-struct PackGeom { int64_t thw_in, thw_out; int ih, iw, oh, ow, dil; const float* scale; };
+// GATE (gradients of a layer with bias_act in its epilogue): x is the gradient dy of the layer's output `gy` (same layout,
+// stride 1), and every element is first multiplied by G(gy), bias_act's gradient rule (ActGate), in fp32.
+struct PackGeom { int64_t thw_in, thw_out; int ih, iw, oh, ow, dil; const float* scale; const void* gy; int act; float alpha, gain, inv_gain, clamp; };
 
-template <class TIn, bool SPLIT, bool SCALE>
-__global__ void __launch_bounds__(256) conv_pack_act_kernel(const TIn* __restrict__ x, uint4* __restrict__ y, int64_t inst, int c,
-                                                             int cblk, PackGeom gm)
+// dy * G(y) as bias_act_elem (bias_act.cu) computes it for grad 1: (dy or dy * alpha by the sign of y / gain) * gain, 0
+// where the forward clamped
+__device__ __forceinline__ float act_gate(float dy, float yv, const PackGeom& gm)
+{
+    float v = (gm.act == 2 && !(yv * gm.inv_gain > 0.f)) ? dy * gm.alpha : dy;
+    v *= gm.gain;
+    return (gm.clamp >= 0.f && !(yv > -gm.clamp && yv < gm.clamp)) ? 0.f : v;
+}
+
+template <class TIn, bool SPLIT, bool SCALE, bool GATE>
+__device__ __forceinline__ void pack_act_grid(const TIn* __restrict__ x, uint4* __restrict__ y, int64_t inst, int c, int cblk, const PackGeom& gm)
 {
     const int64_t thw = gm.thw_in;
     const int64_t total = inst * cblk * thw;
@@ -161,7 +171,14 @@ __global__ void __launch_bounds__(256) conv_pack_act_kernel(const TIn* __restric
             alignas(16) unsigned short v[8];
 #pragma unroll
             for (int j = 0; j < 8; j++) v[j] = (c0 + j < c) ? __half_as_ushort(__ldg(reinterpret_cast<const __half*>(src) + (int64_t)j * thw)) : (unsigned short)0;
-            if constexpr (SCALE) {
+            if constexpr (GATE) {
+                const __half* gy = reinterpret_cast<const __half*>(gm.gy) + ((int64_t)in * c + c0) * thw + p;
+#pragma unroll
+                for (int j = 0; j < 8; j++)
+                    if (c0 + j < c)
+                        v[j] = __half_as_ushort(__float2half_rn(act_gate(__half2float(__ushort_as_half(v[j])), __half2float(__ldg(gy + (int64_t)j * thw)), gm)
+                                                                * __ldg(sc + j * frames)));
+            } else if constexpr (SCALE) {
 #pragma unroll
                 for (int j = 0; j < 8; j++)
                     if (c0 + j < c) v[j] = __half_as_ushort(__float2half_rn(__half2float(__ushort_as_half(v[j])) * __ldg(sc + j * frames)));
@@ -172,7 +189,12 @@ __global__ void __launch_bounds__(256) conv_pack_act_kernel(const TIn* __restric
 #pragma unroll
             for (int j = 0; j < 8; j++) {
                 float f = (c0 + j < c) ? __ldg(reinterpret_cast<const float*>(src) + (int64_t)j * thw) : 0.f;
-                if constexpr (SCALE) { if (c0 + j < c) f *= __ldg(sc + j * frames); }
+                if constexpr (GATE) {
+                    if (c0 + j < c)
+                        f = act_gate(f, __ldg(reinterpret_cast<const float*>(gm.gy) + ((int64_t)in * c + c0 + j) * thw + p), gm) * __ldg(sc + j * frames);
+                } else if constexpr (SCALE) {
+                    if (c0 + j < c) f *= __ldg(sc + j * frames);
+                }
                 hi[j] = bf16_bits(f);
                 lo[j] = bf16_bits(f - bf16_val(hi[j]));
             }
@@ -182,20 +204,44 @@ __global__ void __launch_bounds__(256) conv_pack_act_kernel(const TIn* __restric
     }
 }
 
-// launches the re-tiling of one activation tensor (zeroing the target first when it is dilated)
-int pack_act(const void* x, void* x8, int split, int64_t inst, int c, int cblk, int t, int ih, int iw, int oh, int ow, int dil, cudaStream_t s,
-             const float* scale = nullptr)
+template <class TIn, bool SPLIT, bool SCALE>
+__global__ void __launch_bounds__(256) conv_pack_act_kernel(const TIn* __restrict__ x, uint4* __restrict__ y, int64_t inst, int c,
+                                                             int cblk, PackGeom gm)
 {
-    PackGeom gm;
+    pack_act_grid<TIn, SPLIT, SCALE, false>(x, y, inst, c, cblk, gm);
+}
+
+// the re-tiling of a gradient dy times bias_act's gradient rule G(gy) and the factor
+template <class TIn, bool SPLIT>
+__global__ void __launch_bounds__(256) conv_pack_grad_kernel(const TIn* __restrict__ x, uint4* __restrict__ y, int64_t inst, int c,
+                                                              int cblk, PackGeom gm)
+{
+    pack_act_grid<TIn, SPLIT, true, true>(x, y, inst, c, cblk, gm);
+}
+
+// launches the re-tiling of one activation tensor (zeroing the target first when it is dilated)
+// (gate: the scaled re-tiling of a gradient times bias_act's gradient rule; it needs a scale and unit dilation)
+int pack_act(const void* x, void* x8, int split, int64_t inst, int c, int cblk, int t, int ih, int iw, int oh, int ow, int dil, cudaStream_t s,
+             const float* scale = nullptr, const ActGate* gate = nullptr)
+{
+    PackGeom gm = {};
     gm.thw_in = (int64_t)t * ih * iw; gm.thw_out = (int64_t)t * oh * ow; gm.ih = ih; gm.iw = iw; gm.oh = oh; gm.ow = ow; gm.dil = dil;
     gm.scale = scale;
+    const bool gated = gate != nullptr && gate->y != nullptr;
+    if (gated) {
+        LVG_REQUIRE(scale != nullptr && dil == 1 && (gate->act == 1 || gate->act == 2), "convnd: a gated re-tiling needs a scale, unit stride and linear / lrelu");
+        gm.gy = gate->y; gm.act = gate->act; gm.alpha = gate->alpha; gm.gain = gate->gain; gm.clamp = gate->clamp;
+        gm.inv_gain = gate->gain != 0.f ? 1.f / gate->gain : 0.f;
+    }
     if (dil > 1) LVG_CUDA(cudaMemsetAsync(x8, 0, (size_t)(inst * (split ? 2 : 1) * cblk * gm.thw_out * 16), s));
     const int64_t total = inst * cblk * gm.thw_in;
     int64_t blocks = (total + 255) / 256;
     const int64_t cap = (int64_t)num_sms() * 64;
     if (blocks > cap) blocks = cap;
     // (the scaled variants are separate instantiations: the unscaled re-tiling stays the plain copy it was)
-    if (split && scale) conv_pack_act_kernel<float, true, true><<<(unsigned)blocks, 256, 0, s>>>((const float*)x, (uint4*)x8, inst, c, cblk, gm);
+    if (gated && split) conv_pack_grad_kernel<float, true><<<(unsigned)blocks, 256, 0, s>>>((const float*)x, (uint4*)x8, inst, c, cblk, gm);
+    else if (gated) conv_pack_grad_kernel<__half, false><<<(unsigned)blocks, 256, 0, s>>>((const __half*)x, (uint4*)x8, inst, c, cblk, gm);
+    else if (split && scale) conv_pack_act_kernel<float, true, true><<<(unsigned)blocks, 256, 0, s>>>((const float*)x, (uint4*)x8, inst, c, cblk, gm);
     else if (split) conv_pack_act_kernel<float, true, false><<<(unsigned)blocks, 256, 0, s>>>((const float*)x, (uint4*)x8, inst, c, cblk, gm);
     else if (scale) conv_pack_act_kernel<__half, false, true><<<(unsigned)blocks, 256, 0, s>>>((const __half*)x, (uint4*)x8, inst, c, cblk, gm);
     else conv_pack_act_kernel<__half, false, false><<<(unsigned)blocks, 256, 0, s>>>((const __half*)x, (uint4*)x8, inst, c, cblk, gm);
@@ -819,7 +865,7 @@ int run_igemm(const IgemmJob& j, void* workspace, int64_t workspace_bytes, cudaS
 
     // re-tile the operands
     {
-        const int rc = j.x8_pre ? LVG_OK : pack_act(j.x, x8, split, inst, j.ck, g.cblk, j.t, j.xin_h, j.xin_w, j.h, j.wd, j.dil, s, j.in_scale);
+        const int rc = j.x8_pre ? LVG_OK : pack_act(j.x, x8, split, inst, j.ck, g.cblk, j.t, j.xin_h, j.xin_w, j.h, j.wd, j.dil, s, j.in_scale, &j.in_gate);
         if (rc) return rc;
         const int64_t wblocks = (int64_t)j.groups * g.mt * g.kc;
         LVG_REQUIRE(wblocks < (1ll << 31), "convnd: too many weight tiles");
@@ -1273,7 +1319,8 @@ int run_wgrad(const ConvShape& sh, const void* x, const void* dy, void* dw, cons
     const int64_t thw_a = (int64_t)to * ho * wo, thw_b = sh.thw();
     {
         // dy of a strided convolution is spread over every stride-th pixel of the stride-1 output grid (zeros between)
-        int rc = in.dy8_pre ? LVG_OK : pack_act(dy, dy8, q.split, inst, sh.cout, q.cpad_a / 8, to, sh.hos(), sh.wos(), ho, wo, sh.stride, s, in.dy_scale);
+        int rc = in.dy8_pre ? LVG_OK : pack_act(dy, dy8, q.split, inst, sh.cout, q.cpad_a / 8, to, sh.hos(), sh.wos(), ho, wo, sh.stride, s, in.dy_scale,
+                                                &in.dy_gate);
         if (rc) return rc;
         rc = in.x8_pre ? LVG_OK : pack_act(x, x8, q.split, inst, sh.cin, q.cpad_b / 8, sh.t, sh.h, sh.wd, sh.h, sh.wd, 1, s, in.x_scale);
         if (rc) return rc;
@@ -1345,7 +1392,7 @@ int64_t backward_workspace(const ConvShape& s)
 }
 
 int backward_dgrad(const ConvShape& s, const void* dy, const float* d, const void* w, void* dx, void* workspace, int64_t workspace_bytes,
-                   cudaStream_t st, Backward& b)
+                   cudaStream_t st, Backward& b, const ActGate* gate)
 {
     const bool shared = shares_dy8(s);
     const BackwardRooms r = backward_rooms(s, shared);
@@ -1355,13 +1402,16 @@ int backward_dgrad(const ConvShape& s, const void* dy, const float* d, const voi
     b.rest = ws + r.dy8;
     b.rest_bytes = workspace_bytes - r.dy8;
     b.x8 = b.rest + r.x8;
+    b.gate = gate ? *gate : ActGate{};
     IgemmJob j = dgrad_job(s, dy, w, dx);
     if (shared) {
-        const int rc = pack_act(dy, ws, s.split(), s.inst(), s.cout, job_geometry(j).cblk, s.to(), s.hos(), s.wos(), s.ho(), s.wo(), s.stride, st, d);
+        const int rc = pack_act(dy, ws, s.split(), s.inst(), s.cout, job_geometry(j).cblk, s.to(), s.hos(), s.wos(), s.ho(), s.wo(), s.stride, st, d,
+                                &b.gate);
         if (rc) return rc;
         j.x8_pre = ws;
     } else {
         j.in_scale = d;
+        j.in_gate = b.gate;
     }
     // (stream order: the weight gradient's re-tiling of x overwrites the packed weights only after the input gradient read them)
     return run_igemm(j, b.rest, b.rest_bytes, st);
@@ -1370,7 +1420,7 @@ int backward_dgrad(const ConvShape& s, const void* dy, const float* d, const voi
 int backward_wgrad(const ConvShape& s, const Backward& b, const void* x, const void* dy, const float* d, void* dw, const float* x_scale,
                    const unsigned char* x8_pre, cudaStream_t st)
 {
-    const WgradInputs in = {b.dy8, x8_pre, x_scale, b.dy8 ? nullptr : d};
+    const WgradInputs in = {b.dy8, x8_pre, x_scale, b.dy8 ? nullptr : d, b.dy8 ? ActGate{} : b.gate};
     return run_wgrad(s, x, dy, dw, in, b.rest, b.rest_bytes, st);
 }
 

@@ -107,6 +107,9 @@ _SIGNATURES = {
     'lvg_lres_torgb_fprop': (_c_int, [_c_void_p] * 7 + [_c_int] * 8 + [_c_float, _c_void_p, _c_i64, _c_void_p]),
     'lvg_lres_torgb_finish': (_c_int, [_c_void_p] * 4 + [_c_int] * 5 + [_c_float, _c_void_p]),
     'lvg_lres_torgb_backward': (_c_int, [_c_void_p] * 9 + [_c_int] * 8 + [_c_float, _c_void_p, _c_i64, _c_void_p]),
+    'lvg_gblock_conv0_workspace': (_c_i64, [_c_int] * 13),
+    'lvg_gblock_conv0_fprop': (_c_int, [_c_void_p] * 7 + [_c_int] * 14 + [_c_float] * 3 + [_c_void_p, _c_i64, _c_void_p]),
+    'lvg_gblock_conv0_backward': (_c_int, [_c_void_p] * 12 + [_c_int] * 14 + [_c_float] * 3 + [_c_void_p, _c_i64, _c_void_p]),
     'lvg_sres_dblock_conv1_workspace': (_c_i64, [_c_int] * 6),
     'lvg_sres_dblock_conv1': (_c_int, [_c_void_p] * 3 + [_c_int] + [_c_void_p] * 3 + [_c_int] * 7 + [_c_float] * 3 + [_c_void_p, _c_i64, _c_void_p]),
     'lvg_sres_dblock_conv1_backward_workspace': (_c_i64, [_c_int] * 6),
@@ -222,8 +225,8 @@ _ws = {}
 
 def _workspace(device, need):
     """The convolution engine's workspace on ``device``: one buffer of at least ``need`` bytes (and 4 MiB), grown on
-    demand and shared by every ConvNdPlugin and SresDblockPlugin call, the SresCondPlugin layer calls and the LresTorgbPlugin calls
-    that need one."""
+    demand and shared by every ConvNdPlugin, SresDblockPlugin and GblockConv0Plugin call, the SresCondPlugin layer calls and the
+    LresTorgbPlugin calls that need one."""
     if need < 0:
         raise RuntimeError('convnd: configuration outside the tensor-core kernel envelope')
     buf = _ws.get(device)
@@ -1232,6 +1235,70 @@ class LresTorgbPlugin:
         return dx, dw, da, db
 
 
+class GblockConv0Plugin:
+    """The first modulated convolution of the low-res generator's residual block with its bias_act (DESIGN.md 7m; no
+    reference plugin: Synthesis3dResBlock.forward composes temporal_modulated_conv3d, bias_act and MagnitudeEMA,
+    generator_lres.py:568-575). x [N, Cin, T, H, W] fp16 / fp32, w [Cout, Cin, kt, kh, kw] in x's dtype, a fp32 [N, Cin, T],
+    d fp32 [N, Cout, T], b fp32 [Cout] or None; act 1 linear, 2 lrelu."""
+
+    def __init__(self, lib):
+        self._lib = lib
+
+    def workspace(self, dtype, n, cin, cout, t, h, w, kernel, padding):
+        """Workspace bytes of lvg_gblock_conv0_fprop / _backward, or -1 where the op does not take the call."""
+        return int(self._lib.lvg_gblock_conv0_workspace(_DTYPE_CODE.get(dtype, -1), n, cin, cout, t, h, w, *(int(k) for k in kernel),
+                                                        *(int(p) for p in padding)))
+
+    def _args(self, x, w, a, d, b, padding):
+        """Checked, dense arguments shared by both entry points, and the workspace the call needs."""
+        if not x.is_cuda or x.dtype not in (torch.float16, torch.float32) or x.ndim != 5:
+            raise RuntimeError('gblock_conv0: x must be a 5-D float16 / float32 CUDA tensor')
+        n, cin, t, h, wd = x.shape
+        if w.dtype != x.dtype or w.ndim != 5 or w.shape[1] != cin or w.device != x.device:
+            raise RuntimeError(f'gblock_conv0: w must be a {x.dtype} [Cout, {cin}, kt, kh, kw] tensor on the device of x')
+        cout = int(w.shape[0])
+        for name, f, shape in (('a', a, (n, cin, t)), ('d', d, (n, cout, t))):
+            if f is None or f.dtype != torch.float32 or tuple(f.shape) != shape or f.device != x.device:
+                raise RuntimeError(f'gblock_conv0: {name} must be a float32 {list(shape)} tensor on the device of x')
+        if b is not None and (b.dtype != torch.float32 or tuple(b.shape) != (cout,) or b.device != x.device):
+            raise RuntimeError(f'gblock_conv0: b must be a float32 [{cout}] tensor on the device of x')
+        pad = tuple(int(p) for p in padding)
+        need = self.workspace(x.dtype, n, cin, cout, t, h, wd, w.shape[2:], pad)
+        if need < 0:
+            raise RuntimeError(f'gblock_conv0: no kernel for x {list(x.shape)} ({x.dtype}), w {list(w.shape)}, padding {list(pad)}')
+        dims = (_DTYPE_CODE[x.dtype], n, cin, cout, t, h, wd) + tuple(int(k) for k in w.shape[2:]) + pad
+        return (x.contiguous(), w.contiguous(), a.contiguous(), d.contiguous(), None if b is None else b.contiguous(), dims, need)
+
+    def fprop(self, x, w, a, d, b, padding, act, alpha, gain, clamp, want_sumsq=False):
+        """(y [N, Cout, T, Ho, Wo] in x's dtype = clamp(act(d conv(a x, w) + b) gain), sum of y^2 as stored (0-dim fp32) or
+        None); clamp < 0: none."""
+        x, w, a, d, b, dims, need = self._args(x, w, a, d, b, padding)
+        ho, wo = [s + 2 * p - k + 1 for s, p, k in zip(x.shape[3:], dims[11:], dims[8:10])]
+        y = torch.empty([dims[1], dims[3], dims[4], ho, wo], dtype=x.dtype, device=x.device)
+        sumsq = torch.empty([], dtype=torch.float32, device=x.device) if want_sumsq else None
+        ws = _workspace(x.device, need)
+        _launch('gblock_conv0_fprop', self._lib.lvg_gblock_conv0_fprop, x, _ptr(x), _ptr(w), _ptr(a), _ptr(d), _ptr(b), _ptr(y), _ptr(sumsq),
+                *dims, int(act), float(alpha), float(gain), float(clamp), _ptr(ws), ws.numel())
+        return y, sumsq
+
+    def backward(self, x, w, a, d, b, y, dy, padding, act, alpha, gain, clamp, want_dw=True, want_dd=True, want_db=True):
+        """(dx, dw or None, da fp32 [N, Cin, T], dd fp32 [N, Cout, T] or None, db fp32 [Cout] or None) of fprop's y, with
+        bias_act's gradient decided from y."""
+        x, w, a, d, b, dims, need = self._args(x, w, a, d, b, padding)
+        if y.dtype != x.dtype or dy.dtype != x.dtype or dy.shape != y.shape or y.device != x.device or dy.device != x.device:
+            raise RuntimeError(f'gblock_conv0_backward: y and dy must be {x.dtype} tensors of one shape on the device of x')
+        y, dy = y.contiguous(), dy.contiguous()
+        dx = torch.empty_like(x)
+        dw = torch.empty_like(w) if want_dw else None
+        da = torch.empty_like(a)
+        dd = torch.empty_like(d) if want_dd else None
+        db = torch.empty([dims[3]], dtype=torch.float32, device=x.device) if want_db else None
+        ws = _workspace(x.device, need)
+        _launch('gblock_conv0_backward', self._lib.lvg_gblock_conv0_backward, x, _ptr(x), _ptr(w), _ptr(a), _ptr(d), _ptr(b), _ptr(y), _ptr(dy),
+                _ptr(dx), _ptr(dw), _ptr(da), _ptr(dd), _ptr(db), *dims, int(act), float(alpha), float(gain), float(clamp), _ptr(ws), ws.numel())
+        return dx, dw, da, dd, db
+
+
 class SresDblockPlugin:
     """The two native layers of a super-res discriminator block (DESIGN.md 7i): ``conv1`` (the 4-tap FIR in the
     convolution's re-tiling pass, the stride-2 3x3 convolution with its bias_act epilogue) and ``skip`` (the 1x1 convolution
@@ -1312,6 +1379,7 @@ class SresDblockPlugin:
 
 
 _PLUGIN_CLASSES = {
+    'gblock_conv0_plugin': GblockConv0Plugin,
     'lres_torgb_plugin': LresTorgbPlugin,
     'sres_dblock_plugin': SresDblockPlugin,
     'sres_cond_plugin': SresCondPlugin,

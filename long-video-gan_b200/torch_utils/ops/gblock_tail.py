@@ -180,11 +180,22 @@ def applies(block, input, dtype, out_seq_length):
     return _plugin().workspace(n, block.out_channels, t, h, w, to, ho, wo, flags) >= 0
 
 
-def block_forward(block, g, input, latent, magnitude_ema_beta=1.0, out_seq_length=None, dtype=None):
+def head(block, g, input, style_0, input_gain_0, magnitude_ema_beta):
+    """The block's first layer as the reference computes it: (bias_act(conv_0), the gain input_magnitude_ema_1 takes from
+    it or None)."""
+    hidden = g['temporal_modulated_conv3d'](input, block.weight_0, style_0, input_gain_0, block.padding, demodulate=True)
+    bias_0 = block.bias_0.type(hidden.dtype)
+    hidden = g['bias_act_wrapper'](hidden, bias_0, act=block.activation, clamp=block.activation_clamp)
+    input_gain_1 = block.input_magnitude_ema_1(hidden, magnitude_ema_beta) if block.magnitude_ema else None
+    return hidden, input_gain_1
+
+
+def block_forward(block, g, input, latent, magnitude_ema_beta=1.0, out_seq_length=None, dtype=None, head=head):
     """Synthesis3dResBlock.forward with the tail as ``gblock_tail`` and the block input's magnitude-EMA gain folded into the
     first modulated convolution (``input_gain=``) and the skip weight. ``g``: the globals of the model module (its
     ``misc``, ``einops``, ``temporal_modulated_conv3d`` and ``bias_act_wrapper``, whatever they are patched to). The same
-    MagnitudeEMA calls and affine layers as the reference, in its order."""
+    MagnitudeEMA calls and affine layers as the reference, in its order. ``head``: the block's first layer, called as
+    ``head`` above (``gblock_conv0`` passes its fused one)."""
     misc, einops = g['misc'], g['einops']
     misc.assert_shape(input, (None, block.in_channels, None, None, None))
     batch_size, in_seq_length = input.size(0), input.size(2)
@@ -198,13 +209,10 @@ def block_forward(block, g, input, latent, magnitude_ema_beta=1.0, out_seq_lengt
     input = input.type(dtype)
     input_gain_0 = block.input_magnitude_ema_0(input, magnitude_ema_beta) if block.magnitude_ema else None
 
-    hidden = g['temporal_modulated_conv3d'](input, block.weight_0, style_0, input_gain_0, block.padding, demodulate=True)
-    bias_0 = block.bias_0.type(hidden.dtype)
-    hidden = g['bias_act_wrapper'](hidden, bias_0, act=block.activation, clamp=block.activation_clamp)
+    hidden, input_gain_1 = head(block, g, input, style_0, input_gain_0, magnitude_ema_beta)
 
     style_1 = block.affine_1(latent)
     style_1 = einops.rearrange(style_1, "(n t) c -> n c t", t=in_seq_length)
-    input_gain_1 = block.input_magnitude_ema_1(hidden, magnitude_ema_beta) if block.magnitude_ema else None
     hidden = g['temporal_modulated_conv3d'](hidden, block.weight_1, style_1, input_gain_1, block.padding, demodulate=True)
 
     weight_skip = block.weight_skip * block.weight_skip_gain
@@ -227,7 +235,10 @@ def _forward(orig):
         dt = dtype if dtype is not None else (torch.float16 if self.use_float16 and input.is_cuda else torch.float32)
         if not applies(self, input, dt, out_seq_length):
             return orig(self, input, latent, magnitude_ema_beta, out_seq_length, dtype)
-        return block_forward(self, g, input, latent, magnitude_ema_beta, out_seq_length, dtype)
+        # gblock_conv0.install: its fused first layer, when it takes the call
+        conv0 = _install.find(type(self).forward, 'lvg_gblock_conv0')
+        h = conv0.head_for(self, input, latent, magnitude_ema_beta, dtype) if conv0 is not None else None
+        return block_forward(self, g, input, latent, magnitude_ema_beta, out_seq_length, dtype, head=h or head)
     return forward
 
 

@@ -159,13 +159,9 @@ def modulated_conv2d(x, w, s, demodulate=True, padding=0, input_gain=None):
 
 # ---------------------------------------------------------------------------------------------------- low-res
 
-def temporal_modulated_conv3d(input, weight, style, input_gain=None, padding=(0, 0, 0), demodulate=True):
-    """generator_lres.temporal_modulated_conv3d: input [N, Cin, T, H, W], weight [Cout, Cin, kt, kh, kw], style [N, Cin, T],
-    input_gain a 0-dim tensor or None. Demodulation uses the style of output frame t only (the reference's definition),
-    so the output must have the input's frame count."""
-    assert input.dim() == 5
-    batch_size, in_channels = input.size(0), input.size(1)
-    assert weight.shape[1] == in_channels and tuple(style.shape[:2]) == (batch_size, in_channels)
+def temporal_factors(weight, style, demodulate=True):
+    """(w~ (fp32), the normalised style, d [N, Cout, T] or None) of ``temporal_modulated_conv3d``: its convolution is
+    d * conv(style * input_gain * input, w~.type(input.dtype)) (the same torch ops, so the same autograd graph)."""
     if demodulate:
         weight = weight / weight.abs().amax(dim=(1, 2, 3, 4), keepdim=True)
         style = style / style.abs().amax(dim=(1, 2), keepdim=True)
@@ -173,6 +169,17 @@ def temporal_modulated_conv3d(input, weight, style, input_gain=None, padding=(0,
     demod = None
     if demodulate:
         demod = torch.einsum('oizyx,nit->not', weight.square(), style.square()).add(1e-8).rsqrt()
+    return weight, style, demod
+
+
+def temporal_modulated_conv3d(input, weight, style, input_gain=None, padding=(0, 0, 0), demodulate=True):
+    """generator_lres.temporal_modulated_conv3d: input [N, Cin, T, H, W], weight [Cout, Cin, kt, kh, kw], style [N, Cin, T],
+    input_gain a 0-dim tensor or None. Demodulation uses the style of output frame t only (the reference's definition),
+    so the output must have the input's frame count."""
+    assert input.dim() == 5
+    batch_size, in_channels = input.size(0), input.size(1)
+    assert weight.shape[1] == in_channels and tuple(style.shape[:2]) == (batch_size, in_channels)
+    weight, style, demod = temporal_factors(weight, style, demodulate)
     if input_gain is not None:
         assert input_gain.dim() == 0
     pad = _pad_tuple(padding, 3)
