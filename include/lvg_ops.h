@@ -249,6 +249,13 @@ int lvg_convnd_route(int mode, int dtype, int n, int groups, int cin, int cout, 
 int lvg_convnd_wgrad_plan(int dtype, int n, int groups, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw,
                           int pad_t, int pad_h, int pad_w, int* out, int out_len);
 /*
+ * Introspection: the K steps lvg_convnd_wgrad takes over one stage of `rows` (1..rh) dy rows of column segment `seg`:
+ * out[0] = steps, then per step the pixel offset of its first 8-pixel group and the distance to its second. Host
+ * arithmetic only: tests/test_wgrad_ksteps_emul.py replays them on the CPU.
+ */
+int lvg_convnd_wgrad_ksteps(int dtype, int n, int groups, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw,
+                            int pad_t, int pad_h, int pad_w, int rows, int seg, int* out, int out_len);
+/*
  * Both gradients of one convolution call (what autograd asks of F.conv3d / conv2d_gradfix in a first-order backward pass,
  * conv2d_gradfix.py:118-141): dx as lvg_convnd_dgrad, dw as lvg_convnd_wgrad, with dy re-tiled ONCE for the two kernels
  * (the separate entry points re-tile it once each). Argument list = the FORWARD convolution; `workspace`:

@@ -105,6 +105,37 @@ struct WgradPlan {
 };
 WgradPlan wgrad_plan(const ConvShape& s, bool fold = true);
 
+// The K steps of the weight-gradient kernel over one stage. A stage tile holds `rows` rows of `ps` pixels, and only the
+// first `width` pixels of a row are dy pixels (TMA zero-fills the rest). A wgmma K step reads two 8-pixel groups. The steps
+// take the gw = ceil(width / 8) groups of each row in row order, two at a time, and skip the rest of the pitch. An odd
+// last group is paired with the 8 zero-filled pixels right after it. Every read stays inside the first
+// ceil(rows * ps / 16) * 16 pixels of the tile. x is read at the same offsets plus the tap shift (equal pitches).
+struct WgradKWalk {
+    int gw, skip, left;          // groups per row, pitch pixels past a row's last group, groups not yet taken
+    int c;                       // group of the next step within its row
+    uint32_t off;                // pixel offset of the next step's first group
+};
+__host__ __device__ __forceinline__ WgradKWalk wgrad_kwalk(int rows, int width, int ps)
+{
+    const int gw = (width + 7) / 8;
+    return {gw, ps - 8 * gw, rows * gw, 0, 0u};
+}
+__host__ __device__ __forceinline__ int wgrad_ksteps(const WgradKWalk& w) { return (w.left + 1) / 2; }
+// The next K step as (offset of its first group) | (distance to its second group) << 16, in pixels of 16 bytes: added to
+// the low word of an MN-major wgmma descriptor with start address `tile` and leading byte offset 0, it gives the start
+// address and the K-direction group stride of the step.
+__host__ __device__ __forceinline__ uint32_t wgrad_kstep(WgradKWalk& w)
+{
+    const uint32_t first = w.off;
+    w.off += 8;
+    if (++w.c == w.gw) { w.c = 0; w.off += (uint32_t)w.skip; }
+    const uint32_t second = w.left == 1 ? first + 8u : w.off;
+    w.off += 8;
+    if (++w.c == w.gw) { w.c = 0; w.off += (uint32_t)w.skip; }
+    w.left -= 2;
+    return first | (second - first) << 16;
+}
+
 // what a weight-gradient call takes in place of re-tiling its operands: dy8_pre / x8_pre (then dy / x are not read), or
 // the factors the re-tiling applies: x_scale [n][cin][t], dy_scale [n][cout][to]
 struct WgradInputs {

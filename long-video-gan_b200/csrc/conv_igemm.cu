@@ -991,7 +991,9 @@ extern "C" int lvg_convnd_dgrad(const void* dy, const void* w, void* dx, int dty
 // PS = (segment width + kw - 1) rounded up to 16. The dy tile is loaded through a tensor map whose W extent is clipped to
 // the column segment, so TMA zero-fills its last PS - width columns -- those are the K positions where the x tile holds
 // the row's halo; with equal pitches on both sides a tap (kx) is a start-address shift of kx * 16 bytes and the tap row
-// (kt, ky) a shifted TMA box. One MMA covers 16 consecutive pixels of the linear index.
+// (kt, ky) a shifted TMA box. One MMA covers two 8-pixel groups of the linear index, and the K steps take only the groups
+// that hold dy pixels (wgrad_kstep): the zero-filled PS - width columns of a row cost no MMA beyond an odd last group's
+// partner.
 // Few groups (discriminators, low-res networks): the stages are cut into `nsplit` ranges over the grid, fp32 partial
 // sums go to a workspace and conv_wgrad_reduce_kernel folds them. fp32 tensors: hi/lo bf16 halves of BOTH operands are
 // staged, three MMAs per k-step (hi*hi + lo*hi + hi*lo).
@@ -1097,7 +1099,8 @@ __global__ void __launch_bounds__(kIgemmThreads, 1) conv_wgrad_v2_kernel(const _
             const int seg = (s / rblocks) % p.nseg;
             const int rb = s % rblocks;
             const int rows = min(p.rh, p.ho - rb * p.rh);
-            const int ksteps = (rows * p.ps[seg] + 15) / 16;                 // (a trailing half step reads the zero-filled next row)
+            const int width = p.seg_w[seg];
+            const int ksteps = wgrad_ksteps(wgrad_kwalk(rows, width, p.ps[seg]));
             const uint32_t blk_a = (uint32_t)(p.rh * p.ps[seg] * 16);                    // bytes of one channel block of the dy tile
             const uint32_t blk_b = (uint32_t)((p.rh + p.khc - 1) * p.ps[seg] * 16);      // ... of the x tile (kh - 1 halo rows when folded)
             const uint32_t ky16 = (uint32_t)p.ps[seg];                                   // one tap row down = one tile row further (>> 4)
@@ -1105,19 +1108,27 @@ __global__ void __launch_bounds__(kIgemmThreads, 1) conv_wgrad_v2_kernel(const _
             wgmma_fence();
             const uint32_t a0 = smem_u32(smem + (size_t)slot * p.stage_bytes) + (uint32_t)cw * 8u * blk_a;
             const uint32_t b0 = smem_u32(smem + (size_t)slot * p.stage_bytes) + (uint32_t)(nop * p.a_bytes);
-            // descriptors as (lo, hi) words: a K step is +16 on the low word (256 bytes >> 4), a tap column +1, a tap row
-            // + ps; the stride byte offset of the x tile (one channel block) spans the NT / 8 blocks of the n-tile
+            // descriptors as (lo, hi) words: a K step adds its group offset and group stride to the low word (both in
+            // 16-byte pixels, wgrad_kstep), a tap column +1, a tap row + ps; the stride byte offset of the x tile (one
+            // channel block) spans the NT / 8 blocks of the n-tile
             const uint32_t a_hi = desc_hi(blk_a), b_hi = desc_hi(blk_b);
             for (int term = 0; term < (p.split ? 3 : 1); term++) {
-                const uint32_t a_lo0 = desc_lo(a0 + (term == 1 ? (uint32_t)p.a_bytes : 0u), 128);     // hi*hi, lo*hi, hi*lo
-                const uint32_t b_lo0 = desc_lo(b0 + (term == 2 ? (uint32_t)p.b_bytes : 0u), 128);
-                for (int k = 0; k < ksteps; k++) {
+                const uint32_t a_lo0 = desc_lo(a0 + (term == 1 ? (uint32_t)p.a_bytes : 0u), 0);     // hi*hi, lo*hi, hi*lo
+                const uint32_t b_lo0 = desc_lo(b0 + (term == 2 ? (uint32_t)p.b_bytes : 0u), 0);
+                WgradKWalk walk = wgrad_kwalk(rows, width, p.ps[seg]);
+                auto mma_step = [&](uint32_t step) {
 #pragma unroll
                     for (int tap = 0; tap < TAPS; tap++) {
                         const int kyi = tap / p.kw, kx = tap - kyi * p.kw;
-                        wgmma_m64nNk16<BF16, NT, 1, 1>(acc[tap], a_lo0 + 16u * k, a_hi, b_lo0 + 16u * k + (uint32_t)kyi * ky16 + (uint32_t)kx, b_hi);
+                        wgmma_m64nNk16<BF16, NT, 1, 1>(acc[tap], a_lo0 + step, a_hi, b_lo0 + step + (uint32_t)kyi * ky16 + (uint32_t)kx, b_hi);
                     }
-                }
+                };
+                // rows without padding groups (skip 0: 1x1 layers, wide rows) walk the tile linearly -- the same steps
+                // without the walk's bookkeeping between the MMAs
+                if (walk.skip == 0)
+                    for (int k = 0; k < ksteps; k++) mma_step(16u * k | 8u << 16);
+                else
+                    for (int k = 0; k < ksteps; k++) mma_step(wgrad_kstep(walk));
             }
             wgmma_commit();
             wgmma_wait<1>();                              // the group of the previous stage has completed: release its slot
@@ -1526,6 +1537,30 @@ extern "C" int lvg_convnd_wgrad_plan(int dtype, int n, int groups, int cin, int 
                        q.stage_bytes, q.tail_bytes, (int)q.smem, q.seg_w[0], q.seg_w[1], q.seg_w[2], q.seg_w[3], q.seg_x0[0], q.seg_x0[1], q.seg_x0[2],
                        q.seg_x0[3], 0, q.mrows, 0, 0, 0, 0};
     for (int i = 0; i < 32; i++) out[i] = v[i];
+    return LVG_OK;
+}
+
+// the K steps conv_wgrad_v2_kernel takes over a stage of `rows` dy rows of column segment `seg` (host arithmetic only, the
+// kernel's own wgrad_kstep; tests/test_wgrad_ksteps_emul.py replays them on the CPU)
+extern "C" int lvg_convnd_wgrad_ksteps(int dtype, int n, int groups, int cin, int cout, int t, int h, int wd, int kt, int kh, int kw, int pad_t,
+                                       int pad_h, int pad_w, int rows, int seg, int* out, int out_len)
+{
+    const ConvShape sh = {dtype, n, groups, cin, cout, t, h, wd, kt, kh, kw, pad_t, pad_h, pad_w, 1};
+    if (!sh.wgrad_ok()) {
+        set_error("convnd_wgrad_ksteps: outside the tensor-core kernel's envelope");
+        return LVG_UNSUPPORTED;
+    }
+    const WgradPlan q = wgrad_plan(sh);
+    LVG_REQUIRE(rows >= 1 && rows <= q.rh && seg >= 0 && seg < q.nseg, "convnd_wgrad_ksteps: rows in [1, %d], seg in [0, %d)", q.rh, q.nseg);
+    WgradKWalk w = wgrad_kwalk(rows, q.seg_w[seg], q.ps);
+    const int steps = wgrad_ksteps(w);
+    LVG_REQUIRE(out && out_len >= 1 + 2 * steps, "convnd_wgrad_ksteps: out must hold %d ints", 1 + 2 * steps);
+    out[0] = steps;
+    for (int k = 0; k < steps; k++) {
+        const uint32_t step = wgrad_kstep(w);
+        out[1 + 2 * k] = (int)(step & 0xffffu);
+        out[2 + 2 * k] = (int)(step >> 16);
+    }
     return LVG_OK;
 }
 

@@ -71,6 +71,7 @@ _SIGNATURES = {
     'lvg_convnd_plan': (_c_int, [_c_int] * 16 + [ctypes.POINTER(_c_int), _c_int]),
     'lvg_convnd_epilogue_plan': (_c_int, [_c_int] * 16 + [ctypes.POINTER(_c_int), _c_int]),
     'lvg_convnd_wgrad_plan': (_c_int, [_c_int] * 14 + [ctypes.POINTER(_c_int), _c_int]),
+    'lvg_convnd_wgrad_ksteps': (_c_int, [_c_int] * 16 + [ctypes.POINTER(_c_int), _c_int]),
     'lvg_convnd_route': (_c_int, [_c_int] * 17),
     'lvg_convnd_backward_workspace': (_c_i64, [_c_int] * 14),
     'lvg_convnd_backward': (_c_int, [_c_void_p] * 5 + [_c_int] * 15 + [_c_void_p, _c_i64, _c_void_p]),
